@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — rays/sec and grid-voxels/sec of the NeRF render / mesh hot path on N B200s (BASELINE.json metric).
+"""bench.py — rays/sec and grid-voxels/sec of the NeRF render / mesh hot path on N H100s (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
-                    [--workload lego|fern|buff|mesh] [--shard auto|replica|rows] [--only]
+                    [--workload lego|fern|buff|mesh] [--shard auto|replica|rows] [--only] [--dump-outputs DIR]
 
 Workloads (BASELINE.json configs[1..4], SURVEY 8d; weights of the reference's shipped checkpoints re-packed under
 tests/golden/, synthetic poses, no dataset or network needed):
@@ -22,7 +22,7 @@ N > 1 (torchrun, one process per GPU), --shard rows (the default, `auto`): ONE i
   (weak scaling, no collective).
   value     whole-job rays/s (voxels/s), inputs resident (pose only), CUDA-event timed, max over ranks
   e2e       the same through host buffers: ray directions H2D from pinned memory, render, [all_gather,] D2H of rgb+disp
-  roofline  the fused-MLP kernel against the measured bf16 tensor peak (algorithmic FLOPs: 1,186,816 per point)
+  roofline  the fused-MLP kernel against the H100 SXM data-sheet dense bf16 peak (algorithmic FLOPs: 1,186,816 per point)
   cpu_baseline / --impl reference: the oracle port (torch-CPU restatement of the reference: the same ATen kernels the
             reference itself runs, in the same order) on the host cores, bounded sample of the same workload
 """
@@ -109,7 +109,7 @@ WORKLOADS = {
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons (and the power limit) during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,"
          "power.limit")
@@ -145,12 +145,10 @@ class ClockSampler:
                 "power_capped_frac": (sum(capped) / len(capped)) if capped else None, "samples": len(sm)}
 
 
-def measured_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1407.1), d.get("hbm_gbs", 6564.5), "measured (MEASURED_PEAKS.json: sustained bf16, copy GB/s)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+def peaks():
+    """NVIDIA's H100 SXM data sheet (a 700 W card): dense bf16 TFLOP/s and HBM3 GB/s.  A card set to a lower power limit
+    (the JSON line's clocks.power_limit_w) reaches less."""
+    return 989.0, 3350.0, "H100 SXM data sheet (dense bf16, HBM3), not measured"
 
 
 # ---------------------------------------------------------------------------------------------------- CPU arm (oracle port)
@@ -296,7 +294,7 @@ def make_model(nm, name, ctx, precision):
     return model, eng
 
 
-def run_render(nm, name, ctx, steps, warmup, precision, with_e2e, clocks=None):
+def run_render(nm, name, ctx, steps, warmup, precision, with_e2e, clocks=None, keep_outputs=False):
     """Device-resident (pose in, maps out) timing of one render workload, optionally followed by the host-buffer arm."""
     from nerfmeshes_b200 import parallel as par
     wl = WORKLOADS[name]
@@ -332,7 +330,7 @@ def run_render(nm, name, ctx, steps, warmup, precision, with_e2e, clocks=None):
     finite = bool(torch.isfinite(out["rgb"]).all())
     images = steps * (1 if rows else ctx.world)
     res = dict(dev_ms=dev_ms, launches=int(launches), mlp_ms=mlp_ms, mlp_pts=mlp_pts, mlp_n=mlp_n, clk=clk, finite=finite,
-               rays=H * W * images)
+               rays=H * W * images, outputs={k: out[k].float().cpu() for k in want} if keep_outputs else None)
 
     if wl["buff"]:          # the AABB sampler alone (a10): warp per ray x 1533 voxels + two bitonic sorts
         o_d, d_d = eng.ray_bundle(pose_of(0), H, W, focal)
@@ -395,7 +393,7 @@ def run_render(nm, name, ctx, steps, warmup, precision, with_e2e, clocks=None):
     return res
 
 
-def run_mesh(nm, ctx, steps, warmup, precision):
+def run_mesh(nm, ctx, steps, warmup, precision, keep_outputs=False):
     """512^3 sigma sweep -> adaptive iso -> marching cubes [-> all_gather of the slab meshes]; everything inside the timed
     region, x-slabs across ranks.  Returns per-stage times (max over ranks is taken by the caller)."""
     from nerfmeshes_b200 import parallel as par
@@ -420,10 +418,30 @@ def run_mesh(nm, ctx, steps, warmup, precision):
     e1.record()
     ctx.barrier()
     res = dict(total_ms=e0.elapsed_time(e1) / steps, launches=(eng.launch_count() - l0) // steps, n_vertices=int(v.shape[0]),
-               n_triangles=int(f.shape[0]), iso=float(iso), **{k: acc[k] / steps for k in keys})
+               n_triangles=int(f.shape[0]), iso=float(iso), **{k: acc[k] / steps for k in keys},
+               outputs=mesh_sample(v, f, n, float(iso)) if keep_outputs else None)
     del model, eng, v, f, n
     torch.cuda.empty_cache()
     return res
+
+
+def mesh_sample(v, f, n, iso, cap=1 << 20):
+    """The last step's mesh as float arrays: vertices, normals and faces (float64 indices), each a fixed seeded sample of at
+    most `cap` rows (the same rows for the same mesh size), and the iso level."""
+    def rows(x):
+        if x.shape[0] <= cap:
+            return x
+        idx = torch.randperm(x.shape[0], generator=torch.Generator().manual_seed(0))[:cap].sort().values
+        return x[idx.to(x.device)]
+    return {"vertices": rows(v).float().cpu(), "normals": rows(n).float().cpu(), "faces": rows(f).double().cpu(),
+            "iso": torch.tensor([iso], dtype=torch.float64)}
+
+
+def dump_outputs(d, outputs):
+    os.makedirs(d, exist_ok=True)
+    for k, x in outputs.items():
+        x = x.numpy()
+        np.save(os.path.join(d, f"{k}.npy"), x if x.dtype in (np.float32, np.float64) else x.astype(np.float32))
 
 
 def run_train(nm, ctx, precision):
@@ -482,6 +500,9 @@ def main():
     ap.add_argument("--precision", default="exact", choices=["exact", "fast", "fp32"])
     ap.add_argument("--cpu-steps", type=int, default=6)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the primary workload's last timed step computed as DIR/<name>.npy (rank 0: with --shard "
+                         "rows the gathered full image / mesh, with --shard replica rank 0's own image)")
     a = ap.parse_args()
     ctx = Ctx(a)
     prim = a.workload
@@ -495,7 +516,7 @@ def main():
         par_s = f"image-parallel x{ctx.world} (independent poses per rank, no collective)" if not is_mesh else "single GPU"
     config = {"workload": label, "shard": ctx.shard, "parallelism": par_s,
               "weights": "the reference's shipped checkpoints re-packed (tests/golden/weights_*.npz)",
-              "l2": "per-step working set (GBs of per-sample arrays / a 537 MB grid) >> 126 MB L2; no explicit flush needed"}
+              "l2": "per-step working set (GBs of per-sample arrays / a 537 MB grid) >> 50 MB L2; no explicit flush needed"}
     if not is_mesh:
         config.update({"rays_per_step": WORKLOADS[prim]["H"] * WORKLOADS[prim]["W"] * (1 if ctx.shard == "rows" else ctx.world),
                        "poses": WORKLOADS[prim]["poses"]})
@@ -517,7 +538,7 @@ def main():
 
     import nerfmeshes_b200 as nm
     ctx.init()
-    peak_tf, peak_gbs, peak_src = measured_peaks()
+    peak_tf, peak_gbs, peak_src = peaks()
     clocks = ClockSampler(ctx.local) if ctx.rank == 0 else None
     sec_steps = max(1, min(a.steps, 3))
     result = {"metric": metric, "unit": unit, "n_gpus": ctx.world, "steps": a.steps, "warmup": a.warmup, "higher_is_better": True,
@@ -545,9 +566,10 @@ def main():
     if is_mesh:
         if clocks:
             clocks.start()
-        m = run_mesh(nm, ctx, a.steps, a.warmup, a.precision)
+        m = run_mesh(nm, ctx, a.steps, a.warmup, a.precision, keep_outputs=bool(a.dump_outputs) and ctx.rank == 0)
         clk = clocks.stop() if clocks else None
         blk = mesh_block(m, a.steps)
+        outputs = m["outputs"]
         result.update({"value": blk["value"], "ms_per_step": blk["ms_per_step"], "clocks": clk, "gpu_launches": blk["gpu_launches"] * a.steps,
                        "roofline": blk["roofline"], "mesh": blk,
                        "e2e": {"value": blk["value"], "unit": unit, "h2d_bytes_per_step": 3 * MESH_RES * 4,
@@ -555,18 +577,12 @@ def main():
                                "api": "extract_geometry_sharded: the grid is generated on the device from three linspace tables "
                                       "(H2D) and the mesh stays on the device; only counts / statistics cross PCIe"}})
     else:
-        r = run_render(nm, prim, ctx, a.steps, a.warmup, a.precision, with_e2e=True, clocks=clocks)
+        r = run_render(nm, prim, ctx, a.steps, a.warmup, a.precision, with_e2e=True, clocks=clocks,
+                       keep_outputs=bool(a.dump_outputs) and ctx.rank == 0)
         dev_ms, e2e_ms = ctx.max_over_ranks(r["dev_ms"], r["e2e_ms"])
         r["dev_ms"] = dev_ms
         blk = render_block(prim, r, ctx, a.steps, peak_tf, peak_src)
-        traffic = None
-        tp = os.path.join(ROOT, "profiles", "r02_mlp_traffic.json")
-        if os.path.exists(tp) and prim == "lego":
-            traffic = json.load(open(tp)).get("mean_bytes_per_launch")       # ncu dram read+write per MLP launch, full-image launch
-        blk["roofline"]["traffic"] = traffic
-        blk["roofline"]["traffic_note"] = ("mean DRAM bytes per full-image MLP launch (ncu, profiles/r02_mlp_traffic.json): the compositor runs "
-                                           "inside the kernel, so a launch reads t (4 B/sample) and writes the per-ray maps (+ the coarse pass's "
-                                           "weights, 4 B/sample); round 1 wrote raw (R,S,4): 1.62 GB per launch")
+        outputs = r["outputs"]
         result.update({"value": blk["value"], "ms_per_step": blk["ms_per_step"], "clocks": r["clk"], "finite": r["finite"],
                        "gpu_launches": r["launches"], "roofline": blk["roofline"],
                        "e2e": {"value": r["rays"] / (e2e_ms * 1e-3), "unit": unit, "h2d_bytes_per_step": r["h2d"],
@@ -597,6 +613,8 @@ def main():
         if ctx.dist is not None:
             ctx.dist.destroy_process_group()
         return
+    if a.dump_outputs:
+        dump_outputs(a.dump_outputs, outputs)
     if not a.no_cpu_baseline:
         v, cores, sample, _, _, cu = cpu_reference_run(prim, a.cpu_steps, 1)
         result["cpu_baseline"] = {"value": v, "unit": cu, "cores": cores, "kind": "port", "sample": sample}

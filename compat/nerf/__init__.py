@@ -1,4 +1,4 @@
-"""`nerf` namespace of the reference (src/nerf/__init__.py:1-5) for the hot path: compute entry points are the B200
+"""`nerf` namespace of the reference (src/nerf/__init__.py:1-5) for the hot path: compute entry points are the H100
 implementation, the rest is the small host-side glue the scripts import by name."""
 from nerfmeshes_b200.cfgnode import CfgNode  # noqa: F401
 from nerfmeshes_b200.models import FlexibleNeRFModel, OutputBundle, PositionalEncoding, TreeSampling  # noqa: F401

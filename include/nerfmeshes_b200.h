@@ -1,5 +1,5 @@
 /*
- * nerfmeshes_b200 — C ABI of the B200-native NeRF render / dense-grid hot path.
+ * nerfmeshes_b200 — C ABI of the H100-native (sm_90a) NeRF render / dense-grid hot path (the name is historical).
  *
  * The reference (qway/nerfmeshes, pure Python) has no FFI layer; its de-facto operator API for this path
  * is the Python surface SURVEY.md section 8(b) lists.  Each entry point below names the reference interface it
@@ -43,8 +43,8 @@ typedef struct NmNetDesc {
 
 /* MLP arithmetic selection (SURVEY 7.3.1). */
 enum {
-  NM_PREC_EXACT = 0, /* tcgen05, fp16 hi/lo split operands, 3 MMAs per product, fp32 accumulate (default) */
-  NM_PREC_FAST = 1,  /* tcgen05, single fp16 operands (misses the 1e-4 target; for comparison only)      */
+  NM_PREC_EXACT = 0, /* wgmma, fp16 hi/lo split operands, 3 MMAs per product, fp32 accumulate (default) */
+  NM_PREC_FAST = 1,  /* wgmma, single fp16 operands (misses the 1e-4 target; for comparison only)      */
   NM_PREC_FP32 = 2   /* CUDA-core fp32 FMA kernel (bit-for-bit fp32 arithmetic; slow; debugging yard-stick) */
 };
 
@@ -250,12 +250,12 @@ int nm_debug_pack(const NmNetDesc* desc, int n_tensors, const char* const* names
                   const int64_t* numel, int sigma_only, void* program_out, size_t program_cap, uint8_t* pack_out,
                   size_t pack_cap, size_t* pack_need);
 
-/* Host-only: how the fused compositor deals tiles to CTAs for `samples_per_ray` samples (nm_mlp_tc.cu).  Returns the group
- * size g = lcm(S,128)/128 (0: the fused compositor is not used for this S); if tiles_out != NULL it receives the tile
- * indices CTA `cta` of `grid` CTAs processes, in order, for a launch of n_tiles tiles (at most cap entries; *n_out = count). */
+/* Host-only: how the fused compositor deals 64-point tiles to the kernel's workers (two consumer warpgroups per CTA) for
+ * `samples_per_ray` samples (nm_mlp_tc.cu).  Returns the group size g = lcm(S,64)/64 (0: the fused compositor is not used
+ * for this S); if tiles_out != NULL it receives the tile indices worker `cta` of `grid` workers processes, in order, for a launch of n_tiles tiles (at most cap entries; *n_out = count). */
 int nm_debug_tile_schedule(int samples_per_ray, int64_t n_tiles, int grid, int cta, int64_t* tiles_out, int64_t cap, int64_t* n_out);
 
-/* Device-side error flags, readable even after a kernel trapped: out2[0] = tcgen05 pipeline watchdog code (0 = ok),
+/* Device-side error flags, readable even after a kernel trapped: out2[0] = tensor-core pipeline watchdog code (0 = ok),
  * out2[1] = AABB hit-list overflow. */
 int nm_kernel_flags(NmHandle h, int32_t* out2);
 /* Synchronises `stream`, then fails (<0, message in nm_last_error) if a kernel of this handle raised a device-side flag.

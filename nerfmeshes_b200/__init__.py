@@ -1,4 +1,4 @@
-"""nerfmeshes_b200 — B200-native (sm_100a) NeRF render / dense-grid hot path of qway/nerfmeshes.
+"""nerfmeshes_b200 — H100-native (sm_90a) NeRF render / dense-grid hot path of qway/nerfmeshes (the name is historical).
 
 Layout: csrc/ (CUDA kernels + C ABI, built into lib/libnerfmeshes_b200.so), _lib.py (ctypes binding), engine.py (handle +
 torch plumbing), models.py / nerf_api.py / mesh.py / train.py / eval.py (host mirror of the reference's interface for this path).

@@ -47,7 +47,7 @@ struct NmHandle_t {
   // workspace
   Buf t_c, raw_c, w_c, t_f, raw_f, t_u, dirs, origins, lin[3], small, stage_in[3], stage_out[12];
   int lin_n[3] = {0, 0, 0};
-  int* d_err = nullptr;       // [0] tcgen05 watchdog code, [1] aabb hit-list overflow (device alias of h_err)
+  int* d_err = nullptr;       // [0] tensor-core pipeline watchdog code, [1] aabb hit-list overflow (device alias of h_err)
   int* h_err = nullptr;       // mapped pinned host memory: still readable after a device-side trap
   double* d_stats = nullptr;
   cudaStream_t own_stream = nullptr;
@@ -106,7 +106,7 @@ int upload(Buf* b, const void* src, size_t bytes) {
 
 int check_kernel_flags(NmHandle h) {
   const volatile int* flags = h->h_err;
-  NM_CHECK(flags[0] == 0, "tcgen05 pipeline watchdog fired (code %d)", flags[0]);
+  NM_CHECK(flags[0] == 0, "tensor-core pipeline watchdog fired (code %d)", flags[0]);
   NM_CHECK(flags[1] == 0, "AABB sampler: more than 512 voxel hits on one ray (samples / voxel indices of that ray are truncated)");
   return 0;
 }
@@ -427,7 +427,7 @@ int nm_device_check(int device) {
   NM_CHECK(device >= 0 && device < n, "device %d out of range (%d visible)", device, n);
   cudaDeviceProp p;
   NM_CUDA(cudaGetDeviceProperties(&p, device));
-  NM_CHECK(p.major == 10, "device %d is sm_%d%d; this library is built for sm_100a (B200) only", device, p.major, p.minor);
+  NM_CHECK(p.major == 9 && p.minor == 0, "device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, p.major, p.minor);
   return 0;
 }
 

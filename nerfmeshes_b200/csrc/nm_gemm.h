@@ -1,5 +1,5 @@
 // GEMM building blocks of the training backward (nm_train.cu): the fp32 CUDA-core SGEMMs (yard-stick, NM_PREC_FP32) and
-// the tcgen05 split-bf16 GEMM on pre-packed operands (nm_gemm_tc.cu).
+// the wgmma split-bf16 GEMM on pre-packed operands (nm_gemm_tc.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

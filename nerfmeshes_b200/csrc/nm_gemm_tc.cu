@@ -1,26 +1,25 @@
-// tcgen05 GEMM for the training backward (nm_train.cu): D (M,N) = A (M,K) * B (N,K)^T with both operands given as
-// pre-packed hi/lo "ptiles" and fp32 accumulation in TMEM.  fp32 accuracy class comes from the same operand split the
+// wgmma GEMM for the training backward (nm_train.cu): D (M,N) = A (M,K) * B (N,K)^T with both operands given as
+// pre-packed hi/lo "ptiles" and fp32 accumulation in registers.  fp32 accuracy class comes from the same operand split the
 // forward kernel uses (x = hi + lo, three MMAs per product: hi*hi + lo*hi + hi*lo).  Halves are bf16 for the gradient
 // GEMMs (gradients span fp32's exponent range; 16 significand bits per operand, ~2^-16 per product) and fp16 for the
 // forward recompute (22 bits, the forward kernel's class: its relu masks must agree with the forward's).
 //
 // ptile = one (128 operand rows) x (64 K) block: [hi | lo], each 16 KB, 128-byte swizzled, K-major or (per segment and
-// operand, TcSeg.mn) MN-major — the shared-memory image tcgen05.mma reads, so a ptile moves global -> shared with ONE 32 KB
-// cp.async.bulk.  A pack is ptiles ordered
-// [row block][K block].  Packs are produced by pack_rows_kernel (K along the source's columns), pack_cols_kernel (K
-// along the source's rows: the A^T / B^T operands of the weight gradient) and, for everything inside the layer chain,
-// by this kernel's own epilogue.
+// operand, TcSeg.mn) MN-major — the shared-memory image wgmma reads through a descriptor, so a ptile moves global ->
+// shared with ONE 32 KB cp.async.bulk.  A pack is ptiles ordered [row block][K block].  Packs are produced by
+// pack_rows_kernel (K along the source's columns), pack_cols_kernel (K along the source's rows: the A^T / B^T operands of
+// the weight gradient) and, for everything inside the layer chain, by this kernel's own epilogue.
 //
-// Kernel: 18 warps — 0-15 epilogue (TMEM lane group w%4, column quarter w/4, blocks of 32 rows x 16 columns), 16 producer
-// (bulk copies into a ring of K-block stages: 2 x 96 KB for 256-wide tiles, 3 x 64 KB for 128-wide), 17 MMA issuer.
-// Data-path GEMMs are persistent (grid = min(tiles, SMs)) with the accumulator double-buffered in TMEM, so the
-// epilogue of tile i overlaps the main loop of tile i+1; the weight gradient (K = points) splits K over one wave of
-// CTAs and reduces with vector atomics.  Barriers: full[s] (tx bytes), empty[s] (tcgen05.commit), acc_full[b]
-// (tcgen05.commit after a tile's last K block), acc_empty[b] (16 epilogue warps).  tests/test_gemm_protocol.py models
-// the protocol with one-bit parities.  In a split-K launch with a_rowsum the 16 epilogue warps first walk the stage ring as
-// readers and sum the rows of the staged A tiles (the bias gradient when A = dZ^T).  The fused epilogue of the layer-wise
-// walk (bias/relu, rank-1 term, 1-bit masks in and out, row pack and point-major pack of the output, column sums) is
-// described in DESIGN.md section 4.4.
+// Kernel: 12 warps — two consumer warpgroups (rows 0-63 / 64-127 of the 128-row tile; m64n128k16 wgmmas into 64 (NB=1)
+// or 128 (NB=2) accumulator registers per thread, then the epilogue from those registers), and a producer warpgroup
+// whose first warp issues the bulk copies into a ring of K-block stages (2 x 96 KB for 256-wide tiles,
+// 3 x 64 KB for 128-wide).  Data-path GEMMs are persistent (grid = min(tiles, SMs)): the producer fills the next tile's
+// stages while the consumers run the epilogue of the current one.  The weight gradient (K = points) splits K over one
+// wave of CTAs and reduces with vector atomics.  Barriers: full[s] (tx bytes), empty[s] (one arrival per consumer
+// warpgroup once its wgmmas on the stage are complete).  In a split-K launch with a_rowsum the consumers also sum the
+// rows of the staged A tiles (the bias gradient when A = dZ^T).  The fused epilogue of the layer-wise walk (bias/relu,
+// rank-1 term, 1-bit masks in and out, row pack and point-major pack of the output, column sums) is described in
+// DESIGN.md section 4.4.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -33,10 +32,8 @@
 namespace nm {
 namespace {
 
-constexpr int kGemmThreads = 576;   // warps 0-15 epilogue (4 TMEM lane groups x 4 column quarters), 16 producer, 17 MMA issuer
-constexpr int kEpiWarps = 16, kProdWarp = 16, kMmaWarp = 17;
-constexpr uint32_t kIdescF16 = ptx::make_idesc_f16(128, 128);                              // A, B = fp16
-constexpr uint32_t kIdescBf16 = kIdescF16 | (1u << 7) | (1u << 10);                        // A, B = bf16
+constexpr int kGemmThreads = 384;   // warps 0-3, 4-7 consumers; 8-11 producer warpgroup (warp 8 issues)
+constexpr int kProdWarp = 8;
 
 // x = hi + lo in two 16-bit floats: bf16 (8+8 significand bits, fp32's exponent range: gradients) or fp16 (11+11
 // bits, |x| < 65504: activations, encodings and weights of the forward recompute, like the forward kernel)
@@ -52,14 +49,152 @@ __device__ __forceinline__ void split16(float x, int fp16, uint16_t* hi, uint16_
   }
 }
 
-constexpr uint32_t kStgOff = 6u * kPtileBytes;                       // epilogue staging: 16 warps x 32 rows x 17 floats
-constexpr uint32_t kStgWarp = 32u * 17u * 4u;
-constexpr uint32_t kBarOff = kStgOff + (uint32_t)kEpiWarps * kStgWarp;                // barriers + TMEM base behind the 1024-aligned stages
+constexpr uint32_t kStgOff = 6u * kPtileBytes;                       // epilogue staging: 8 warps x 16 rows x 17 floats
+constexpr uint32_t kStgWarp = 16u * 17u * 4u;
+constexpr uint32_t kBarOff = kStgOff + 8u * kStgWarp;                // barriers behind the 1024-aligned stages
 constexpr uint32_t kGemmSmem = kBarOff + 128u;
 
+// One K block of the tile: every pass of the four K=16 steps into the NB accumulators (K-major / MN-major operands).
+template <int TA, int TB, int BF16, int NB>
+__device__ __forceinline__ void mma_kblock(float (&acc)[2][64], uint32_t a, uint32_t stage, int nbv, int n_passes) {
+  const uint64_t a_hi = TA ? ptx::make_mnmajor_sw128_desc(a) : ptx::make_kmajor_sw128_desc(a);
+  const uint64_t a_lo = TA ? ptx::make_mnmajor_sw128_desc(a + kPtileHalf) : ptx::make_kmajor_sw128_desc(a + kPtileHalf);
+  constexpr uint64_t a_step = TA ? 128u : 2u, b_step = TB ? 128u : 2u;   // per k16: 2048 B (MN-major) / 32 B (K-major)
+#pragma unroll
+  for (int j = 0; j < NB; ++j) {
+    if (j >= nbv) break;
+    const uint32_t bs = stage + kPtileBytes * (uint32_t)(1 + j);
+    const uint64_t b_hi = TB ? ptx::make_mnmajor_sw128_desc(bs) : ptx::make_kmajor_sw128_desc(bs);
+    const uint64_t b_lo = TB ? ptx::make_mnmajor_sw128_desc(bs + kPtileHalf) : ptx::make_kmajor_sw128_desc(bs + kPtileHalf);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) ptx::wgmma_m64n128<TA, TB, BF16>(acc[j], a_hi + k * a_step, b_hi + k * b_step, 1u);
+    if (n_passes == 3) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) ptx::wgmma_m64n128<TA, TB, BF16>(acc[j], a_lo + k * a_step, b_hi + k * b_step, 1u);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) ptx::wgmma_m64n128<TA, TB, BF16>(acc[j], a_hi + k * a_step, b_lo + k * b_step, 1u);
+    }
+  }
+}
+
+// Epilogue of one 16-row x 16-column block of a warp, staged in stg (pitch 17): lane = (row sub = lane / 4, 4 columns
+// q4 = 4 * (lane % 4)), rows sub and sub + 8.  row0: the block's first global row; rt0: its row within the 128-row block.
+__device__ __noinline__ void epi_block(const TcGemmParams& P, float* stg, int lane, int rb, int row0, int rt0, int n0) {
+  const int sub = lane >> 2, q4 = (lane & 3) * 4;
+  const GemmEpi& E = P.epi;
+  const int n = n0 + q4;                 // first of this lane's 4 global columns
+  if (n >= P.N || (P.dbg & 4)) return;
+  if (P.atomic) {
+    const bool vec_atomic = (P.ldd & 3) == 0 && (reinterpret_cast<uintptr_t>(P.D) & 15) == 0;
+#pragma unroll
+    for (int it = 0; it < 2; ++it) {
+      const int rr = it * 8 + sub, m = row0 + rr;
+      const float* sp = &stg[rr * 17 + q4];
+      const float4 v = make_float4(sp[0], sp[1], sp[2], sp[3]);
+      if (m < P.M) {
+        float* dp = P.D + (size_t)m * P.ldd + n;
+        if (vec_atomic && n + 3 < P.N) {
+          atomicAdd(reinterpret_cast<float4*>(dp), v);      // one 16-byte reduction instead of four
+        } else {
+          atomicAdd(dp, v.x);
+          if (n + 1 < P.N) atomicAdd(dp + 1, v.y);
+          if (n + 2 < P.N) atomicAdd(dp + 2, v.z);
+          if (n + 3 < P.N) atomicAdd(dp + 3, v.w);
+        }
+      }
+    }
+    return;
+  }
+  // data-path outputs: N is a multiple of 64, rows are 16-byte aligned
+  float4 bias = make_float4(0.f, 0.f, 0.f, 0.f), w1 = bias;
+  if (E.bias) bias = *reinterpret_cast<const float4*>(E.bias + n);
+  if (E.r1_vec) w1 = *reinterpret_cast<const float4*>(E.r1_w + n);
+  float4 v[2], cs = make_float4(0.f, 0.f, 0.f, 0.f);
+  uint32_t mw[2];
+  float r1[2];
+#pragma unroll
+  for (int it = 0; it < 2; ++it) {
+    const int rr = it * 8 + sub, m = min(row0 + rr, P.M - 1);
+    const float* sp = &stg[rr * 17 + q4];
+    v[it] = make_float4(sp[0], sp[1], sp[2], sp[3]);
+    mw[it] = P.bits_in ? ((uint32_t)P.bits_in[(size_t)m * P.bits_ld + (n >> 4)] >> (n & 15)) : 0xfu;   // this lane's 4 mask bits
+    r1[it] = E.r1_vec ? E.r1_vec[(size_t)m * E.r1_stride] : 0.f;
+    if (E.accumulate) {
+      const float4 c = *reinterpret_cast<const float4*>(P.D + (size_t)m * P.ldd + n);
+      v[it].x += c.x; v[it].y += c.y; v[it].z += c.z; v[it].w += c.w;
+    }
+  }
+#pragma unroll
+  for (int it = 0; it < 2; ++it) {
+    const int rr = it * 8 + sub, m = row0 + rr;
+    float4 o = v[it];
+    o.x = fmaf(r1[it], w1.x, o.x + bias.x); o.y = fmaf(r1[it], w1.y, o.y + bias.y);
+    o.z = fmaf(r1[it], w1.z, o.z + bias.z); o.w = fmaf(r1[it], w1.w, o.w + bias.w);
+    if (E.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
+    if (!(mw[it] & 1u)) o.x = 0.f;
+    if (!(mw[it] & 2u)) o.y = 0.f;
+    if (!(mw[it] & 4u)) o.z = 0.f;
+    if (!(mw[it] & 8u)) o.w = 0.f;
+    if (P.bits_out) {      // relu mask of this output row segment: 4 lanes x 4 bits -> one halfword
+      uint32_t bits = ((o.x > 0.f ? 1u : 0u) | (o.y > 0.f ? 2u : 0u) | (o.z > 0.f ? 4u : 0u) | (o.w > 0.f ? 8u : 0u)) << q4;
+      bits |= __shfl_xor_sync(0xffffffffu, bits, 1);
+      bits |= __shfl_xor_sync(0xffffffffu, bits, 2);
+      if (!(lane & 3) && m < P.M) P.bits_out[(size_t)m * P.bits_ld + (n >> 4)] = (uint16_t)bits;
+    }
+    if (m < P.M) {
+      if (!P.skip_d) *reinterpret_cast<float4*>(P.D + (size_t)m * P.ldd + n) = o;
+      cs.x += o.x; cs.y += o.y; cs.z += o.z; cs.w += o.w;
+    } else {
+      o = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    if (P.packT_out) { float* sp = &stg[rr * 17 + q4]; sp[0] = o.x; sp[1] = o.y; sp[2] = o.z; sp[3] = o.w; }
+    if (P.pack_out) {
+      // even lanes gather their neighbour's 4 columns: 8 consecutive columns = one 16-byte chunk of the tile row
+      const float e0 = __shfl_down_sync(0xffffffffu, o.x, 1), e1 = __shfl_down_sync(0xffffffffu, o.y, 1);
+      const float e2 = __shfl_down_sync(0xffffffffu, o.z, 1), e3 = __shfl_down_sync(0xffffffffu, o.w, 1);
+      if (!(lane & 1)) {
+        const float vals[8] = {o.x, o.y, o.z, o.w, e0, e1, e2, e3};
+        __align__(16) uint16_t hi[8], lo[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) split16(vals[e], P.pack_fp16, &hi[e], &lo[e]);
+        const int r_t = rt0 + rr, c8 = (n & 63) >> 3;
+        uint8_t* tile = P.pack_out + ((size_t)rb * P.pack_kbt + (n >> 6)) * kPtileBytes;
+        const uint32_t off = (uint32_t)r_t * 128u + (uint32_t)((c8 ^ (r_t & 7)) << 4);
+        *reinterpret_cast<uint4*>(tile + off) = *reinterpret_cast<const uint4*>(hi);
+        *reinterpret_cast<uint4*>(tile + kPtileHalf + off) = *reinterpret_cast<const uint4*>(lo);
+      }
+    }
+  }
+  if (P.packT_out) {   // the finished 16x16 block, transposed: lane = (column f, 8-row chunk)
+    __syncwarp();
+    const int f = lane & 15, c = lane >> 4;
+    const int nf = n0 + f;
+    const int row = nf & 127;
+    // points rt0 .. rt0+15 of row block rb: K block rb * 2 + rt0 / 64, 8-point chunk (rt0 % 64) / 8 + c
+    uint8_t* tile = P.packT_out + ((size_t)(nf >> 7) * P.packT_kbt + (rb * 2 + (rt0 >> 6))) * kPtileBytes;
+    __align__(16) uint16_t hi[8], lo[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) split16(stg[(c * 8 + e) * 17 + f], 0, &hi[e], &lo[e]);
+    const int c8 = ((rt0 & 63) >> 3) + c;
+    const uint32_t off = (uint32_t)row * 128u + (uint32_t)((c8 ^ (row & 7)) << 4);
+    *reinterpret_cast<uint4*>(tile + off) = *reinterpret_cast<const uint4*>(hi);
+    *reinterpret_cast<uint4*>(tile + kPtileHalf + off) = *reinterpret_cast<const uint4*>(lo);
+  }
+  if (P.colsum) {      // lanes with equal lane%4 hold the same 4 columns
+#pragma unroll
+    for (int d = 4; d <= 16; d <<= 1) {
+      cs.x += __shfl_xor_sync(0xffffffffu, cs.x, d); cs.y += __shfl_xor_sync(0xffffffffu, cs.y, d);
+      cs.z += __shfl_xor_sync(0xffffffffu, cs.z, d); cs.w += __shfl_xor_sync(0xffffffffu, cs.w, d);
+    }
+    if (lane < 4) {
+      atomicAdd(P.colsum + n, cs.x); atomicAdd(P.colsum + n + 1, cs.y);
+      atomicAdd(P.colsum + n + 2, cs.z); atomicAdd(P.colsum + n + 3, cs.w);
+    }
+  }
+}
+
 // Tiles of one CTA.  Data-path GEMMs are persistent: grid = min(tiles, SMs), tile t = blockIdx.x + i * gridDim.x walks
-// (row block, column group) pairs, and the accumulator is double-buffered in TMEM so that the epilogue of tile i
-// overlaps the main loop of tile i+1.  Split-K (weight gradient) launches one tile per CTA: (row block, column group,
+// (row block, column group) pairs.  Split-K (weight gradient) launches one tile per CTA: (row block, column group,
 // K split) = blockIdx.
 template <int NB>
 __global__ void __launch_bounds__(kGemmThreads, 1) tc_gemm_kernel(const __grid_constant__ TcGemmParams P) {
@@ -69,11 +204,8 @@ __global__ void __launch_bounds__(kGemmThreads, 1) tc_gemm_kernel(const __grid_c
   const uint32_t sbase = ptx::smem_u32(smem);
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   const uint32_t bar0 = sbase + kBarOff;
-  volatile uint32_t* s_tmem = reinterpret_cast<volatile uint32_t*>(smem + kBarOff + 120);
   auto full = [&](int s) { return bar0 + 8u * s; };
   auto empty = [&](int s) { return bar0 + 8u * (NS + s); };
-  auto acc_full = [&](int b) { return bar0 + 8u * (2 * NS + b); };
-  auto acc_empty = [&](int b) { return bar0 + 8u * (2 * NS + 2 + b); };
 
   const bool pers = P.atomic == 0;
   const int n_tiles = pers ? P.n_rb_a * P.col_groups : 1;
@@ -90,22 +222,15 @@ __global__ void __launch_bounds__(kGemmThreads, 1) tc_gemm_kernel(const __grid_c
   const bool sum_rows = !pers && P.a_rowsum != nullptr && blockIdx.y == 0;
   if (threadIdx.x == 0) {
     if (sbase & 1023u) { if (P.err) atomicExch(P.err, 90); __trap(); }
-    for (int s = 0; s < NS; ++s) { ptx::mbar_init(full(s), 1); ptx::mbar_init(empty(s), sum_rows ? 1 + kEpiWarps : 1); }
-    for (int b = 0; b < 2; ++b) { ptx::mbar_init(acc_full(b), 1); ptx::mbar_init(acc_empty(b), kEpiWarps); }
+    for (int s = 0; s < NS; ++s) { ptx::mbar_init(full(s), 1); ptx::mbar_init(empty(s), 2); }
     ptx::fence_mbar_init();
   }
-  if (warp == kMmaWarp) {
-    ptx::tmem_alloc(bar0 + 120u, 256 * NB);          // two accumulator buffers of 128*NB columns
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem = *s_tmem;
 
-  if (warp == kProdWarp) {
+  if (warp >= kProdWarp) {
     // ------------------------------------------------------------ producer
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp == kProdWarp && lane == 0) {
       int it = 0;
       for (int t = t_first; t < n_tiles; t += t_step) {
         const int rb = tile_rb(t), cb0 = tile_cb0(t);
@@ -117,7 +242,6 @@ __global__ void __launch_bounds__(kGemmThreads, 1) tc_gemm_kernel(const __grid_c
           const int kb = kk < n0 ? k0 + kk : kk - n0;
           const TcSeg& S = P.seg[sg];
           const uint32_t dst = sbase + (uint32_t)s * STAGE;
-          if (P.dbg & 2) { ptx::mbar_arrive(full(s)); continue; }
           ptx::mbar_expect_tx(full(s), kPtileBytes * (uint32_t)(1 + nbv));
           ptx::bulk_g2s(dst, S.a + ((size_t)rb * S.a_kbt + kb) * kPtileBytes, kPtileBytes, full(s));
           for (int j = 0; j < nbv; ++j)
@@ -126,266 +250,106 @@ __global__ void __launch_bounds__(kGemmThreads, 1) tc_gemm_kernel(const __grid_c
         }
       }
     }
-  } else if (warp == kMmaWarp) {
-    // ------------------------------------------------------------ MMA issuer (whole warp converged; one lane issues)
-    const uint32_t idesc = P.fp16 ? kIdescF16 : kIdescBf16;
-    int it = 0, i = 0;
-    for (int t = t_first; t < n_tiles; t += t_step, ++i) {
-      const int nbv = min(NB, P.n_rb_b - tile_cb0(t));
-      const int b = i & 1;
-      if (i >= 2) {                                   // the epilogue must have drained this accumulator buffer
-        ptx::mbar_wait(acc_empty(b), (uint32_t)(((i >> 1) - 1) & 1), P.err, 94);
-        ptx::tc_fence_after();
+    return;
+  }
+  // ------------------------------------------------------------ consumers: main loop, then the epilogue from the registers
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int wg = warp >> 2, wi = warp & 3, t = threadIdx.x & 127;
+  float* stg = reinterpret_cast<float*>(smem + kStgOff + (uint32_t)warp * kStgWarp);     // 16 rows, pitch 17 floats
+  float rsum = 0.f;                                                                    // sum_rows: this thread's row part
+  float acc[2][64];
+  int it = 0;
+  for (int tt = t_first; tt < n_tiles; tt += t_step) {
+    const int rb = tile_rb(tt), cb0 = tile_cb0(tt);
+    const int nbv = min(NB, P.n_rb_b - cb0);
+#pragma unroll
+    for (int j = 0; j < 2; ++j)
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[j][i] = 0.f;
+    ptx::wgmma_fence();
+    int prev = -1;
+    for (int kk = 0; kk < nk; ++kk, ++it) {
+      const int s = it % NS;
+      ptx::mbar_wait(full(s), (uint32_t)((it / NS) & 1), P.err, 92);
+      const uint32_t st = sbase + (uint32_t)s * STAGE;
+      const int mn = P.seg[kk < n0 ? 0 : 1].mn;
+      if (sum_rows) {
+        // Row sums of the A tile (this warpgroup's 64 rows) while the tensor cores consume it; hi + lo halves.
+        const uint8_t* at = smem + (size_t)s * STAGE;
+        if (mn & 1) {
+          // MN-major: [feature group of 64][K row (point) 0..63][128 B = 8 chunks of 8 features, chunk ^= row & 7]
+          const int f = t & 63, kr0 = (t >> 6) * 32;
+          for (int k = kr0; k < kr0 + 32; ++k) {
+            const uint32_t off = (uint32_t)wg * 8192u + (uint32_t)k * 128u + ((((uint32_t)f >> 3) ^ ((uint32_t)k & 7u)) << 4) + (uint32_t)(f & 7) * 2u;
+            const uint32_t h = *reinterpret_cast<const uint16_t*>(at + off), l = *reinterpret_cast<const uint16_t*>(at + kPtileHalf + off);
+            rsum += __uint_as_float(h << 16) + __uint_as_float(l << 16);
+          }
+        } else {
+          // K-major: two threads per row, 32 K elements each (the swizzle only permutes chunks within the row)
+          const int row = wg * 64 + (t >> 1);
+          const uint4* rp = reinterpret_cast<const uint4*>(at + (size_t)row * 128u + (size_t)(t & 1) * 64u);
+          float acc_r = 0.f;
+#pragma unroll
+          for (int c = 0; c < 4; ++c) {
+            const uint4 h = rp[c], l = rp[c + kPtileHalf / 16];
+            const uint32_t w[8] = {h.x, h.y, h.z, h.w, l.x, l.y, l.z, l.w};
+#pragma unroll
+            for (int e = 0; e < 8; ++e) acc_r += __uint_as_float(w[e] << 16) + __uint_as_float(w[e] & 0xffff0000u);
+          }
+          rsum += acc_r;
+        }
       }
-      const uint32_t dacc = tmem + (uint32_t)(b * 128 * NB);
-      for (int kk = 0; kk < nk; ++kk, ++it) {
-        const int s = it % NS;
-        ptx::mbar_wait(full(s), (uint32_t)((it / NS) & 1), P.err, 92);
-        ptx::tc_fence_after();
-        const uint32_t a = sbase + (uint32_t)s * STAGE;
-        const int mn = P.seg[kk < n0 ? 0 : 1].mn;
+      const uint32_t a = st + (uint32_t)wg * 8192u;    // rows 64.. : +64 rows (K-major) / the second MN group (MN-major)
+      if (!(P.dbg & 1)) {
         const bool amn = mn & 1, bmn = mn & 2;
-        const uint32_t idesc_s = idesc | (amn ? (1u << 15) : 0u) | (bmn ? (1u << 16) : 0u);
-        const uint64_t a_step = amn ? 128u : 2u, b_step = bmn ? 128u : 2u;       // per k16: 2048 B (MN-major) / 32 B (K-major)
-        const uint64_t a_hi = amn ? ptx::make_mnmajor_sw128_desc(a) : ptx::make_kmajor_sw128_desc(a);
-        const uint64_t a_lo = amn ? ptx::make_mnmajor_sw128_desc(a + kPtileHalf) : ptx::make_kmajor_sw128_desc(a + kPtileHalf);
-        for (int j = 0; j < ((P.dbg & 1) ? 0 : nbv); ++j) {
-          const uint32_t bs = a + kPtileBytes * (uint32_t)(1 + j);
-          const uint64_t b_hi = bmn ? ptx::make_mnmajor_sw128_desc(bs) : ptx::make_kmajor_sw128_desc(bs);
-          const uint64_t b_lo = bmn ? ptx::make_mnmajor_sw128_desc(bs + kPtileHalf) : ptx::make_kmajor_sw128_desc(bs + kPtileHalf);
-          if (P.n_passes == 3) ptx::mma_block_ss3g(dacc + 128u * j, a_hi, a_lo, b_hi, b_lo, idesc_s, kk > 0 ? 1u : 0u, 4u, a_step, b_step);
-          else ptx::mma_block_ss1g(dacc + 128u * j, a_hi, b_hi, idesc_s, kk > 0 ? 1u : 0u, 4u, a_step, b_step);
+        if (P.fp16) {
+          if (amn) { if (bmn) mma_kblock<1, 1, 0, NB>(acc, a, st, nbv, P.n_passes); else mma_kblock<1, 0, 0, NB>(acc, a, st, nbv, P.n_passes); }
+          else     { if (bmn) mma_kblock<0, 1, 0, NB>(acc, a, st, nbv, P.n_passes); else mma_kblock<0, 0, 0, NB>(acc, a, st, nbv, P.n_passes); }
+        } else {
+          if (amn) { if (bmn) mma_kblock<1, 1, 1, NB>(acc, a, st, nbv, P.n_passes); else mma_kblock<1, 0, 1, NB>(acc, a, st, nbv, P.n_passes); }
+          else     { if (bmn) mma_kblock<0, 1, 1, NB>(acc, a, st, nbv, P.n_passes); else mma_kblock<0, 0, 1, NB>(acc, a, st, nbv, P.n_passes); }
         }
-        ptx::tc_commit_elect(empty(s));
       }
-      ptx::tc_commit_elect(acc_full(b));
+      ptx::wgmma_commit();
+      ptx::wgmma_wait<1>();                              // the previous K block's MMAs are complete: release its stage
+      if (prev >= 0 && t == 0) ptx::mbar_arrive(empty(prev));
+      prev = s;
     }
-  } else {
-    // ------------------------------------------------------------ epilogue: TMEM -> registers -> shared -> global
-    // 16 warps: warp w reads TMEM lanes 32*(w%4).. (its 32 rows) and the column quarter w/4 of the CTA tile, in blocks of
-    // 32 rows x 16 columns.  A thread owns one accumulator row; each block is transposed through a per-warp staging tile
-    // so that global accesses are contiguous row segments: a lane then handles 4 columns of rows sub, sub+8, ...
-    // The epilogue is instruction-latency bound, hence many warps with short dependent chains rather than few wide ones.
-    if (sum_rows && (P.seg[0].mn & 1)) {
-      // MN-major A tile: [feature group of 64][K row (point) 0..63][128 B = 8 chunks of 8 features, chunk ^= row & 7].  Thread t
-      // owns the 8 features of chunk column fc = t % 16 (group fc / 8, chunk fc % 8) over the two K rows 2 * (t / 16) + {0, 1}.
-      const int t = (int)threadIdx.x;                      // 0..511: the 16 epilogue warps
-      const int fc = t & 15, r2 = (t >> 4) * 2;
-      float acc[8];
+    ptx::wgmma_wait<0>();
+    if (prev >= 0 && t == 0) ptx::mbar_arrive(empty(prev));
 #pragma unroll
-      for (int e = 0; e < 8; ++e) acc[e] = 0.f;
-      for (int kk = 0; kk < nk; ++kk) {
-        const int s = kk % NS;
-        ptx::mbar_wait(full(s), (uint32_t)((kk / NS) & 1), P.err, 95);
-        const uint8_t* at = smem + (size_t)s * STAGE + (size_t)(fc >> 3) * 8192u;
+    for (int j = 0; j < 2; ++j) ptx::fence_regs<64>(acc[j]);
+
+    // epilogue: warp wi of warpgroup wg owns rows 16 wi .. 16 wi + 15 of the warpgroup's 64; each 16 x 16 block goes
+    // through the warp's staging tile so that global accesses are contiguous row segments
+    const int rt0 = wg * 64 + wi * 16, row0 = rb * 128 + rt0;
+    const int lr = lane >> 2, lc = 2 * (lane & 3);
 #pragma unroll
-        for (int u = 0; u < 2; ++u) {
-          const int row = r2 + u;
-          const uint32_t off = (uint32_t)row * 128u + (uint32_t)((((fc & 7) ^ (row & 7))) << 4);
-          const uint4 h = *reinterpret_cast<const uint4*>(at + off);
-          const uint4 l = *reinterpret_cast<const uint4*>(at + kPtileHalf + off);
-          const uint32_t hw[4] = {h.x, h.y, h.z, h.w}, lw[4] = {l.x, l.y, l.z, l.w};
+    for (int j = 0; j < NB; ++j) {
+      if (j >= nbv) break;
 #pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            acc[2 * e] += __uint_as_float(hw[e] << 16) + __uint_as_float(lw[e] << 16);
-            acc[2 * e + 1] += __uint_as_float(hw[e] & 0xffff0000u) + __uint_as_float(lw[e] & 0xffff0000u);
-          }
-        }
+      for (int blk = 0; blk < 8; ++blk) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int q = 0; q < 4; ++q)
+            stg[(lr + 8 * (q >> 1)) * 17 + h * 8 + lc + (q & 1)] = acc[j][(blk * 2 + h) * 4 + q];
         __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(empty(s));
-      }
-      // fold the 32 row slices: lanes l and l ^ 16 share fc; then one shared-memory accumulator per feature across the warps
-#pragma unroll
-      for (int e = 0; e < 8; ++e) acc[e] += __shfl_xor_sync(0xffffffffu, acc[e], 16);
-      float* red = reinterpret_cast<float*>(smem + kStgOff);            // epilogue staging, not in use yet
-      if (t < 128) red[t] = 0.f;
-      ptx::named_bar_sync(1, kEpiWarps * 32);
-      if (lane < 16) {
-#pragma unroll
-        for (int e = 0; e < 8; ++e) atomicAdd(red + fc * 8 + e, acc[e]);
-      }
-      ptx::named_bar_sync(1, kEpiWarps * 32);
-      if (t < 128) {
-        const int row = (int)blockIdx.x * 128 + t;
-        if (row < P.M) atomicAdd(P.a_rowsum + row, red[t]);
-      }
-      ptx::named_bar_sync(1, kEpiWarps * 32);                           // red[] is the staging area of the epilogue below
-    } else if (sum_rows) {
-      // Row sums of the A tiles while the MMA warp consumes them: warp w owns rows 8w..8w+7, 8 lanes cover one 128-byte row
-      // (64 K elements; the swizzle only permutes chunks within the row, irrelevant for a sum), hi + lo halves.
-      float acc[2] = {0.f, 0.f};
-      const int r0 = warp * 8 + (lane >> 3);
-      for (int kk = 0; kk < nk; ++kk) {
-        const int s = kk % NS;
-        ptx::mbar_wait(full(s), (uint32_t)((kk / NS) & 1), P.err, 95);
-        const uint8_t* at = smem + (size_t)s * STAGE + (size_t)(lane & 7) * 16u;
-#pragma unroll
-        for (int u = 0; u < 2; ++u) {
-          const uint4 h = *reinterpret_cast<const uint4*>(at + (size_t)(r0 + 4 * u) * 128u);
-          const uint4 l = *reinterpret_cast<const uint4*>(at + kPtileHalf + (size_t)(r0 + 4 * u) * 128u);
-          const uint32_t w[8] = {h.x, h.y, h.z, h.w, l.x, l.y, l.z, l.w};
-          float t = 0.f;
-#pragma unroll
-          for (int e = 0; e < 8; ++e) t += __uint_as_float(w[e] << 16) + __uint_as_float(w[e] & 0xffff0000u);
-          acc[u] += t;
-        }
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(empty(s));
-      }
-#pragma unroll
-      for (int u = 0; u < 2; ++u) {
-        float t = acc[u];
-        t += __shfl_xor_sync(0xffffffffu, t, 1); t += __shfl_xor_sync(0xffffffffu, t, 2); t += __shfl_xor_sync(0xffffffffu, t, 4);
-        const int row = (int)blockIdx.x * 128 + r0 + 4 * u;
-        if ((lane & 7) == 0 && row < P.M) atomicAdd(P.a_rowsum + row, t);
-      }
-    }
-    float* stg = reinterpret_cast<float*>(smem + kStgOff + (uint32_t)warp * kStgWarp);     // 32 rows, pitch 17 floats
-    const int lg = warp & 3, quarter = warp >> 2;
-    const int sub = lane >> 2, q4 = (lane & 3) * 4;
-    const GemmEpi& E = P.epi;
-    const bool vec_atomic = (P.ldd & 3) == 0 && (reinterpret_cast<uintptr_t>(P.D) & 15) == 0;
-    int i = 0;
-    for (int t = t_first; t < n_tiles; t += t_step, ++i) {
-      const int rb = tile_rb(t), cb0 = tile_cb0(t);
-      const int nbv = min(NB, P.n_rb_b - cb0);
-      const int b = i & 1;
-      const uint32_t dacc = tmem + (uint32_t)(b * 128 * NB);
-      ptx::mbar_wait(acc_full(b), (uint32_t)((i >> 1) & 1), P.err, 93);
-      ptx::tc_fence_after();
-      const int row0 = rb * 128 + lg * 32;
-#pragma unroll 1
-      for (int blk = quarter * 2 * NB; blk < (quarter + 1) * 2 * NB; ++blk) {
-        const int cbase = blk * 16, j = cbase >> 7, c0 = cbase & 127;
-        if (j >= nbv) continue;
-        uint32_t r[16];
-        NM_TMEM_LD16(dacc + ((uint32_t)(lg * 32) << 16) + (uint32_t)cbase, r);
-        ptx::tmem_wait_ld();
-#pragma unroll
-        for (int c = 0; c < 16; ++c) stg[lane * 17 + c] = __uint_as_float(r[c]);
-        __syncwarp();
-        const int n = (cb0 + j) * 128 + c0 + q4;                 // first of this lane's 4 global columns
-        if (n < P.N && !(P.dbg & 4)) {
-          if (P.atomic) {
-#pragma unroll
-            for (int it = 0; it < 4; ++it) {
-              const int rr = it * 8 + sub, m = row0 + rr;
-              const float* sp = &stg[rr * 17 + q4];
-              const float4 v = make_float4(sp[0], sp[1], sp[2], sp[3]);
-              if (m < P.M) {
-                float* dp = P.D + (size_t)m * P.ldd + n;
-                if (vec_atomic && n + 3 < P.N) {
-                  atomicAdd(reinterpret_cast<float4*>(dp), v);      // one 16-byte reduction instead of four
-                } else {
-                  atomicAdd(dp, v.x);
-                  if (n + 1 < P.N) atomicAdd(dp + 1, v.y);
-                  if (n + 2 < P.N) atomicAdd(dp + 2, v.z);
-                  if (n + 3 < P.N) atomicAdd(dp + 3, v.w);
-                }
-              }
-            }
-          } else {
-            // data-path outputs: N is a multiple of 64, rows are 16-byte aligned
-            float4 bias = make_float4(0.f, 0.f, 0.f, 0.f), w1 = bias;
-            if (E.bias) bias = *reinterpret_cast<const float4*>(E.bias + n);
-            if (E.r1_vec) w1 = *reinterpret_cast<const float4*>(E.r1_w + n);
-            float4 v[4], cs = make_float4(0.f, 0.f, 0.f, 0.f);
-            uint32_t mw[4];
-            float r1[4];
-#pragma unroll
-            for (int it = 0; it < 4; ++it) {
-              const int rr = it * 8 + sub, m = min(row0 + rr, P.M - 1);
-              const float* sp = &stg[rr * 17 + q4];
-              v[it] = make_float4(sp[0], sp[1], sp[2], sp[3]);
-              mw[it] = P.bits_in ? ((uint32_t)P.bits_in[(size_t)m * P.bits_ld + (n >> 4)] >> q4) : 0xfu;   // this lane's 4 mask bits
-              r1[it] = E.r1_vec ? E.r1_vec[(size_t)m * E.r1_stride] : 0.f;
-              if (E.accumulate) {
-                const float4 c = *reinterpret_cast<const float4*>(P.D + (size_t)m * P.ldd + n);
-                v[it].x += c.x; v[it].y += c.y; v[it].z += c.z; v[it].w += c.w;
-              }
-            }
-#pragma unroll
-            for (int it = 0; it < 4; ++it) {
-              const int rr = it * 8 + sub, m = row0 + rr;
-              float4 o = v[it];
-              o.x = fmaf(r1[it], w1.x, o.x + bias.x); o.y = fmaf(r1[it], w1.y, o.y + bias.y);
-              o.z = fmaf(r1[it], w1.z, o.z + bias.z); o.w = fmaf(r1[it], w1.w, o.w + bias.w);
-              if (E.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-              if (!(mw[it] & 1u)) o.x = 0.f;
-              if (!(mw[it] & 2u)) o.y = 0.f;
-              if (!(mw[it] & 4u)) o.z = 0.f;
-              if (!(mw[it] & 8u)) o.w = 0.f;
-              if (P.bits_out) {      // relu mask of this output row segment: 4 lanes x 4 bits -> one halfword
-                uint32_t bits = ((o.x > 0.f ? 1u : 0u) | (o.y > 0.f ? 2u : 0u) | (o.z > 0.f ? 4u : 0u) | (o.w > 0.f ? 8u : 0u)) << q4;
-                bits |= __shfl_xor_sync(0xffffffffu, bits, 1);
-                bits |= __shfl_xor_sync(0xffffffffu, bits, 2);
-                if (!(lane & 3) && m < P.M) P.bits_out[(size_t)m * P.bits_ld + (n >> 4)] = (uint16_t)bits;
-              }
-              if (m < P.M) {
-                if (!P.skip_d) *reinterpret_cast<float4*>(P.D + (size_t)m * P.ldd + n) = o;
-                cs.x += o.x; cs.y += o.y; cs.z += o.z; cs.w += o.w;
-              } else {
-                o = make_float4(0.f, 0.f, 0.f, 0.f);
-              }
-              if (P.packT_out) { float* sp = &stg[rr * 17 + q4]; sp[0] = o.x; sp[1] = o.y; sp[2] = o.z; sp[3] = o.w; }
-              if (P.pack_out) {
-                // even lanes gather their neighbour's 4 columns: 8 consecutive columns = one 16-byte chunk of the tile row
-                const float e0 = __shfl_down_sync(0xffffffffu, o.x, 1), e1 = __shfl_down_sync(0xffffffffu, o.y, 1);
-                const float e2 = __shfl_down_sync(0xffffffffu, o.z, 1), e3 = __shfl_down_sync(0xffffffffu, o.w, 1);
-                if (!(lane & 1)) {
-                  const float vals[8] = {o.x, o.y, o.z, o.w, e0, e1, e2, e3};
-                  __align__(16) uint16_t hi[8], lo[8];
-#pragma unroll
-                  for (int e = 0; e < 8; ++e) split16(vals[e], P.pack_fp16, &hi[e], &lo[e]);
-                  const int r_t = lg * 32 + rr, c8 = (n & 63) >> 3;
-                  uint8_t* tile = P.pack_out + ((size_t)rb * P.pack_kbt + (n >> 6)) * kPtileBytes;
-                  const uint32_t off = (uint32_t)r_t * 128u + (uint32_t)((c8 ^ (r_t & 7)) << 4);
-                  *reinterpret_cast<uint4*>(tile + off) = *reinterpret_cast<const uint4*>(hi);
-                  *reinterpret_cast<uint4*>(tile + kPtileHalf + off) = *reinterpret_cast<const uint4*>(lo);
-                }
-              }
-            }
-            if (P.packT_out) {   // the finished 32x16 block, transposed: lane = (column f, pair of 8-row chunks)
-              __syncwarp();
-              const int f = lane & 15, ch0 = (lane >> 4) * 2;
-              const int nf = (cb0 + j) * 128 + c0 + f;
-              const int row = nf & 127;
-              uint8_t* tile = P.packT_out + ((size_t)(nf >> 7) * P.packT_kbt + (rb * 2 + (lg >> 1))) * kPtileBytes;
-#pragma unroll
-              for (int c = ch0; c < ch0 + 2; ++c) {
-                __align__(16) uint16_t hi[8], lo[8];
-#pragma unroll
-                for (int e = 0; e < 8; ++e) split16(stg[(c * 8 + e) * 17 + f], 0, &hi[e], &lo[e]);
-                const int c8 = (lg & 1) * 4 + c;
-                const uint32_t off = (uint32_t)row * 128u + (uint32_t)((c8 ^ (row & 7)) << 4);
-                *reinterpret_cast<uint4*>(tile + off) = *reinterpret_cast<const uint4*>(hi);
-                *reinterpret_cast<uint4*>(tile + kPtileHalf + off) = *reinterpret_cast<const uint4*>(lo);
-              }
-            }
-            if (P.colsum) {      // lanes with equal lane%4 hold the same 4 columns
-#pragma unroll
-              for (int d = 4; d <= 16; d <<= 1) {
-                cs.x += __shfl_xor_sync(0xffffffffu, cs.x, d); cs.y += __shfl_xor_sync(0xffffffffu, cs.y, d);
-                cs.z += __shfl_xor_sync(0xffffffffu, cs.z, d); cs.w += __shfl_xor_sync(0xffffffffu, cs.w, d);
-              }
-              if (lane < 4) {
-                atomicAdd(P.colsum + n, cs.x); atomicAdd(P.colsum + n + 1, cs.y);
-                atomicAdd(P.colsum + n + 2, cs.z); atomicAdd(P.colsum + n + 3, cs.w);
-              }
-            }
-          }
-        }
+        epi_block(P, stg, lane, rb, row0, rt0, (cb0 + j) * 128 + blk * 16);
         __syncwarp();
       }
-      // all TMEM reads of this warp for tile i are complete (wait::ld above): hand the buffer back to the MMA warp
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(acc_empty(b));
     }
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == kMmaWarp) ptx::tmem_dealloc(tmem, 256 * NB);
+  if (sum_rows) {
+    if (P.seg[0].mn & 1) {
+      const int row = (int)blockIdx.x * 128 + wg * 64 + (t & 63);
+      if (row < P.M) atomicAdd(P.a_rowsum + row, rsum);
+    } else {
+      rsum += __shfl_xor_sync(0xffffffffu, rsum, 1);
+      const int row = (int)blockIdx.x * 128 + wg * 64 + (t >> 1);
+      if (!(t & 1) && row < P.M) atomicAdd(P.a_rowsum + row, rsum);
+    }
+  }
 }
 
 // ------------------------------------------------------------------------------------------------ packers

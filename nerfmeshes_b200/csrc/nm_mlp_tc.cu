@@ -1,42 +1,34 @@
-// Fused FlexibleNeRFModel forward on the 5th-gen tensor cores (sm_100a): positional encoding -> all linear layers ->
-// sigma / rgb heads in ONE persistent kernel.  Activations never leave the SM: the fp32 accumulator of a layer lives
-// in TMEM, the epilogue warps turn it (bias, ReLU, fp16 hi/lo split) into the next layer's A operand, again in TMEM
-// (tcgen05.mma with A from tensor memory), and the weights stream through a shared-memory ring filled by the
-// bulk-copy (TMA) engine from an L2-resident, pre-swizzled, schedule-ordered image (nm_program.cu).
+// Fused FlexibleNeRFModel forward on the Hopper tensor cores (sm_90a, wgmma): positional encoding -> all linear layers
+// -> sigma / rgb heads in ONE persistent kernel.  Activations never leave the SM: the fp32 accumulator of a layer lives
+// in the registers of a warpgroup, whose epilogue turns it (bias, ReLU, fp16 hi/lo split) into the next layer's A
+// operand in shared memory (128B-swizzled K-major tiles that wgmma reads through a descriptor), and the weights stream
+// through a shared-memory ring filled by the bulk-copy (TMA) engine from an L2-resident, pre-swizzled,
+// schedule-ordered image (nm_program.cu).
 //
 // Reference semantics: src/nerf/models.py:60-80 (network), src/nerf/modules.py:26-34 (encoding).
 //
 // Arithmetic (NM_PREC_EXACT): every product x*W is evaluated as xh*Wh + xl*Wh + xh*Wl with x = xh + xl, W = Wh + Wl
-// fp16 splits and fp32 accumulation — three kind::f16 MMAs per K-step (SURVEY 7.3.1: 1.5e-6 max-abs on composited
-// RGB against fp32, where plain fp16 gives 3.3e-3).  NM_PREC_FAST issues only xh*Wh.
+// fp16 splits and fp32 accumulation — three f16 MMAs per K-step (SURVEY 7.3.1: 1.5e-6 max-abs on composited RGB
+// against fp32, where plain fp16 gives 3.3e-3).  NM_PREC_FAST issues only xh*Wh.
 //
-// CTA = one 128-point tile at a time (TMEM lane = point), 17 warps:
-//   warps 0-7   epilogue (two sets of 4, one warp per TMEM lane quarter; set s converts accumulator chunks s, s+2):
-//               tcgen05.ld chunk -> +bias, ReLU, heads -> fp16 hi/lo -> tcgen05.st A operand -> zero the chunk
-//   warps 8-11  front-end: fetch/synthesise the NEXT tile's points, positional encoding -> swizzled smem A tiles
-//   warp 12     producer: cp.async.bulk weight stages (16 KB = one 64x64 block, hi|lo) into the ring; TMEM allocator
-//   warps 13-16 MMA issuers: schedule block b is issued by warp (b & 3), all lanes converged, one elected lane
-//               issuing.  Four issuers because one warp sustains only ~1 tcgen05.mma per 100 cycles while an
-//               M=128,N=64,K=16 MMA executes in 32 (tools/umma_bench.cu): four overlap to the execution rate.
-// TMEM (512 columns): [0,256) fp32 accumulator D, [256,384) A_hi, [384,512) A_lo (two fp16 per column).
-// A layer is issued as 64x64 blocks (M=128,N=64,K=16 MMAs) in the order nm_program.cu derives, which lets layer
-// l+1 start as soon as the epilogue has converted the first 64 columns of layer l.  Because blocks of one
-// accumulator chunk come from different issuers (no cross-warp order), every MMA accumulates and the epilogue
-// re-zeroes a chunk after draining it.  mbarriers per layer transition:
-//   d_full[n]      (4 commits)  every issuer is done with accumulator chunk n           -> epilogue may drain it
-//   kb_free[k]     (4 commits)  every issuer is done reading activation K-block k       -> epilogue may overwrite it
-//   chunk_ready[n] (4 arrives)  chunk n drained + zeroed, K-block n of the new layer written -> issuers may use both
+// CTA = 12 warps:
+//   warps 0-3, 4-7  two consumer warpgroups.  Each owns a 64-point tile at a time (its own tile sequence), its own
+//                   activation buffer (4 K-blocks x hi/lo, 64 KB) and encoding buffer (one K-block x hi/lo, 16 KB), and
+//                   walks the layer program: encodings -> for each layer, m64n64k16 wgmmas of every 64x64 weight block
+//                   into register accumulator chunk nc (4 chunks = 128 fp32 registers per thread) -> epilogue straight
+//                   from the accumulator fragments back into the activation buffer.  While one warpgroup runs its
+//                   epilogue the other keeps the tensor cores busy.
+//   warps 8-11      producer: warp 8 issues cp.async.bulk weight stages (16 KB = one 64x64 block, hi|lo) into the ring.  Both
+//                   warpgroups consume every stage in schedule order; a stage is free once both have released it
+//                   (empty barrier count 2), so one L2 read of the weights feeds 128 points.
+// The view-direction encoding reuses the encoding buffer: every layer that reads the xyz encoding precedes the one that
+// reads the directions (checked at launch).
 //
-// Round 2 (DESIGN.md 4.1, 4.4):
-//   * three template modes — 0 inference; 1 training forward, whose epilogue also emits the backward's operands (relu bit
-//     masks, head activations, point-major bf16 hi/lo packs); 2 the whole data-gradient chain of the backward on a backward
-//     layer program (dZ as the A operand in TMEM, W^T streamed through the ring, MN-major packs out through per-warp bulk
-//     stores, register file re-divided with setmaxnreg)
-//   * mode 0 on ray inputs composites in the kernel: the last layer's (rgb, sigma) go to the front-end warps through shared
-//     memory (raw_full / raw_empty), which run VolumeRenderer per ray in sample order (nm_composite.cuh) — tiles are dealt in
-//     ray-aligned groups and a carry slot passes the ray cut by a tile edge to the next tile
-//   * CTA pairs (cluster of 2) share ONE weight stream: rank 0 multicasts every stage into both rings, a stage is released
-//     by multicast commits of both CTAs' issuers (w_empty counts 2), rank 1 runs ghost iterations when it has no tile
+// Three template modes — 0 inference; 1 training forward, whose epilogue also emits the backward's operands (relu bit
+// masks, head activations, point-major bf16 hi/lo packs); 2 the whole data-gradient chain of the backward on a backward
+// layer program (dZ as the A operand, W^T streamed through the ring, bf16 hi/lo).  Mode 0 on ray inputs composites in
+// the kernel: the warpgroup runs VolumeRenderer per ray in sample order (nm_composite.cuh) on its tile's staged outputs;
+// tiles are dealt in ray-aligned groups and a carry slot passes the ray cut by a tile edge to the next tile.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -53,19 +45,16 @@ namespace nm {
 
 namespace {
 
-constexpr int kThreads = 544;
-constexpr int kEpiWarps = 8;
-constexpr int kFeWarp0 = 8;
-constexpr int kProdWarp = 12;
-constexpr int kMmaWarp0 = 13;
-constexpr uint32_t kPeTile = 16384;      // 128 rows x 128 B
-constexpr uint32_t kPeBuf = 2 * kPeTile;  // one xyz encoding buffer: hi, lo (double-buffered: needed at the START of a tile)
-constexpr uint32_t kPeTotal = 3 * kPeBuf; // + one single-buffered view-direction buffer (needed only by the LAST layer)
-constexpr uint32_t kColAhi = 256, kColAlo = 384;
+constexpr int kThreads = 384;
+constexpr int kProdWarp = 8;                       // warps 8-11: the producer warpgroup (warp 8 issues, 9-11 only lend registers)
+constexpr uint32_t kKBlock = 2 * 8192;             // one K-block of a 64-point tile: [hi 64 rows x 128 B | lo]
+constexpr uint32_t kActBytes = 4 * kKBlock;        // activation buffer of one warpgroup (K up to 256)
+constexpr uint32_t kWgBytes = kActBytes + kKBlock; // + its encoding buffer
 constexpr int kMaxStages = 8;
+constexpr uint32_t kCompBytes = 64 * 16 + 64 * 4 + 64 * 4 + 64;   // per warpgroup: staged q / products, keep / T, weights, carry slots
 
 struct TcParams {
-  NetProgram net;   // by value: lives in the constant bank, so the issuer warps index it with uniform registers
+  NetProgram net;   // by value: lives in the constant bank
   const uint8_t* wpack;
   const float* bias;
   const float* head;
@@ -77,9 +66,7 @@ struct TcParams {
   int num_stages;
   long long n_tiles;
   int* err;
-  unsigned long long* trace;   // NM_TC_TRACE: CTA 0 logs (kind, id, index, layer, t0..t3) records; trace[0] = count
-  int dbg;   // bring-up switches (env NM_TC_DEBUG): 1 = no MMA issue, 2 = no epilogue math, 4 = no weight copies
-  uint32_t off_pe, off_bias, off_head, off_red, off_bars;
+  uint32_t off_wg, off_bias, off_head, off_bars, off_comp;
   int has_emit;     // training: the epilogue also writes the backward pass's operands (MlpEmit)
   MlpEmit emit;
   // mode 2: the data-gradient chain of the training backward (a KIND_LOAD / KIND_BWD program, W^T stages in bf16 hi/lo):
@@ -88,27 +75,19 @@ struct TcParams {
   const float* dz_in;     // (M, dz_ld) fp32: dZ of the last forward layer
   int dz_ld;
   const float* dout;      // (M, 4): compositor adjoint, column 3 = d sigma
-  int fe_emit;            // mode 1, K-major packs: the front-end warps emit the packs of accumulator chunks 2 and 3 (emit_done barriers)
-  int cluster;            // 2: CTAs 2p, 2p+1 form a cluster that shares ONE weight stream (rank 0 multicasts every stage into both)
-  int emit_mn;            // modes 1 / 2: packs as MN-major tiles, written by per-warp bulk stores from a shared-memory staging block
-  uint32_t off_stg;       //   its eight 8 KB blocks: the (unused) encoding buffers in mode 2, an own region in mode 1
-  // fused compositor (mode 0, ray inputs): the last layer's (rgb, sigma) of a tile go to the front-end warps through shared
-  // memory instead of to `out`; they composite every ray in sample order (nm_composite.cuh) and write the per-ray maps.
+  int emit_mn;            // modes 1 / 2: packs as MN-major tiles instead of K-major ones
+  // fused compositor (mode 0, ray inputs): the last layer's (rgb, sigma) of a tile are staged in shared memory instead of
+  // going to `out`; the warpgroup composites every ray in sample order (nm_composite.cuh) and writes the per-ray maps.
   int comp_on;
-  int tile_group;         // tiles per scheduling group = lcm(S, 128) / 128 when compositing (rays never straddle groups), else 1
-  uint32_t off_comp;      // shared memory of the fused compositor (kCompBytes)
+  int tile_group;         // tiles per scheduling group = lcm(S, 64) / 64 when compositing (rays never straddle groups), else 1
   CompositeArgs comp;
 };
 static_assert(sizeof(TcParams) <= 4096, "TcParams must fit the 4 KB kernel-parameter window");
 
 // barrier slots (8 B each) relative to off_bars
-constexpr uint32_t kBarWFull = 0, kBarWEmpty = 64, kBarPeFull = 128, kBarPeEmpty = 144, kBarChunk = 160,
-                   kBarDFull = 192, kBarKbFree = 224, kTmemPtr = 256, kLoadedCnt = 264, kBarDirFull = 272, kBarDirEmpty = 280,
-                   kBarRawFull = 288, kBarRawEmpty = 296, kBarEmitDone = 304 /* [2] */, kBarBytes = 320;
-constexpr uint32_t kCompBytes = 128 * 16 + 128 * 4 + 128 * 4 + 64;   // staged q / products, keep / T, weights, two carry slots
+constexpr uint32_t kBarWFull = 0, kBarWEmpty = 64, kBarBytes = 128;
 
-enum : int { ERR_ALIGN = 1, ERR_W_EMPTY = 2, ERR_W_FULL = 3, ERR_PE_FULL = 4, ERR_PE_EMPTY = 5, ERR_CHUNK = 6,
-             ERR_DFULL = 7, ERR_KBFREE = 8, ERR_RAW = 9 };
+enum : int { ERR_ALIGN = 1, ERR_W_EMPTY = 2, ERR_W_FULL = 3 };
 
 __device__ __forceinline__ uint16_t f16_bits_sat(float a) {
   uint16_t h;
@@ -120,20 +99,32 @@ __device__ __forceinline__ float f16_bits_to_float(uint16_t h) {
   asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"(h));
   return f;
 }
-// Event log of CTA 0 (NM_TC_TRACE).  Six writers (4 issuers, 2 epilogue sets) own disjoint regions and keep their own
-// cursor, so a record is five fire-and-forget global stores — no atomics, negligible perturbation.
-constexpr int kTraceRegion = 10000;
-__device__ __forceinline__ void trace_rec(const TcParams& P, unsigned kind, unsigned id, unsigned idx, unsigned gl, long long t0,
-                                          long long t1, long long t2, long long t3, unsigned& cursor) {
-  if (!P.trace || blockIdx.x != 0 || cursor >= (unsigned)kTraceRegion) return;
-  const unsigned region = (kind == 1 ? 0u : 4u) + id;
-  unsigned long long* r = P.trace + 1 + ((unsigned long long)region * kTraceRegion + cursor) * 5;
-  r[0] = ((unsigned long long)kind << 48) | ((unsigned long long)id << 40) | ((unsigned long long)idx << 24) | gl;
-  r[1] = (unsigned long long)t0; r[2] = (unsigned long long)t1; r[3] = (unsigned long long)t2; r[4] = (unsigned long long)t3;
-  ++cursor;
-}
 __device__ __forceinline__ uint32_t swz_off(int r, int c) {
   return (uint32_t)r * 128u + (uint32_t)((((c >> 3) ^ (r & 7)) << 4) + ((c & 7) << 1));
+}
+__device__ __forceinline__ void split_bf16x2(float a0, float a1, uint32_t* hi, uint32_t* lo) {
+  const __nv_bfloat162 h2 = __floats2bfloat162_rn(a0, a1);
+  const float2 f = __bfloat1622float2(h2);
+  const __nv_bfloat162 l2 = __floats2bfloat162_rn(a0 - f.x, a1 - f.y);
+  *hi = *reinterpret_cast<const uint32_t*>(&h2);
+  *lo = *reinterpret_cast<const uint32_t*>(&l2);
+}
+
+// One 64x64 weight block: ksteps K=16 steps of every pass (exact: a_hi*b_hi, a_lo*b_hi, a_hi*b_lo) into chunk d.
+template <int BF16>
+__device__ __forceinline__ void mma_block(float* d, uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo, int ksteps,
+                                          int n_passes) {
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    if (k < ksteps) ptx::wgmma_m64n64<0, 0, BF16>(d, a_hi + 2 * k, b_hi + 2 * k, 1u);
+  if (n_passes == 3) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      if (k < ksteps) ptx::wgmma_m64n64<0, 0, BF16>(d, a_lo + 2 * k, b_hi + 2 * k, 1u);
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      if (k < ksteps) ptx::wgmma_m64n64<0, 0, BF16>(d, a_hi + 2 * k, b_lo + 2 * k, 1u);
+  }
 }
 
 // MODE 0: inference; 1: training forward (the epilogue also emits the backward's operands); 2: data-gradient chain
@@ -141,795 +132,429 @@ template <int MODE>
 __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_constant__ TcParams P) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const uint32_t sbase = ptx::smem_u32(smem);
-  // broadcast from lane 0 so the compiler can prove the role / issuer index warp-uniform (uniform datapath, UR operands)
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   const uint32_t bars = sbase + P.off_bars;
   const int NS = P.num_stages;
   float* s_bias = reinterpret_cast<float*>(smem + P.off_bias);
   float* s_head = reinterpret_cast<float*>(smem + P.off_head);
-  float* s_red = reinterpret_cast<float*>(smem + P.off_red);   // [128] sigma partials, then [128][4]
   const int n_layers = P.net.n_layers, n_blocks = P.net.n_blocks;
 
   // ---------------------------------------------------------------- one-time setup
   if (threadIdx.x == 0) {
     if (sbase & 1023u) { atomicExch(P.err, ERR_ALIGN); __trap(); }
-    // a weight stage is released by its consuming issuer of EVERY CTA of the cluster (multicast commits): count = cluster size
-    for (int i = 0; i < kMaxStages; ++i) { ptx::mbar_init(bars + kBarWFull + 8 * i, 1); ptx::mbar_init(bars + kBarWEmpty + 8 * i, P.cluster == 2 ? 2 : 1); }
-    for (int i = 0; i < 2; ++i) { ptx::mbar_init(bars + kBarPeFull + 8 * i, 128); ptx::mbar_init(bars + kBarPeEmpty + 8 * i, kIssuers); }
-    ptx::mbar_init(bars + kBarDirFull, 128);
-    ptx::mbar_init(bars + kBarDirEmpty, kIssuers);
-    ptx::mbar_init(bars + kBarRawFull, 128);
-    ptx::mbar_init(bars + kBarRawEmpty, 1);
-    ptx::mbar_init(bars + kBarEmitDone, 4);
-    ptx::mbar_init(bars + kBarEmitDone + 8, 4);
-    for (int i = 0; i < 4; ++i) {
-      ptx::mbar_init(bars + kBarChunk + 8 * i, 4);
-      ptx::mbar_init(bars + kBarDFull + 8 * i, kIssuers);
-      ptx::mbar_init(bars + kBarKbFree + 8 * i, kIssuers);
-    }
-    *reinterpret_cast<volatile uint32_t*>(smem + P.off_bars + kLoadedCnt) = 0u;
+    for (int i = 0; i < kMaxStages; ++i) { ptx::mbar_init(bars + kBarWFull + 8 * i, 1); ptx::mbar_init(bars + kBarWEmpty + 8 * i, 2); }
     ptx::fence_mbar_init();
   }
-  {
-    uint4* z = reinterpret_cast<uint4*>(smem + P.off_pe);
-    for (int i = threadIdx.x; i < (int)(kPeTotal / 16); i += kThreads) z[i] = make_uint4(0, 0, 0, 0);
-    for (int i = threadIdx.x; i < P.net.n_bias; i += kThreads) s_bias[i] = (MODE == 2) ? 0.f : P.bias[i];
-    for (int i = threadIdx.x; i < P.net.n_head; i += kThreads) s_head[i] = P.head[i];
-  }
-  ptx::fence_proxy_async_smem();
-  if (warp == kProdWarp) {
-    ptx::tmem_alloc(bars + kTmemPtr, 512);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
+  for (int i = threadIdx.x; i < P.net.n_bias; i += kThreads) s_bias[i] = (MODE == 2) ? 0.f : P.bias[i];
+  for (int i = threadIdx.x; i < P.net.n_head; i += kThreads) s_head[i] = P.head[i];
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem = *reinterpret_cast<volatile uint32_t*>(smem + P.off_bars + kTmemPtr);
-  if (threadIdx.x == 0 && tmem != 0u) { atomicExch(P.err, ERR_ALIGN + 10); __trap(); }   // a 512-column allocation starts at 0
-  if (warp < kEpiWarps && P.net.accumulate_only) {   // all MMAs accumulate: start from a zero accumulator
-    uint32_t z[16];
-#pragma unroll
-    for (int j = 0; j < 16; ++j) z[j] = 0u;
-    const uint32_t base = tmem + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)((warp >> 2) * 128);
-#pragma unroll
-    for (int c = 0; c < 8; ++c) NM_TMEM_ST16(base + 16u * c, z);
-    ptx::tmem_wait_st();
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  ptx::tc_fence_after();
 
-  const float so = P.act_scale, si = P.act_inv_scale;
-  const int n_passes = P.n_passes;
-  // i-th tile of this CTA: groups of `tile_group` consecutive tiles are dealt round-robin to the CTAs (group size 1: the plain
-  // strided order).  Returns -1 past the end.  In a cluster of two both CTAs must walk the weight ring the same number of
-  // times: iter_exists(i) is decided by rank 0's tile, and rank 1 runs a "ghost" iteration (ring traffic only) when its own
-  // tile of that round does not exist — which can only be its last one.
-  const uint32_t Gt = (uint32_t)P.tile_group;
-  const bool cl2 = P.cluster == 2;
-  const uint32_t crank = cl2 ? (blockIdx.x & 1u) : 0u;     // == %cluster_ctarank for cluster dims (2,1,1); from blockIdx it stays on the uniform datapath
-  auto tile_of = [&](uint32_t i) -> long long {
-    const long long g = (long long)blockIdx.x + (long long)(i / Gt) * (long long)gridDim.x;     // blockIdx.x = 2 * pair + rank
+  // i-th tile of worker v (two workers per CTA, one per consumer warpgroup): groups of `tile_group` consecutive tiles are
+  // dealt round-robin to the workers.  Returns -1 past the end.  Both warpgroups walk the weight ring the same number of
+  // times: iteration i exists when worker 2 * blockIdx.x (the lower one) has a tile; warpgroup 1 runs a "ghost" iteration
+  // (ring traffic only) when its own tile of that round does not exist — which can only be its last one.
+  const uint32_t Gt = (uint32_t)P.tile_group, V = 2u * gridDim.x, v0 = 2u * blockIdx.x;
+  auto tile_of = [&](uint32_t v, uint32_t i) -> long long {
+    const long long g = (long long)v + (long long)(i / Gt) * (long long)V;
     const long long t = g * (long long)Gt + (long long)(i % Gt);
     return t < P.n_tiles ? t : -1;
   };
-  auto iter_exists = [&](uint32_t i) -> bool {
-    const long long g0 = (long long)(blockIdx.x - crank) + (long long)(i / Gt) * (long long)gridDim.x;
-    return g0 * (long long)Gt + (long long)(i % Gt) < P.n_tiles;
-  };
-  if (cl2) ptx::cluster_sync_all();              // the peer's barriers are initialised before anything is multicast at them
 
-  // K-major pack emission of accumulator chunk n of layer li for the 32 rows of TMEM lane quarter `lq` (this warp's quarter):
-  // the values are read back from the A operand (hi + lo 16-bit halves) and stored as the point-major bf16 hi/lo pack of the
-  // weight-gradient GEMM (rows past M as zeros).  done_bar != 0: arrive there once every TMEM read of the chunk has landed.
-  auto emit_kmajor = [&](int li, int n, long long tile, int lq, uint32_t done_bar) {
-    const uint32_t lane_addr = (uint32_t)(lq * 32) << 16;
-    const long long pt = tile * kTileM + lq * 32 + lane;
-    const bool valid = pt < P.in.M;
-    const uint32_t c8 = (uint32_t)((pt & 63) >> 3);
-#pragma unroll 1
-    for (int half = 0; half < 2; ++half) {
-      uint32_t h16[16], l16[16];
-      const uint32_t acol = (uint32_t)(n * 32 + half * 16);
-      NM_TMEM_LD16(tmem + lane_addr + kColAhi + acol, h16);
-      if (n_passes == 3) NM_TMEM_LD16(tmem + lane_addr + kColAlo + acol, l16);
-      ptx::tmem_wait_ld();
-      if (half == 1 && done_bar) {
-        ptx::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(done_bar);
-      }
-      const int col0 = n * 64 + half * 32;
-      if (!valid) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) { h16[j] = 0u; l16[j] = 0u; }
-      } else if (n_passes != 3) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) l16[j] = 0u;
-      }
-      // element (feature f, point pt) of a tile: row f%128, 16-byte chunk ((pt%64)/8) ^ (f%8), 2-byte slot pt%8; col0 is a
-      // multiple of 32, so f%8 = j%8: one base address per (feature % 8), immediates for the rest; features 2j, 2j+1 = register j
-      uint8_t* tb = P.emit.packT[li] + ((size_t)(col0 >> 7) * (size_t)P.emit.kbt + (size_t)(pt >> 6)) * 32768u +
-                    (size_t)(col0 & 127) * 128u + (size_t)(pt & 7) * 2u;
-#pragma unroll
-      for (int q8 = 0; q8 < 8; ++q8) {
-        uint8_t* bq = tb + ((c8 ^ (uint32_t)q8) << 4);
-#pragma unroll
-        for (int rr = 0; rr < 4; ++rr) {
-          const int f = q8 + 8 * rr, j = f >> 1, odd = f & 1;
-          uint16_t oh, ol;
-          if (MODE == 2) {        // already bf16 hi / lo
-            oh = (uint16_t)(odd ? (h16[j] >> 16) : (h16[j] & 0xffffu));
-            ol = (uint16_t)(odd ? (l16[j] >> 16) : (l16[j] & 0xffffu));
-          } else {                // fp16 hi + lo (22 bits) -> bf16 hi / lo
-            const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(&h16[j]));
-            const float2 fl = __half22float2(*reinterpret_cast<const __half2*>(&l16[j]));
-            const float x = ((odd ? fh.y : fh.x) + (odd ? fl.y : fl.x)) * so;
-            const __nv_bfloat16 b0 = __float2bfloat16_rn(x);
-            oh = __bfloat16_as_ushort(b0);
-            ol = __bfloat16_as_ushort(__float2bfloat16_rn(x - __bfloat162float(b0)));
-          }
-          *reinterpret_cast<uint16_t*>(bq + f * 128) = oh;
-          *reinterpret_cast<uint16_t*>(bq + f * 128 + 16384) = ol;
-        }
-      }
-    }
-  };
-
-  // Mode 2 (data-gradient chain): the epilogue holds a 32-column slab, its bf16 hi/lo halves and the mask at once and spilled
-  // under the 96-register launch budget (17 warps: one SM sub-partition hosts five).  Its front-end warps are idle and the
-  // issuers are light, so the register file is re-divided per warpgroup: per sub-partition 2 x 160 (epilogue) + 24 (front
-  // end) + 40 (producer / issuer) [+ 96 for the 17th warp, which is in no complete warpgroup] = the 4 (5) x 96 it was given.
-  if (MODE == 2) {
-    if (warp < kEpiWarps) asm volatile("setmaxnreg.inc.sync.aligned.u32 160;");
-    else if (warp < kProdWarp) asm volatile("setmaxnreg.dec.sync.aligned.u32 24;");
-    else if (warp < kProdWarp + 4) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-  }
-  if (warp < kEpiWarps) {
-    // =============================================================== epilogue warps
-    const int q = warp & 3, hcol = warp >> 2;
-    const int row = q * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-    const bool acc_only = P.net.accumulate_only != 0;
-    uint32_t gl = 0;
-    unsigned trace_cursor = 0;
-    float sigma_val = 0.f;
-    for (uint32_t it = 0;; ++it) {
-      const long long tile = tile_of(it);
-      if (tile < 0) break;
-      const long long m = tile * kTileM + row;
-      for (int li = 0; li < n_layers; ++li, ++gl) {
-        const LayerProg& L = P.net.layers[li];
-        const int NC = L.n_out >> 6;
-        const bool writes_a = (L.kind == KIND_HIDDEN) || (L.kind == KIND_SIGMA && !L.is_final) || (L.kind == KIND_LOAD) ||
-                              (L.kind == KIND_BWD && !L.is_final);
-        constexpr bool bwd = MODE == 2;
-        const int heads = L.kind == KIND_SIGMA ? 1 : (L.kind == KIND_RGB ? 3 : (L.kind == KIND_OUT4 ? 4 : 0));
-        float part[4] = {0.f, 0.f, 0.f, 0.f};
-        // Warp set `hcol` (warps 4*hcol..4*hcol+3, one per TMEM lane quarter) owns accumulator chunks hcol and hcol+2:
-        // the two sets convert neighbouring chunks concurrently, so the commit -> wake -> convert -> arrive latency of
-        // one chunk overlaps the next chunk's instead of adding to it.
-        for (int nn = 0; nn < 2; ++nn) {
-          const int n = hcol + 2 * nn;
-          // mode 2: the relu mask words (and d sigma) of this chunk come from HBM / L2 — issue the loads BEFORE waiting for the
-          // accumulator, so that their latency hides behind the MMAs instead of sitting on the chunk's conversion path
-          uint32_t mk_pre[2] = {0xffffffffu, 0xffffffffu};
-          float dsg_pre = 0.f;
-          if (MODE == 2 && L.kind == KIND_BWD && n < NC && m < P.in.M) {
-            if (L.relu) {
-              const uint2 bw = *reinterpret_cast<const uint2*>(P.emit.bits[li] + (size_t)m * (size_t)(L.n_out >> 5) + (size_t)(n * 2));
-              mk_pre[0] = bw.x; mk_pre[1] = bw.y;       // n_out is a multiple of 64: the two words of a chunk are 8-byte aligned
-            }
-            if (L.aux2) dsg_pre = P.dout[(size_t)m * 4 + 3];
-          }
-          const long long tr0 = P.trace ? clock64() : 0;
-          ptx::mbar_wait(bars + kBarDFull + 8 * n, gl & 1, P.err, ERR_DFULL);
-          const long long tr1 = P.trace ? clock64() : 0;
-          long long tr2 = 0;
-          if (n < NC && !(P.dbg & 2)) {
-            ptx::tc_fence_after();
-#pragma unroll 1
-            for (int half = 0; half < 2; ++half) {
-              uint32_t r[32];
-              const int col0 = n * 64 + half * 32;
-              float v[32];
-              if (MODE == 2 && L.kind == KIND_LOAD) {
-                // top of the data-gradient chain: dZ of the last forward layer, from HBM (rows past M are zero)
-                const bool valid = m < P.in.M;
-                const float4* src = reinterpret_cast<const float4*>(P.dz_in + (size_t)(valid ? m : 0) * P.dz_ld + col0);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  const float4 x = valid ? src[j] : make_float4(0.f, 0.f, 0.f, 0.f);
-                  v[4 * j] = x.x; v[4 * j + 1] = x.y; v[4 * j + 2] = x.z; v[4 * j + 3] = x.w;
-                }
-              } else {
-                NM_TMEM_LD32(tmem + lane_addr + (uint32_t)col0, r);
-                ptx::tmem_wait_ld();
-              }
-              if (MODE == 2 && L.kind == KIND_BWD) {
-                // dA = dZ W (+ d sigma * w_alpha), masked by relu' of the forward layer below.  (Its column sums — the bias
-                // gradient — are taken by the weight-gradient GEMM from the pack emitted below: nm_gemm_tc.cu a_rowsum.)
-                const bool valid = m < P.in.M;
-#pragma unroll
-                for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) * so;
-                if (L.aux2) {
-                  const float dsg = valid ? dsg_pre : 0.f;
-                  const float4* w4 = reinterpret_cast<const float4*>(s_head + L.head_off + col0);
-#pragma unroll
-                  for (int j = 0; j < 8; ++j) {
-                    const float4 ww = w4[j];
-                    v[4 * j + 0] = fmaf(dsg, ww.x, v[4 * j + 0]); v[4 * j + 1] = fmaf(dsg, ww.y, v[4 * j + 1]);
-                    v[4 * j + 2] = fmaf(dsg, ww.z, v[4 * j + 2]); v[4 * j + 3] = fmaf(dsg, ww.w, v[4 * j + 3]);
-                  }
-                }
-                const uint32_t mk = valid ? (half ? mk_pre[1] : mk_pre[0]) : 0u;
-#pragma unroll
-                for (int j = 0; j < 32; ++j) v[j] = ((mk >> j) & 1u) ? v[j] : 0.f;
-              } else if (MODE != 2 || L.kind != KIND_LOAD) {
-                const float4* b4 = reinterpret_cast<const float4*>(s_bias + L.bias_off + col0);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  const float4 bb = b4[j];
-                  v[4 * j + 0] = fmaf(__uint_as_float(r[4 * j + 0]), so, bb.x);
-                  v[4 * j + 1] = fmaf(__uint_as_float(r[4 * j + 1]), so, bb.y);
-                  v[4 * j + 2] = fmaf(__uint_as_float(r[4 * j + 2]), so, bb.z);
-                  v[4 * j + 3] = fmaf(__uint_as_float(r[4 * j + 3]), so, bb.w);
-                }
-                if (L.relu) {
-#pragma unroll
-                  for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-                }
-              }
-              for (int hh = 0; hh < heads; ++hh) {
-                const float4* w4 = reinterpret_cast<const float4*>(s_head + L.head_off + hh * L.n_out + col0);
-                float acc = part[hh];
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  const float4 ww = w4[j];
-                  acc = fmaf(ww.x, v[4 * j + 0], acc);
-                  acc = fmaf(ww.y, v[4 * j + 1], acc);
-                  acc = fmaf(ww.z, v[4 * j + 2], acc);
-                  acc = fmaf(ww.w, v[4 * j + 3], acc);
-                }
-                part[hh] = acc;
-              }
-              if (MODE >= 1) {
-                // by-products for the training backward: relu mask, fp32 copy (layers the head kernels read) and the
-                // point-major bf16 hi/lo pack the weight-gradient GEMM consumes (rows past M are written as zeros)
-                const bool valid = m < P.in.M;
-                if (!bwd && P.emit.bits[li] && valid) {
-                  uint32_t mk = 0;
-#pragma unroll
-                  for (int j = 0; j < 32; ++j) mk |= (v[j] > 0.f ? 1u : 0u) << j;
-                  P.emit.bits[li][(size_t)m * (size_t)(L.n_out >> 5) + (size_t)(col0 >> 5)] = mk;
-                }
-                if (!bwd && P.emit.act[li] && valid) {
-                  float4* dst = reinterpret_cast<float4*>(P.emit.act[li] + (size_t)m * L.n_out + col0);
-#pragma unroll
-                  for (int j = 0; j < 8; ++j) dst[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                }
-                if (MODE == 2 && P.emit_mn && P.emit.packT[li] && !writes_a) {
-                  // the chain's last layer (no A operand to read back): the same MN-major staging block as below, filled half
-                  // by half from the registers; the bulk stores follow the second half
-                  uint8_t* stg = smem + P.off_stg + (uint32_t)warp * 8192u;
-                  if (half == 0) {
-                    if (lane == 0) ptx::bulk_wait_group_read0();
-                    __syncwarp();
-                  }
-#pragma unroll
-                  for (int c = 0; c < 4; ++c) {
-                    uint32_t h4[4], l4[4];
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                      const float x0 = valid ? v[c * 8 + 2 * e] : 0.f, x1 = valid ? v[c * 8 + 2 * e + 1] : 0.f;
-                      const __nv_bfloat162 h2 = __floats2bfloat162_rn(x0, x1);
-                      const float2 f = __bfloat1622float2(h2);
-                      const __nv_bfloat162 l2 = __floats2bfloat162_rn(x0 - f.x, x1 - f.y);
-                      h4[e] = *reinterpret_cast<const uint32_t*>(&h2);
-                      l4[e] = *reinterpret_cast<const uint32_t*>(&l2);
-                    }
-                    const uint32_t off = (uint32_t)lane * 128u + ((((uint32_t)(half * 4 + c)) ^ ((uint32_t)lane & 7u)) << 4);
-                    *reinterpret_cast<uint4*>(stg + off) = make_uint4(h4[0], h4[1], h4[2], h4[3]);
-                    *reinterpret_cast<uint4*>(stg + 4096u + off) = make_uint4(l4[0], l4[1], l4[2], l4[3]);
-                  }
-                  if (half == 1) {
-                    ptx::fence_proxy_async_smem();
-                    __syncwarp();
-                    if (lane == 0) {
-                      uint8_t* dst = P.emit.packT[li] + ((size_t)(n >> 1) * (size_t)P.emit.kbt + (size_t)(tile * 2 + (q >> 1))) * 32768u +
-                                     (size_t)(n & 1) * 8192u + (size_t)((q & 1) * 32) * 128u;
-                      ptx::bulk_s2g(dst, ptx::smem_u32(stg), 4096u);
-                      ptx::bulk_s2g(dst + 16384u, ptx::smem_u32(stg) + 4096u, 4096u);
-                      ptx::bulk_commit_group();
-                    }
-                  }
-                } else if (P.emit.packT[li] && !writes_a) {     // (layers that write the A operand emit from it after the hand-over, below)
-                  const long long pt = tile * kTileM + row;
-                  // element (feature f, point pt) of a tile: row f%128, 16-byte chunk ((pt%64)/8) ^ (f%8), 2-byte slot pt%8.
-                  // col0 is a multiple of 32, so f%8 = j%8: one base address per j%8, the rest are immediates
-                  uint8_t* tb = P.emit.packT[li] + ((size_t)(col0 >> 7) * (size_t)P.emit.kbt + (size_t)(pt >> 6)) * 32768u +
-                                (size_t)(col0 & 127) * 128u + (size_t)(pt & 7) * 2u;
-                  const uint32_t c8 = (uint32_t)((pt & 63) >> 3);
-#pragma unroll
-                  for (int q = 0; q < 8; ++q) {
-                    uint8_t* bq = tb + ((c8 ^ (uint32_t)q) << 4);
-#pragma unroll
-                    for (int rr = 0; rr < 4; ++rr) {
-                      const int j = q + 8 * rr;
-                      const float x = valid ? v[j] : 0.f;
-                      const __nv_bfloat16 h = __float2bfloat16_rn(x);
-                      const __nv_bfloat16 l = __float2bfloat16_rn(x - __bfloat162float(h));
-                      *reinterpret_cast<uint16_t*>(bq + j * 128) = __bfloat16_as_ushort(h);
-                      *reinterpret_cast<uint16_t*>(bq + j * 128 + 16384) = __bfloat16_as_ushort(l);
-                    }
-                  }
-                }
-              }
-              if (writes_a) {
-                uint32_t hi[16], lo[16];
-                if (bwd) {     // gradients: bf16 hi/lo (fp32's exponent range)
-#pragma unroll
-                  for (int j = 0; j < 16; ++j) {
-                    const float a0 = v[2 * j] * si, a1 = v[2 * j + 1] * si;
-                    const __nv_bfloat162 h2 = __floats2bfloat162_rn(a0, a1);
-                    const float2 f = __bfloat1622float2(h2);
-                    const __nv_bfloat162 l2 = __floats2bfloat162_rn(a0 - f.x, a1 - f.y);
-                    hi[j] = *reinterpret_cast<const uint32_t*>(&h2);
-                    lo[j] = *reinterpret_cast<const uint32_t*>(&l2);
-                  }
-                } else {
-#pragma unroll
-                  for (int j = 0; j < 16; ++j) {
-                    const float a0 = v[2 * j] * si, a1 = v[2 * j + 1] * si;
-                    hi[j] = ptx::pack_f16x2_sat(a0, a1);
-                    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hi[j]));
-                    lo[j] = ptx::pack_f16x2_sat(a0 - f.x, a1 - f.y);
-                  }
-                }
-                if (half == 0) {
-                  if (P.trace) tr2 = clock64();
-                  ptx::mbar_wait(bars + kBarKbFree + 8 * n, gl & 1, P.err, ERR_KBFREE);
-                  // ... and the front-end warps are done with the previous layer's contents of this K block (fe_emit: they
-                  // signal emit_done once per layer, emission or not, so that both sides stay within one barrier phase)
-                  if (MODE == 1 && P.fe_emit && nn == 1 && gl > 0)
-                    ptx::mbar_wait(bars + kBarEmitDone + 8 * (n - 2), (gl - 1) & 1, P.err, ERR_RAW);
-                }
-                const uint32_t acol = (uint32_t)(n * 32 + half * 16);
-                NM_TMEM_ST16(tmem + lane_addr + kColAhi + acol, hi);
-                if (n_passes == 3) NM_TMEM_ST16(tmem + lane_addr + kColAlo + acol, lo);
-              }
-            }
-            if (acc_only) {   // hand the chunk back zeroed (issuers only ever accumulate)
-              uint32_t z[16];
-#pragma unroll
-              for (int j = 0; j < 16; ++j) z[j] = 0u;
-#pragma unroll
-              for (int c = 0; c < 4; ++c) NM_TMEM_ST16(tmem + lane_addr + (uint32_t)(n * 64 + 16 * c), z);
-            }
-            ptx::tmem_wait_st();
-          }
-          if (!(n < NC && !(P.dbg & 2) && writes_a)) {
-            ptx::mbar_wait(bars + kBarKbFree + 8 * n, gl & 1, P.err, ERR_KBFREE);
-            if (MODE == 1 && P.fe_emit && nn == 1 && gl > 0)      // no A write in this layer: keep the lockstep with the front end all the same
-              ptx::mbar_wait(bars + kBarEmitDone + 8 * (n - 2), (gl - 1) & 1, P.err, ERR_RAW);
-          }
-          ptx::tc_fence_before();
-          __syncwarp();
-          if (lane == 0) ptx::mbar_arrive(bars + kBarChunk + 8 * n);
-          if (P.trace && (warp & 3) == 0 && lane == 0) trace_rec(P, 2, hcol, n, gl, tr0, tr1, tr2, clock64(), trace_cursor);
-          if (MODE >= 1 && writes_a && n < NC && P.emit.packT[li]) {
-            // Off the critical path: the chunk has been handed back to the issuers; its values are read back from the A operand
-            // this warp has just written (hi + lo 16-bit halves; it stays untouched until this warp's next epilogue of chunk n)
-            // and stored as the point-major bf16 hi/lo pack of the weight-gradient GEMM (rows past M as zeros).
-            const bool valid = m < P.in.M;
-            if (MODE >= 1 && P.emit_mn) {
-              // MN-major pack (ptx::make_mnmajor_sw128_desc: a point's 64 features of a group are one 128-byte line, chunks
-              // XOR-swizzled by the row).  Sixteen-byte global stores from here would touch 32 lines per instruction; instead the
-              // warp lays its 32 rows x 128 B (hi, lo) out in a private shared-memory block — exactly the contiguous 4 KB the rows
-              // occupy in the global tile — and one lane hands each to the bulk-copy engine.  The encoding buffers, unused by
-              // the data-gradient chain, hold the eight 8 KB blocks (mode 1: a region of its own, taken from the weight ring).
-              uint8_t* stg = smem + P.off_stg + (uint32_t)warp * 8192u;
-              if (lane == 0) ptx::bulk_wait_group_read0();          // the previous chunk's stores have drained this block
-              __syncwarp();
-#pragma unroll 1
-              for (int half = 0; half < 2; ++half) {
-                uint32_t h16[16], l16[16];
-                const uint32_t acol = (uint32_t)(n * 32 + half * 16);
-                NM_TMEM_LD16(tmem + lane_addr + kColAhi + acol, h16);
-                if (n_passes == 3) NM_TMEM_LD16(tmem + lane_addr + kColAlo + acol, l16);
-                ptx::tmem_wait_ld();
-                if (!valid) {
-#pragma unroll
-                  for (int j = 0; j < 16; ++j) { h16[j] = 0u; l16[j] = 0u; }
-                } else if (n_passes != 3) {
-#pragma unroll
-                  for (int j = 0; j < 16; ++j) l16[j] = 0u;
-                }
-                if (MODE == 1) {       // fp16 hi + lo (22 bits) -> bf16 hi / lo, two features per register
-#pragma unroll
-                  for (int j = 0; j < 16; ++j) {
-                    const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(&h16[j]));
-                    const float2 fl = __half22float2(*reinterpret_cast<const __half2*>(&l16[j]));
-                    const float x0 = (fh.x + fl.x) * so, x1 = (fh.y + fl.y) * so;
-                    const __nv_bfloat162 h2 = __floats2bfloat162_rn(x0, x1);
-                    const float2 f = __bfloat1622float2(h2);
-                    const __nv_bfloat162 l2 = __floats2bfloat162_rn(x0 - f.x, x1 - f.y);
-                    h16[j] = *reinterpret_cast<const uint32_t*>(&h2);
-                    l16[j] = *reinterpret_cast<const uint32_t*>(&l2);
-                  }
-                }
-#pragma unroll
-                for (int c = 0; c < 4; ++c) {
-                  const uint32_t off = (uint32_t)lane * 128u + ((((uint32_t)(half * 4 + c)) ^ ((uint32_t)lane & 7u)) << 4);
-                  *reinterpret_cast<uint4*>(stg + off) = make_uint4(h16[4 * c], h16[4 * c + 1], h16[4 * c + 2], h16[4 * c + 3]);
-                  *reinterpret_cast<uint4*>(stg + 4096u + off) = make_uint4(l16[4 * c], l16[4 * c + 1], l16[4 * c + 2], l16[4 * c + 3]);
-                }
-              }
-              ptx::fence_proxy_async_smem();
-              __syncwarp();
-              if (lane == 0) {
-                // rows q*32.. of the tile = rows (q&1)*32.. of K block tile*2 + (q>>1); feature block n>>1, feature group n&1
-                uint8_t* dst = P.emit.packT[li] + ((size_t)(n >> 1) * (size_t)P.emit.kbt + (size_t)(tile * 2 + (q >> 1))) * 32768u +
-                               (size_t)(n & 1) * 8192u + (size_t)((q & 1) * 32) * 128u;
-                ptx::bulk_s2g(dst, ptx::smem_u32(stg), 4096u);
-                ptx::bulk_s2g(dst + 16384u, ptx::smem_u32(stg) + 4096u, 4096u);
-                ptx::bulk_commit_group();
-              }
-            } else if (MODE == 1 && P.fe_emit && nn == 1) {
-              // the front-end warp of this lane quarter emits chunk n (2 or 3)
-            } else {
-              emit_kmajor(li, n, tile, q, 0u);
-            }
-          }
-        }
-        if (heads) {
-          // the two chunk sets of a row live in warps w and w+4: combine their partial dot products through smem
-          const float* hb = s_head + L.head_off + heads * L.n_out;
-          if (L.kind == KIND_SIGMA) {
-            if (hcol == 1) s_red[row] = part[0];
-            ptx::named_bar_sync(1, kEpiWarps * 32);
-            if (hcol == 0) {
-              sigma_val = part[0] + s_red[row] + hb[0];
-              if (L.is_final && m < P.in.M && P.out) P.out[m] = sigma_val;   // sigma-only program
-            }
-          } else {
-            float* r4 = s_red + 128 + 4 * row;
-            if (hcol == 1) { r4[0] = part[0]; r4[1] = part[1]; r4[2] = part[2]; r4[3] = part[3]; }
-            ptx::named_bar_sync(2, kEpiWarps * 32);
-            if (hcol == 0 && (P.comp_on || (m < P.in.M && P.out))) {
-              float o[4];
-#pragma unroll
-              for (int hh = 0; hh < 4; ++hh) o[hh] = (hh < heads) ? part[hh] + r4[hh] + hb[hh] : 0.f;
-              const float sg = (L.kind == KIND_RGB) ? sigma_val : o[3];
-              if (P.out_sigma_only) {
-                P.out[m] = sg;
-              } else {
-                float4 res;
-                res.x = 1.f / (1.f + expf(-o[0]));
-                res.y = 1.f / (1.f + expf(-o[1]));
-                res.z = 1.f / (1.f + expf(-o[2]));
-                res.w = sg;
-                if (MODE == 0 && P.comp_on) {
-                  // hand the tile's outputs to the front-end warps (single staging block: they are a whole tile ahead of us)
-                  ptx::mbar_wait(bars + kBarRawEmpty, (it & 1) ^ 1, P.err, ERR_RAW);
-                  reinterpret_cast<float4*>(smem + P.off_comp)[row] = res;
-                  ptx::mbar_arrive(bars + kBarRawFull);
-                } else {
-                  reinterpret_cast<float4*>(P.out)[m] = res;
-                }
-              }
-            }
-          }
-        }
-      }
-    }
-    if (MODE >= 1 && lane == 0) ptx::bulk_wait_group0();      // outstanding pack stores (emit_mn) before the block goes away
-  } else if (warp < kProdWarp) {
-    // =============================================================== front-end warps: next tile's encodings
-    const int r = (warp - kFeWarp0) * 32 + lane;
-    const int Lx = P.net.L_xyz, Ld = P.net.L_dir, ix = P.net.inc_xyz, id = P.net.inc_dir;
-    const int has_dir = P.net.uses_dir;
-    const float* fx = P.net.freq_xyz;
-    const float* fd = P.net.freq_dir;
-    // Fused compositor: tile `itp` of this CTA, whose last layer the epilogue has staged in shared memory.  Same arithmetic,
-    // in the same order, as composite_kernel (nm_composite.cuh) — but laid out for few issue slots, because these warps share
-    // their schedulers with the epilogue warps:  A  every thread takes ONE sample: alpha, keep (the exp lives here);
-    // B  one thread per ray segment runs the transmittance product chain through shared memory;  C  every thread: weight,
-    // mask, the four products;  D  one lane per (segment, accumulator) runs the five ordered sums.  The ray cut by the tile's
-    // upper edge leaves T and its partial sums in a carry slot for the next tile (tiles of a group are consecutive in this
-    // CTA and groups start on ray boundaries).
-    auto composite_tile = [&](uint32_t itp) {
-      const long long tp = tile_of(itp);
-      const CompositeArgs& A = P.comp;
-      ptx::mbar_wait(bars + kBarRawFull, itp & 1, P.err, ERR_RAW);
-      float4* stage = reinterpret_cast<float4*>(smem + P.off_comp);            // q per sample, later (w r, w g, w b, w t)
-      float* keepT = reinterpret_cast<float*>(smem + P.off_comp + 2048);       // keep per sample, later T
-      float* wv = keepT + 128;                                                 // weight per sample
-      const float* carry_in = wv + 128 + ((itp & 1) ^ 1) * 8;                  // written by the previous tile
-      float* carry_out = wv + 128 + (itp & 1) * 8;
-      const long long p0 = tp * kTileM, p1 = min(p0 + (long long)kTileM, P.in.M);
-      const int S = A.S;
-      const long long ray_first = p0 / S;
-      const int n_seg = (int)((p1 - 1) / S - ray_first) + 1;
-      // ---- A
-      const long long p = p0 + r;
-      const bool live = p < p1;
-      float tc = 0.f, alpha = 0.f;
-      float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (live) {
-        const long long ray = p / S;
-        const int i = (int)(p - ray * S);
-        const float* tr = A.t + ray * S;
-        tc = tr[i];
-        const float tn = (i + 1 < S) ? tr[i + 1] : 0.f;
-        q = stage[r];
-        float keep;
-        alpha = comp_alpha(A, ray, i, tc, tn, comp_ray_norm(A.dirs, ray), q.w, &keep);
-        keepT[r] = keep;
-      }
-      ptx::named_bar_sync(3, 128);
-      // ---- B
-      for (int k = r; k < n_seg; k += 128) {
-        const long long rayk = ray_first + k;
-        const long long s0 = max(rayk * (long long)S, p0), s1 = min((rayk + 1) * (long long)S, p1);
-        float T = (s0 > rayk * (long long)S) ? carry_in[0] : 1.0f;
-        for (int j = (int)(s0 - p0); j < (int)(s1 - p0); ++j) { const float kp = keepT[j]; keepT[j] = T; T = __fmul_rn(T, kp); }
-        if (s1 < (rayk + 1) * (long long)S) carry_out[0] = T;
-      }
-      ptx::named_bar_sync(3, 128);
-      // ---- C
-      if (live) {
-        const float T = keepT[r];
-        const float w = __fmul_rn(alpha, T);
-        if (A.weights) A.weights[p] = w;
-        if (A.mask_weights) A.mask_weights[p] = (T > A.thr) ? 1.f : 0.f;
-        wv[r] = w;
-        stage[r] = make_float4(__fmul_rn(w, q.x), __fmul_rn(w, q.y), __fmul_rn(w, q.z), __fmul_rn(w, tc));
-      }
-      ptx::named_bar_sync(3, 128);
-      // ---- D: lane c of an 8-lane group owns accumulator c (r, g, b, acc, depth) of the group's segment
-      for (int k0 = 0; k0 < n_seg; k0 += 16) {
-        const int k = k0 + (r >> 3), c = r & 7;
-        const long long rayk = ray_first + k;
-        const long long s0 = max(rayk * (long long)S, p0), s1 = min((rayk + 1) * (long long)S, p1);
-        const bool act = k < n_seg && c < 5;
-        float sum = 0.f;
-        if (act) {
-          if (s0 > rayk * (long long)S) sum = carry_in[1 + c];
-          const float* src = (c == 3) ? wv : reinterpret_cast<const float*>(stage) + (c == 4 ? 3 : c);
-          const int stride = (c == 3) ? 1 : 4;
-          for (int j = (int)(s0 - p0); j < (int)(s1 - p0); ++j) sum = __fadd_rn(sum, src[j * stride]);
-        }
-        const float s_g = __shfl_down_sync(0xffffffffu, sum, 1), s_b = __shfl_down_sync(0xffffffffu, sum, 2);
-        const float s_a = __shfl_down_sync(0xffffffffu, sum, 3), s_d = __shfl_down_sync(0xffffffffu, sum, 4);
-        if (act && c == 0) {
-          if (s1 == (rayk + 1) * (long long)S) {
-            CompState cs;
-            cs.T = 0.f; cs.r = sum; cs.g = s_g; cs.b = s_b; cs.acc = s_a; cs.depth = s_d;
-            comp_finish(cs, A, rayk);
-          } else {
-            carry_out[1] = sum; carry_out[2] = s_g; carry_out[3] = s_b; carry_out[4] = s_a; carry_out[5] = s_d;
-          }
-        }
-      }
-      ptx::named_bar_sync(3, 128);                 // staging block consumed, carry visible to the next tile
-      if (r == 0) ptx::mbar_arrive(bars + kBarRawEmpty);
-    };
-    // fe_emit (mode 1): these warps are idle for ~95 % of a tile, the epilogue warps are what paces the training forward — so
-    // warp 8+q emits the packs of accumulator chunks 2 and 3 for TMEM lane quarter q, layer by layer, as soon as the epilogue
-    // has written that K block (chunk_ready) and before it overwrites it in the next layer (emit_done)
-    auto fe_emit_tile = [&](uint32_t itp) {
-      const long long tp = tile_of(itp);
-      uint32_t glp = itp * (uint32_t)n_layers;
-      for (int li = 0; li < n_layers; ++li, ++glp) {
-        const LayerProg& L = P.net.layers[li];
-        const bool writes_a = (L.kind == KIND_HIDDEN) || (L.kind == KIND_SIGMA && !L.is_final);
-        const int NC = L.n_out >> 6;
-        for (int n = 2; n < 4; ++n) {
-          // every layer, emission or not: observe chunk_ready and answer with emit_done, so that neither side can run more than
-          // one phase ahead of the other on these one-parity-bit barriers
-          ptx::mbar_wait(bars + kBarChunk + 8 * n, glp & 1, P.err, ERR_CHUNK);
-          if (writes_a && P.emit.packT[li] && n < NC) {
-            ptx::tc_fence_after();
-            emit_kmajor(li, n, tp, warp - kFeWarp0, bars + kBarEmitDone + 8 * (n - 2));
-          } else {
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(bars + kBarEmitDone + 8 * (n - 2));
-          }
-        }
-      }
-    };
-    uint32_t it = 0;
-    for (;; ++it) {
-      const long long tile = tile_of(it);
-      if (tile < 0) break;
-      const uint32_t buf = it & 1;
-      ptx::mbar_wait(bars + kBarPeEmpty + 8 * buf, ((it >> 1) & 1) ^ 1, P.err, ERR_PE_EMPTY);
-      if (MODE == 2) { ptx::mbar_arrive(bars + kBarPeFull + 8 * buf); continue; }   // no encodings in the data-gradient chain
-      long long m = tile * kTileM + r;
-      if (m >= P.in.M) m = P.in.M - 1;
-      float p[3], d[3];
-      fetch_point(P.in, m, p, d);
-      uint8_t* tb = smem + P.off_pe + buf * kPeBuf;
-      auto emit_to = [&](uint8_t* hi_tile, int j, float val) {
-        const float a = val * si;
-        const uint16_t h = f16_bits_sat(a);
-        const uint32_t off = swz_off(r, j);
-        *reinterpret_cast<uint16_t*>(hi_tile + off) = h;
-        *reinterpret_cast<uint16_t*>(hi_tile + kPeTile + off) = f16_bits_sat(a - f16_bits_to_float(h));
-      };
-      positional_encoding(p, Lx, ix, fx, [&](int j, float val) { emit_to(tb, j, val); });
-      ptx::fence_proxy_async_smem();
-      ptx::mbar_arrive(bars + kBarPeFull + 8 * buf);
-      if (MODE == 1 && P.fe_emit && it > 0) fe_emit_tile(it - 1);      // the previous tile is being processed right now
-      if (has_dir) {   // the view-direction tile is free once the previous tile's last layer has read it
-        ptx::mbar_wait(bars + kBarDirEmpty, (it & 1) ^ 1, P.err, ERR_PE_EMPTY);
-        positional_encoding(d, Ld, id, fd, [&](int j, float val) { emit_to(smem + P.off_pe + 2 * kPeBuf, j, val); });
-        ptx::fence_proxy_async_smem();
-        ptx::mbar_arrive(bars + kBarDirFull);
-      }
-      if (MODE == 0 && P.comp_on && it > 0) composite_tile(it - 1);     // the previous tile is finishing while this one starts
-    }
-    if (MODE == 0 && P.comp_on && it > 0) composite_tile(it - 1);
-    if (MODE == 1 && P.fe_emit && it > 0) fe_emit_tile(it - 1);
-  } else if (warp == kProdWarp) {
+  // the register file is re-divided per warpgroup: 2 x 232 for the consumers (128 accumulators each), 40 for the producer
+  if (warp >= kProdWarp) {
     // =============================================================== weight producer
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp == kProdWarp && lane == 0) {
       int slot = 0;
-      uint32_t ph = 0, issued = 0;
-      const uint32_t cnt_addr = bars + kLoadedCnt;
-      const uint32_t bytes = (n_passes == 3) ? (uint32_t)kStageBytes : (uint32_t)kHalfStage;
-      for (uint32_t itile = 0; iter_exists(itile); ++itile) {
+      uint32_t ph = 0;
+      const uint32_t bytes = (P.n_passes == 3) ? (uint32_t)kStageBytes : (uint32_t)kHalfStage;
+      for (uint32_t i = 0; tile_of(v0, i) >= 0; ++i) {
         for (int b = 0; b < n_blocks; ++b) {
           ptx::mbar_wait(bars + kBarWEmpty + 8 * slot, ph ^ 1, P.err, ERR_W_EMPTY);
-          if (P.dbg & 4) {
-            ptx::mbar_arrive(bars + kBarWFull + 8 * slot);
-          } else {
-            // every CTA arms its own barrier; in a cluster rank 0 alone reads L2 and the copy lands in both CTAs (the slot is
-            // free in both: its `empty` barrier counts the consuming issuer of each)
-            ptx::mbar_expect_tx(bars + kBarWFull + 8 * slot, bytes);
-            if (!cl2) ptx::bulk_g2s(sbase + (uint32_t)slot * kStageBytes, P.wpack + (size_t)b * kStageBytes, bytes, bars + kBarWFull + 8 * slot);
-            else if (crank == 0)
-              ptx::bulk_g2s_multicast(sbase + (uint32_t)slot * kStageBytes, P.wpack + (size_t)b * kStageBytes, bytes,
-                                      bars + kBarWFull + 8 * slot, (uint16_t)3);
-          }
-          // Publish how many stages have been armed.  The ring's mbarriers carry one parity bit, and an issuer whose
-          // consecutive blocks are more than NS apart in the schedule could otherwise look at a slot a full round early
-          // and mistake the previous round's completion for its own.
-          ++issued;
-          asm volatile("st.release.cta.shared::cta.u32 [%0], %1;" ::"r"(cnt_addr), "r"(issued) : "memory");
+          ptx::mbar_expect_tx(bars + kBarWFull + 8 * slot, bytes);
+          ptx::bulk_g2s(sbase + (uint32_t)slot * kStageBytes, P.wpack + (size_t)b * kStageBytes, bytes, bars + kBarWFull + 8 * slot);
           if (++slot == NS) { slot = 0; ph ^= 1; }
         }
       }
     }
-  } else {
-    // =============================================================== MMA issuers (4 converged warps)
-    const int w = warp - kMmaWarp0;
-    const uint32_t acc_only = P.net.accumulate_only ? 1u : 0u;
-    const uint32_t idesc = ptx::make_idesc_f16(kTileM, kChunk) | (MODE == 2 ? ((1u << 7) | (1u << 10)) : 0u);   // mode 2: A, B = bf16
-    int slot = 0;
-    uint32_t ph = 0, gl = 0, it = 0, cur_pos = 0;
-    unsigned trace_cursor = 0;
-    const uint32_t cnt_addr = bars + kLoadedCnt;
-    auto release_stage = [&](int sl) {
-      if (cl2) ptx::tc_commit_elect_multicast(bars + kBarWEmpty + 8 * sl, (uint16_t)3);
-      else ptx::tc_commit_elect(bars + kBarWEmpty + 8 * sl);
-    };
-    for (; iter_exists(it); ++it) {
-      if (tile_of(it) < 0) {
-        // ghost iteration (cluster rank 1, last round): no tile of our own, but the peer's producer multicasts this round's
-        // stages into our ring and waits for our release of each — walk our blocks' stages and hand them straight back
-        const uint32_t base_pos = it * (uint32_t)n_blocks;
-        for (int li = 0; li < n_layers; ++li) {
-          const LayerProg& L = P.net.layers[li];
-          const uint32_t fb = ((uint32_t)L.first_blk >> (8 * w)) & 0xFFu;
-          if (fb == 0xFFu) continue;
-          int b = L.blk_begin + (int)fb;
-          while (true) {
-            const BlockProg& B = P.net.blocks[b];
-            const uint32_t gpos = base_pos + (uint32_t)b;
-            slot += (int)(gpos - cur_pos);
-            cur_pos = gpos;
-            while (slot >= NS) { slot -= NS; ph ^= 1; }
-            uint32_t c;
-            do { asm volatile("ld.acquire.cta.shared::cta.u32 %0, [%1];" : "=r"(c) : "r"(cnt_addr) : "memory"); } while (c <= gpos);
-            ptx::mbar_wait(bars + kBarWFull + 8 * slot, ph, P.err, ERR_W_FULL);
-            release_stage(slot);
-            if (!B.next) break;
-            b += (int)B.next;
-          }
-        }
-        continue;
-      }
-      const uint32_t buf = it & 1;
-      ptx::mbar_wait(bars + kBarPeFull + 8 * buf, (it >> 1) & 1, P.err, ERR_PE_FULL);
-      ptx::tc_fence_after();
-      const uint32_t base_pos = it * (uint32_t)n_blocks;
-      const uint32_t pe_base = sbase + P.off_pe + buf * kPeBuf;
-      const uint32_t dir_base = sbase + P.off_pe + 2 * kPeBuf;
-      bool dir_waited = false;
-      for (int li = 0; li < n_layers; ++li, ++gl) {
-        const LayerProg& L = P.net.layers[li];
-        const uint32_t none_d = (uint32_t)L.none_d >> (4 * w), none_k = (uint32_t)L.none_k >> (4 * w);
-        int waited = -1;
-        // Passing group g means the previous layer's chunk g is drained and its K-block g written; it is also the
-        // earliest phase-safe point for this issuer's "nothing to do" commits on index g.
-        auto pass_group = [&](int g) {
-          while (waited < g) {
-            ++waited;
-            if (gl > 0) ptx::mbar_wait(bars + kBarChunk + 8 * waited, (gl - 1) & 1, P.err, ERR_CHUNK);
-            if ((none_d >> waited) & 1u) ptx::tc_commit_elect(bars + kBarDFull + 8 * waited);
-            if ((none_k >> waited) & 1u) ptx::tc_commit_elect(bars + kBarKbFree + 8 * waited);
-          }
-        };
-        // walk this issuer's own blocks of the layer (first_blk, then BlockProg.next): no scan over other issuers' blocks
-        const uint32_t fb = ((uint32_t)L.first_blk >> (8 * w)) & 0xFFu;
-        if (fb != 0xFFu) {
-          int b = L.blk_begin + (int)fb;
-          while (true) {
-            const BlockProg& B = P.net.blocks[b];
-            const uint32_t gpos = base_pos + (uint32_t)b;          // schedule position since kernel start = ring position
-            slot += (int)(gpos - cur_pos);
-            cur_pos = gpos;
-            while (slot >= NS) { slot -= NS; ph ^= 1; }
-            const long long tr0 = P.trace ? clock64() : 0;
-            pass_group((int)B.group);
-            const long long tr1 = P.trace ? clock64() : 0;
-            {   // the producer must have armed this stage for THIS round before its parity means anything
-              uint32_t c;
-              asm volatile("ld.acquire.cta.shared::cta.u32 %0, [%1];" : "=r"(c) : "r"(cnt_addr) : "memory");
-              if (c <= gpos) {
-                const long long t0 = clock64();
-                do {
-                  asm volatile("ld.acquire.cta.shared::cta.u32 %0, [%1];" : "=r"(c) : "r"(cnt_addr) : "memory");
-                  if (c <= gpos && clock64() - t0 > 4000000000LL) { atomicExch(P.err, ERR_W_FULL + 100); __trap(); }
-                } while (c <= gpos);
-              }
-            }
-            ptx::mbar_wait(bars + kBarWFull + 8 * slot, ph, P.err, ERR_W_FULL);
-            const long long tr2 = P.trace ? clock64() : 0;
-            ptx::tc_fence_after();
-            const uint32_t wst = sbase + (uint32_t)slot * kStageBytes;
-            const uint32_t d_t = (uint32_t)B.nc * 64u;            // TMEM base is 0 (checked at start-up)
-            if (!(P.dbg & 1)) {
-              const uint64_t b_hi = ptx::make_kmajor_sw128_desc(wst), b_lo = ptx::make_kmajor_sw128_desc(wst + (uint32_t)kHalfStage);
-              const uint32_t acc_first = acc_only | (B.first ? 0u : 1u);
-              if (B.src == SRC_ACT) {
-                const uint32_t a_hi = kColAhi + (uint32_t)B.kb * 32u, a_lo = kColAlo + (uint32_t)B.kb * 32u;
-                if (n_passes == 3) ptx::mma_block_ts3(d_t, a_hi, a_lo, b_hi, b_lo, idesc, acc_first);
-                else ptx::mma_block_ts1(d_t, a_hi, a_lo, b_hi, b_lo, idesc, acc_first);
-              } else {
-                if (B.src == SRC_PE_DIR && !dir_waited) {
-                  ptx::mbar_wait(bars + kBarDirFull, it & 1, P.err, ERR_PE_FULL);
-                  ptx::tc_fence_after();
-                  dir_waited = true;
-                }
-                const uint32_t pe_t = (B.src == SRC_PE_DIR) ? dir_base : pe_base;
-                const uint64_t a_hi = ptx::make_kmajor_sw128_desc(pe_t), a_lo = ptx::make_kmajor_sw128_desc(pe_t + kPeTile);
-                if (n_passes == 3) ptx::mma_block_ss3(d_t, a_hi, a_lo, b_hi, b_lo, idesc, acc_first, (uint32_t)B.ksteps);
-                else ptx::mma_block_ss1(d_t, a_hi, a_lo, b_hi, b_lo, idesc, acc_first, (uint32_t)B.ksteps);
-              }
-            }
-            release_stage(slot);
-            if (B.flags & 1) ptx::tc_commit_elect(bars + kBarDFull + 8 * B.nc);
-            if (B.flags & 2) ptx::tc_commit_elect(bars + kBarKbFree + 8 * B.kb);
-            if (P.trace && lane == 0) trace_rec(P, 1, w, b, gl, tr0, tr1, tr2, clock64(), trace_cursor);
-            if (!B.next) break;
-            b += (int)B.next;
-          }
-        }
-        pass_group(3);
-      }
-      ptx::tc_commit_elect(bars + kBarPeEmpty + 8 * buf);
-      ptx::tc_commit_elect(bars + kBarDirEmpty);
-    }
+    return;
   }
 
-  // ---------------------------------------------------------------- teardown
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (cl2) ptx::cluster_sync_all();              // the peer may still be crediting our barriers / have copies in flight at us
-  if (warp == kProdWarp) ptx::tmem_dealloc(tmem, 512);
+  // =============================================================== consumer warpgroups
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int wg = warp >> 2, t = threadIdx.x & 127, wi = warp & 3;
+  const uint32_t v = v0 + (uint32_t)wg;
+  const int bar_id = 1 + wg;
+  uint8_t* act = smem + P.off_wg + (uint32_t)wg * kWgBytes;       // K-block kb: hi at kb * kKBlock, lo 8 KB further
+  uint8_t* pe = act + kActBytes;
+  const uint32_t act_s = ptx::smem_u32(act), pe_s = ptx::smem_u32(pe);
+  const int r0 = wi * 16 + (lane >> 2);                           // this thread's accumulator rows: r0, r0 + 8
+  const int cq = 2 * (lane & 3);                                  // ... and columns 8 j + cq, + 1
+  const float so = P.act_scale, si = P.act_inv_scale;
+  const int n_passes = P.n_passes;
+  const int Lx = P.net.L_xyz, Ld = P.net.L_dir, ix = P.net.inc_xyz, idr = P.net.inc_dir;
+  int slot = 0;
+  uint32_t ph = 0;
+  float acc[4][32];
+
+  // encoding of this tile's points (xyz or view direction) -> the encoding buffer, columns past the width zeroed
+  auto encode = [&](long long tile, bool dir) {
+    ptx::named_bar_sync(bar_id, 128);          // every wgmma of the warpgroup that read the buffer has completed
+    if (t < 64) {
+      long long m = tile * kTileM + t;
+      if (m >= P.in.M) m = P.in.M - 1;
+      float p[3], d[3];
+      fetch_point(P.in, m, p, d);
+      auto emit = [&](int j, float val) {
+        const float a = val * si;
+        const uint16_t h = f16_bits_sat(a);
+        const uint32_t off = swz_off(t, j);
+        *reinterpret_cast<uint16_t*>(pe + off) = h;
+        *reinterpret_cast<uint16_t*>(pe + 8192 + off) = f16_bits_sat(a - f16_bits_to_float(h));
+      };
+      const int dim = dir ? P.net.dim_dir : P.net.dim_xyz;
+      for (int j = dim; j < 64; ++j) {
+        const uint32_t off = swz_off(t, j);
+        *reinterpret_cast<uint16_t*>(pe + off) = 0;
+        *reinterpret_cast<uint16_t*>(pe + 8192 + off) = 0;
+      }
+      if (dir) positional_encoding(d, Ld, idr, P.net.freq_dir, emit);
+      else positional_encoding(p, Lx, ix, P.net.freq_xyz, emit);
+    }
+    ptx::fence_proxy_async_smem();
+    ptx::named_bar_sync(bar_id, 128);
+  };
+
+  // Fused compositor on tile `itp` of this warpgroup, whose last layer is staged in shared memory.  Same arithmetic, in the
+  // same order, as composite_kernel (nm_composite.cuh):  A  every thread takes ONE sample: alpha, keep (the exp lives
+  // here);  B  one thread per ray segment runs the transmittance product chain through shared memory;  C  every thread:
+  // weight, mask, the four products;  D  one lane per (segment, accumulator) runs the five ordered sums.  The ray cut by
+  // the tile's upper edge leaves T and its partial sums in a carry slot for the next tile (tiles of a group are
+  // consecutive for this warpgroup and groups start on ray boundaries).
+  uint8_t* comp_s = smem + P.off_comp + (uint32_t)wg * kCompBytes;
+  auto composite_tile = [&](uint32_t itp, long long tp) {
+    const CompositeArgs& A = P.comp;
+    const int r = t;
+    float4* stage = reinterpret_cast<float4*>(comp_s);                      // q per sample, later (w r, w g, w b, w t)
+    float* keepT = reinterpret_cast<float*>(comp_s + 64 * 16);              // keep per sample, later T
+    float* wv = keepT + 64;                                                 // weight per sample
+    const float* carry_in = wv + 64 + ((itp & 1) ^ 1) * 8;                  // written by the previous tile
+    float* carry_out = wv + 64 + (itp & 1) * 8;
+    const long long p0 = tp * kTileM, p1 = min(p0 + (long long)kTileM, P.in.M);
+    const int S = A.S;
+    const long long ray_first = p0 / S;
+    const int n_seg = (int)((p1 - 1) / S - ray_first) + 1;
+    ptx::named_bar_sync(bar_id, 128);            // the staged outputs are visible
+    // ---- A
+    const long long p = p0 + r;
+    const bool live = r < kTileM && p < p1;
+    float tc = 0.f, alpha = 0.f;
+    float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (live) {
+      const long long ray = p / S;
+      const int i = (int)(p - ray * S);
+      const float* tr = A.t + ray * S;
+      tc = tr[i];
+      const float tn = (i + 1 < S) ? tr[i + 1] : 0.f;
+      q = stage[r];
+      float keep;
+      alpha = comp_alpha(A, ray, i, tc, tn, comp_ray_norm(A.dirs, ray), q.w, &keep);
+      keepT[r] = keep;
+    }
+    ptx::named_bar_sync(bar_id, 128);
+    // ---- B
+    for (int k = r; k < n_seg; k += 128) {
+      const long long rayk = ray_first + k;
+      const long long s0 = max(rayk * (long long)S, p0), s1 = min((rayk + 1) * (long long)S, p1);
+      float T = (s0 > rayk * (long long)S) ? carry_in[0] : 1.0f;
+      for (int j = (int)(s0 - p0); j < (int)(s1 - p0); ++j) { const float kp = keepT[j]; keepT[j] = T; T = __fmul_rn(T, kp); }
+      if (s1 < (rayk + 1) * (long long)S) carry_out[0] = T;
+    }
+    ptx::named_bar_sync(bar_id, 128);
+    // ---- C
+    if (live) {
+      const float T = keepT[r];
+      const float w = __fmul_rn(alpha, T);
+      if (A.weights) A.weights[p] = w;
+      if (A.mask_weights) A.mask_weights[p] = (T > A.thr) ? 1.f : 0.f;
+      wv[r] = w;
+      stage[r] = make_float4(__fmul_rn(w, q.x), __fmul_rn(w, q.y), __fmul_rn(w, q.z), __fmul_rn(w, tc));
+    }
+    ptx::named_bar_sync(bar_id, 128);
+    // ---- D: lane c of an 8-lane group owns accumulator c (r, g, b, acc, depth) of the group's segment
+    for (int k0 = 0; k0 < n_seg; k0 += 16) {
+      const int k = k0 + (r >> 3), c = r & 7;
+      const long long rayk = ray_first + k;
+      const long long s0 = max(rayk * (long long)S, p0), s1 = min((rayk + 1) * (long long)S, p1);
+      const bool actv = k < n_seg && c < 5;
+      float sum = 0.f;
+      if (actv) {
+        if (s0 > rayk * (long long)S) sum = carry_in[1 + c];
+        const float* src = (c == 3) ? wv : reinterpret_cast<const float*>(stage) + (c == 4 ? 3 : c);
+        const int stride = (c == 3) ? 1 : 4;
+        for (int j = (int)(s0 - p0); j < (int)(s1 - p0); ++j) sum = __fadd_rn(sum, src[j * stride]);
+      }
+      const float s_g = __shfl_down_sync(0xffffffffu, sum, 1), s_b = __shfl_down_sync(0xffffffffu, sum, 2);
+      const float s_a = __shfl_down_sync(0xffffffffu, sum, 3), s_d = __shfl_down_sync(0xffffffffu, sum, 4);
+      if (actv && c == 0) {
+        if (s1 == (rayk + 1) * (long long)S) {
+          CompState cs;
+          cs.T = 0.f; cs.r = sum; cs.g = s_g; cs.b = s_b; cs.acc = s_a; cs.depth = s_d;
+          comp_finish(cs, A, rayk);
+        } else {
+          carry_out[1] = sum; carry_out[2] = s_g; carry_out[3] = s_b; carry_out[4] = s_a; carry_out[5] = s_d;
+        }
+      }
+    }
+    ptx::named_bar_sync(bar_id, 128);            // staging block consumed, carry visible to the next tile
+  };
+
+  // point-major bf16 hi/lo pack of the weight-gradient GEMM: features f, f+1 of point pt (nm_gemm.h ptiles of 128 features
+  // x 64 points, K-major: row f % 128, 16-byte chunk ((pt % 64) / 8) ^ (f % 8); MN-major: feature group (f % 128) / 64,
+  // point row pt % 64, chunk ((f % 64) / 8) ^ (pt % 8))
+  auto emit_pack = [&](uint8_t* packT, int f, long long pt, uint32_t hi2, uint32_t lo2) {
+    uint8_t* tb = packT + ((size_t)(f >> 7) * (size_t)P.emit.kbt + (size_t)(pt >> 6)) * 32768u;
+    if (P.emit_mn) {
+      const uint32_t off = (uint32_t)((f & 127) >> 6) * 8192u + (uint32_t)(pt & 63) * 128u +
+                           ((((uint32_t)(f & 63) >> 3) ^ (uint32_t)(pt & 7)) << 4) + (uint32_t)(f & 7) * 2u;
+      *reinterpret_cast<uint32_t*>(tb + off) = hi2;
+      *reinterpret_cast<uint32_t*>(tb + 16384u + off) = lo2;
+    } else {
+      const uint32_t c8 = (uint32_t)((pt & 63) >> 3);
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int fe = f + e;
+        const uint32_t off = (uint32_t)(fe & 127) * 128u + ((c8 ^ (uint32_t)(fe & 7)) << 4) + (uint32_t)(pt & 7) * 2u;
+        *reinterpret_cast<uint16_t*>(tb + off) = (uint16_t)(e ? (hi2 >> 16) : (hi2 & 0xffffu));
+        *reinterpret_cast<uint16_t*>(tb + 16384u + off) = (uint16_t)(e ? (lo2 >> 16) : (lo2 & 0xffffu));
+      }
+    }
+  };
+
+  float sigma_val[2] = {0.f, 0.f};
+  for (uint32_t it = 0; tile_of(v0, it) >= 0; ++it) {
+    const long long tile = tile_of(v, it);
+    if (tile < 0) {
+      // ghost iteration: no tile of our own, but the other warpgroup consumes this round's stages — wait for each stage and
+      // hand it straight back
+      for (int b = 0; b < n_blocks; ++b) {
+        if (t == 0) {
+          ptx::mbar_wait(bars + kBarWFull + 8 * slot, ph, P.err, ERR_W_FULL);
+          ptx::mbar_arrive(bars + kBarWEmpty + 8 * slot);
+        }
+        if (++slot == NS) { slot = 0; ph ^= 1; }
+      }
+      continue;
+    }
+    if (MODE != 2) encode(tile, false);
+    const long long m0 = tile * kTileM + r0, m1 = m0 + 8;
+    const bool val0 = m0 < P.in.M, val1 = m1 < P.in.M;
+    for (int li = 0; li < n_layers; ++li) {
+      const LayerProg& L = P.net.layers[li];
+      if (MODE != 2 && L.pe_src == SRC_PE_DIR) encode(tile, true);
+      // ------------------------------------------------------------ main loop: this layer's weight blocks
+      if (L.kind != KIND_LOAD) {
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+#pragma unroll
+          for (int i = 0; i < 32; ++i) acc[c][i] = 0.f;
+        ptx::wgmma_fence();
+        int prev = -1;
+        for (int b = L.blk_begin; b < L.blk_end; ++b) {
+          const BlockProg& B = P.net.blocks[b];
+          ptx::mbar_wait(bars + kBarWFull + 8 * slot, ph, P.err, ERR_W_FULL);
+          const uint32_t wst = sbase + (uint32_t)slot * kStageBytes;
+          const uint64_t b_hi = ptx::make_kmajor_sw128_desc(wst), b_lo = ptx::make_kmajor_sw128_desc(wst + (uint32_t)kHalfStage);
+          const uint32_t a_t = (B.src == SRC_ACT) ? act_s + (uint32_t)B.kb * kKBlock : pe_s;
+          const uint64_t a_hi = ptx::make_kmajor_sw128_desc(a_t), a_lo = ptx::make_kmajor_sw128_desc(a_t + 8192u);
+          const int ks = (B.src == SRC_ACT) ? 4 : (int)B.ksteps;
+          switch (B.nc) {
+            case 0: mma_block<MODE == 2>(acc[0], a_hi, a_lo, b_hi, b_lo, ks, n_passes); break;
+            case 1: mma_block<MODE == 2>(acc[1], a_hi, a_lo, b_hi, b_lo, ks, n_passes); break;
+            case 2: mma_block<MODE == 2>(acc[2], a_hi, a_lo, b_hi, b_lo, ks, n_passes); break;
+            default: mma_block<MODE == 2>(acc[3], a_hi, a_lo, b_hi, b_lo, ks, n_passes); break;
+          }
+          ptx::wgmma_commit();
+          ptx::wgmma_wait<1>();                      // the previous block's MMAs are complete: release its stage
+          if (prev >= 0 && t == 0) ptx::mbar_arrive(bars + kBarWEmpty + 8 * prev);
+          prev = slot;
+          if (++slot == NS) { slot = 0; ph ^= 1; }
+        }
+        ptx::wgmma_wait<0>();
+        if (prev >= 0 && t == 0) ptx::mbar_arrive(bars + kBarWEmpty + 8 * prev);
+#pragma unroll
+        for (int c = 0; c < 4; ++c) ptx::fence_regs<32>(acc[c]);
+      }
+      // ------------------------------------------------------------ epilogue, straight from the accumulator fragments
+      const int NC = L.n_out >> 6;
+      const bool writes_a = (L.kind == KIND_HIDDEN) || (L.kind == KIND_SIGMA && !L.is_final) || (L.kind == KIND_LOAD) ||
+                            (L.kind == KIND_BWD && !L.is_final);
+      const int heads = L.kind == KIND_SIGMA ? 1 : (L.kind == KIND_RGB ? 3 : (L.kind == KIND_OUT4 ? 4 : 0));
+      uint8_t* packT = (MODE >= 1) ? P.emit.packT[li] : nullptr;
+      float part[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+      float dsg[2] = {0.f, 0.f};
+      if (MODE == 2 && L.kind == KIND_BWD && L.aux2) {
+        dsg[0] = val0 ? P.dout[(size_t)m0 * 4 + 3] : 0.f;
+        dsg[1] = val1 ? P.dout[(size_t)m1 * 4 + 3] : 0.f;
+      }
+      if (writes_a) ptx::named_bar_sync(bar_id, 128);    // every warp of the warpgroup is past this layer's MMAs
+#pragma unroll
+      for (int nc = 0; nc < 4; ++nc) {
+        if (nc >= NC) continue;
+        uint32_t mk_in[2][2] = {{0xffffffffu, 0xffffffffu}, {0xffffffffu, 0xffffffffu}};   // mode 2: [row][32-column word]
+        if (MODE == 2 && L.kind == KIND_BWD && L.relu) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const long long m = e ? m1 : m0;
+            if (e ? val1 : val0) {
+              const uint2 bw = *reinterpret_cast<const uint2*>(P.emit.bits[li] + (size_t)m * (size_t)(L.n_out >> 5) + (size_t)(nc * 2));
+              mk_in[e][0] = bw.x; mk_in[e][1] = bw.y;
+            }
+          }
+        }
+        uint32_t mk_out[2][2] = {{0u, 0u}, {0u, 0u}};
+#pragma unroll
+        for (int j8 = 0; j8 < 8; ++j8) {
+          const int col = nc * 64 + j8 * 8 + cq;
+          float x[2][2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const bool valid = e ? val1 : val0;
+            const long long m = e ? m1 : m0;
+            if (MODE == 2 && L.kind == KIND_LOAD) {
+              // top of the data-gradient chain: dZ of the last forward layer, from HBM (rows past M are zero)
+              const float2 z = valid ? *reinterpret_cast<const float2*>(P.dz_in + (size_t)m * P.dz_ld + col) : make_float2(0.f, 0.f);
+              x[e][0] = z.x; x[e][1] = z.y;
+            } else if (MODE == 2) {
+              // dA = dZ W (+ d sigma * w_alpha), masked by relu' of the forward layer below.  (Its column sums — the bias
+              // gradient — are taken by the weight-gradient GEMM from the pack emitted below: nm_gemm_tc.cu a_rowsum.)
+#pragma unroll
+              for (int u = 0; u < 2; ++u) {
+                float y = acc[nc][j8 * 4 + 2 * e + u] * so;
+                if (L.aux2) y = fmaf(dsg[e], s_head[L.head_off + col + u], y);
+                const uint32_t w = valid ? mk_in[e][j8 >> 2] : 0u;
+                x[e][u] = ((w >> ((col + u) & 31)) & 1u) ? y : 0.f;
+              }
+            } else {
+#pragma unroll
+              for (int u = 0; u < 2; ++u) {
+                float y = fmaf(acc[nc][j8 * 4 + 2 * e + u], so, s_bias[L.bias_off + col + u]);
+                if (L.relu) y = fmaxf(y, 0.f);
+                x[e][u] = y;
+              }
+            }
+          }
+#pragma unroll
+          for (int hh = 0; hh < 4; ++hh) {
+            if (hh >= heads) break;
+            const float* w = s_head + L.head_off + hh * L.n_out + col;
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              part[e][hh] = fmaf(w[0], x[e][0], part[e][hh]);
+              part[e][hh] = fmaf(w[1], x[e][1], part[e][hh]);
+            }
+          }
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const bool valid = e ? val1 : val0;
+            const long long m = e ? m1 : m0;
+            const int row = r0 + 8 * e;
+            if (MODE == 1) {
+              // by-products for the training backward: relu mask bits and the fp32 copy (layers the head kernels read)
+              mk_out[e][j8 >> 2] |= ((x[e][0] > 0.f ? 1u : 0u) | (x[e][1] > 0.f ? 2u : 0u)) << (col & 31);
+              if (P.emit.act[li] && valid) *reinterpret_cast<float2*>(P.emit.act[li] + (size_t)m * L.n_out + col) = make_float2(x[e][0], x[e][1]);
+            }
+            if (writes_a) {
+              uint32_t hi, lo;
+              const float a0 = x[e][0] * si, a1 = x[e][1] * si;
+              if (MODE == 2) {            // gradients: bf16 hi/lo (fp32's exponent range)
+                split_bf16x2(a0, a1, &hi, &lo);
+              } else {
+                hi = ptx::pack_f16x2_sat(a0, a1);
+                const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+                lo = ptx::pack_f16x2_sat(a0 - f.x, a1 - f.y);
+              }
+              if (n_passes != 3) lo = 0u;
+              const uint32_t off = (uint32_t)nc * kKBlock + swz_off(row, col & 63);
+              *reinterpret_cast<uint32_t*>(act + off) = hi;
+              *reinterpret_cast<uint32_t*>(act + 8192u + off) = lo;
+              if (MODE >= 1 && packT) {
+                // the weight-gradient operand is the A operand's value (hi + lo), as bf16 hi / lo; rows past M as zeros
+                uint32_t ph2 = 0u, pl2 = 0u;
+                if (valid) {
+                  if (MODE == 2) {
+                    ph2 = hi; pl2 = lo;
+                  } else {
+                    const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+                    const float2 fl = __half22float2(*reinterpret_cast<const __half2*>(&lo));
+                    split_bf16x2((fh.x + fl.x) * so, (fh.y + fl.y) * so, &ph2, &pl2);
+                  }
+                }
+                emit_pack(packT, col, tile * kTileM + row, ph2, pl2);
+              }
+            } else if (MODE >= 1 && packT) {
+              uint32_t ph2, pl2;
+              split_bf16x2(valid ? x[e][0] : 0.f, valid ? x[e][1] : 0.f, &ph2, &pl2);
+              emit_pack(packT, col, tile * kTileM + row, ph2, pl2);
+            }
+          }
+        }
+        if (MODE == 1 && P.emit.bits[li]) {     // relu mask: the four lanes of a quad hold the 32 bits of a row's word
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+#pragma unroll
+            for (int g = 0; g < 2; ++g) {
+              uint32_t w = mk_out[e][g];
+              w |= __shfl_xor_sync(0xffffffffu, w, 1);
+              w |= __shfl_xor_sync(0xffffffffu, w, 2);
+              const long long m = e ? m1 : m0;
+              if ((lane & 3) == 0 && (e ? val1 : val0)) P.emit.bits[li][(size_t)m * (size_t)(L.n_out >> 5) + (size_t)(nc * 2 + g)] = w;
+            }
+        }
+      }
+      if (writes_a) {
+        ptx::fence_proxy_async_smem();           // the next layer's wgmmas read what the generic proxy wrote
+        ptx::named_bar_sync(bar_id, 128);
+      }
+      if (heads) {
+        // a row's columns are spread over the four lanes of a quad
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+#pragma unroll
+          for (int hh = 0; hh < 4; ++hh) {
+            part[e][hh] += __shfl_xor_sync(0xffffffffu, part[e][hh], 1);
+            part[e][hh] += __shfl_xor_sync(0xffffffffu, part[e][hh], 2);
+          }
+        const float* hb = s_head + L.head_off + heads * L.n_out;
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const long long m = e ? m1 : m0;
+          const bool valid = e ? val1 : val0;
+          if (L.kind == KIND_SIGMA) {
+            sigma_val[e] = part[e][0] + hb[0];
+            if (L.is_final && (lane & 3) == 0 && valid && P.out) P.out[m] = sigma_val[e];   // sigma-only program
+          } else if ((lane & 3) == 0 && (P.comp_on || (valid && P.out))) {
+            float o[4];
+#pragma unroll
+            for (int hh = 0; hh < 4; ++hh) o[hh] = (hh < heads) ? part[e][hh] + hb[hh] : 0.f;
+            const float sg = (L.kind == KIND_RGB) ? sigma_val[e] : o[3];
+            if (P.out_sigma_only) {
+              P.out[m] = sg;
+            } else {
+              float4 res;
+              res.x = 1.f / (1.f + expf(-o[0]));
+              res.y = 1.f / (1.f + expf(-o[1]));
+              res.z = 1.f / (1.f + expf(-o[2]));
+              res.w = sg;
+              if (MODE == 0 && P.comp_on) reinterpret_cast<float4*>(comp_s)[r0 + 8 * e] = res;
+              else reinterpret_cast<float4*>(P.out)[m] = res;
+            }
+          }
+        }
+      }
+    }
+    if (MODE == 0 && P.comp_on) composite_tile(it, tile);
+  }
 }
 
 }  // namespace
@@ -938,29 +563,28 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
 static int launch_prepared(TcParams& P, int num_sms, cudaStream_t st, int64_t* launches) {
   const NetProgram& hp = P.net;
   {
-    const char* e = getenv("NM_TC_DEBUG");
-    P.dbg = e ? atoi(e) : 0;
+    bool dir_seen = false;
+    for (int i = 0; i < hp.n_layers; ++i) {
+      NM_CHECK(!(dir_seen && hp.layers[i].pe_src == SRC_PE_XYZ), "xyz encoding read after the view-direction encoding");
+      if (hp.layers[i].pe_src == SRC_PE_DIR) dir_seen = true;
+    }
   }
   auto align_up = [](uint32_t x, uint32_t a) { return (x + a - 1) / a * a; };
   int dev = 0, max_smem = 0;
   NM_CUDA(cudaGetDevice(&dev));
   NM_CUDA(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-  const uint32_t fixed = kPeTotal + align_up(hp.n_bias * 4, 16) + align_up((hp.n_head > 0 ? hp.n_head : 4) * 4, 16) +
-                         (128 + 512) * 4 + kBarBytes + (P.comp_on ? kCompBytes : 0u) + ((P.emit_mn && P.mode != 2) ? kEpiWarps * 8192u + 1024u : 0u);
+  const uint32_t fixed = 2 * kWgBytes + align_up(hp.n_bias * 4, 16) + align_up((hp.n_head > 0 ? hp.n_head : 4) * 4, 16) +
+                         kBarBytes + (P.comp_on ? 2 * kCompBytes : 0u);
   int ns = ((int)max_smem - (int)fixed) / kStageBytes;
   if (ns > kMaxStages) ns = kMaxStages;
-  if (const char* e = getenv("NM_TC_STAGES")) { int v = atoi(e); if (v >= 2 && v < ns) ns = v; }
   NM_CHECK(ns >= 2, "network too large for the shared-memory budget (%u B fixed, %d B available)", fixed, max_smem);
   P.num_stages = ns;
   uint32_t off = (uint32_t)ns * kStageBytes;
-  P.off_pe = off; off += kPeTotal;
+  P.off_wg = off; off += 2 * kWgBytes;
   P.off_bias = off; off += align_up(hp.n_bias * 4, 16);
   P.off_head = off; off += align_up((hp.n_head > 0 ? hp.n_head : 4) * 4, 16);
-  P.off_red = off; off += (128 + 512) * 4;
   P.off_bars = off; off += kBarBytes;
-  P.off_comp = off; off += P.comp_on ? kCompBytes : 0u;
-  if (P.emit_mn && P.mode != 2) { off = align_up(off, 1024); P.off_stg = off; off += kEpiWarps * 8192u; }
-  else P.off_stg = P.off_pe;
+  P.off_comp = off; off += P.comp_on ? 2 * kCompBytes : 0u;
   if (P.tile_group < 1) P.tile_group = 1;
   NM_CHECK((int)off <= max_smem, "shared-memory layout overflow");
 
@@ -972,40 +596,10 @@ static int launch_prepared(TcParams& P, int num_sms, cudaStream_t st, int64_t* l
     configured_devs[mode] |= 1u << (dev & 31);
   }
   const long long n_groups = (P.n_tiles + P.tile_group - 1) / P.tile_group;
-  long long grid = n_groups < num_sms ? n_groups : num_sms;
-  // pairs of CTAs share the weight stream when the grid allows it (NM_TC_CLUSTER=0: every CTA streams its own copy)
-  static const bool cluster_env = [] { const char* e = getenv("NM_TC_CLUSTER"); return !e || atoi(e) != 0; }();
-  P.cluster = 1;
-  if (cluster_env && grid >= 2 && !(P.dbg & 4)) {
-    grid += grid & 1;                             // an odd grid gets one more CTA: rank 1 of the last pair only runs ghosts... or a real group
-    if (grid > num_sms) grid -= 2;
-    if (grid >= 2) P.cluster = 2;
-  }
-  const char* trace_path = getenv("NM_TC_TRACE");
-  const size_t trace_words = 1 + 6 * (size_t)kTraceRegion * 5;
-  if (trace_path) {
-    NM_CUDA(cudaMalloc(&P.trace, trace_words * 8));
-    NM_CUDA(cudaMemset(P.trace, 0, trace_words * 8));
-  }
-  if (P.cluster == 2) {
-    cudaLaunchConfig_t lc{};
-    lc.gridDim = dim3((unsigned)grid); lc.blockDim = dim3(kThreads); lc.dynamicSmemBytes = off; lc.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    lc.attrs = at; lc.numAttrs = 1;
-    NM_CUDA(cudaLaunchKernelEx(&lc, kern, P));
-  } else {
-    kern<<<(unsigned)grid, kThreads, off, st>>>(P);
-  }
+  const long long pairs = (n_groups + 1) / 2;                   // two workers (consumer warpgroups) per CTA
+  const long long grid = pairs < num_sms ? pairs : num_sms;
+  kern<<<(unsigned)grid, kThreads, off, st>>>(P);
   NM_CUDA(cudaGetLastError());
-  if (trace_path) {   // debugging aid: synchronous dump of CTA 0's event log
-    NM_CUDA(cudaStreamSynchronize(st));
-    std::vector<unsigned long long> h(trace_words);
-    NM_CUDA(cudaMemcpy(h.data(), P.trace, trace_words * 8, cudaMemcpyDeviceToHost));
-    if (FILE* f = fopen(trace_path, "wb")) { fwrite(h.data(), 8, trace_words, f); fclose(f); }
-    cudaFree(P.trace);
-  }
   if (launches) ++*launches;
   return 0;
 }
@@ -1015,9 +609,9 @@ int mlp_tc_composite_group(int S) {
   if (S <= 0) return 0;
   int a = S, b = kTileM;
   while (b) { const int t = a % b; a = b; b = t; }
-  const long long l = (long long)S / a * kTileM;      // lcm(S, 128)
+  const long long l = (long long)S / a * kTileM;      // lcm(S, kTileM)
   const long long g = l / kTileM;
-  return g <= 8 ? (int)g : 0;                          // long groups would unbalance the CTAs
+  return g <= 16 ? (int)g : 0;                         // long groups would unbalance the workers
 }
 
 int launch_mlp_tc(const NetDev& net, bool sigma_only, int n_passes, int act_scale_log2, const MlpInput& in, float* out,
@@ -1039,8 +633,7 @@ int launch_mlp_tc(const NetDev& net, bool sigma_only, int n_passes, int act_scal
   P.err = d_err;
   if (emit) {
     P.has_emit = 1; P.emit = *emit; P.emit_mn = emit->mn;
-    static const bool fe_env = [] { const char* e = getenv("NM_TRAIN_FE_EMIT"); return e && atoi(e) != 0; }();
-    P.fe_emit = (fe_env && !emit->mn) ? 1 : 0;
+    P.n_tiles = 2 * ((in.M + 127) / 128);      // the packs hold whole 128-point blocks: their zero rows are written too
   }
   P.tile_group = 1;
   if (comp) {
@@ -1060,7 +653,7 @@ int launch_mlp_tc_bwd(const NetDev& net, long long M, const float* dz_in, int dz
                       const MlpEmit& io, int n_passes, int num_sms, int* d_err, cudaStream_t st, int64_t* launches, int emit_mn) {
   if (M <= 0) return 0;
   NM_CHECK(net.bwd_valid && net.d_wpack_bwd, "backward weight stream not built");
-  NM_CHECK((dz_ld & 3) == 0 && (reinterpret_cast<uintptr_t>(dz_in) & 15) == 0, "dz_in must be 16-byte aligned rows");
+  NM_CHECK((dz_ld & 1) == 0 && (reinterpret_cast<uintptr_t>(dz_in) & 7) == 0, "dz_in must be 8-byte aligned rows");
   TcParams P{};
   P.net = net.bwd;
   P.wpack = net.d_wpack_bwd;
@@ -1069,11 +662,10 @@ int launch_mlp_tc_bwd(const NetDev& net, long long M, const float* dz_in, int dz
   P.in.M = M;
   P.n_passes = n_passes;
   P.act_scale = 1.f; P.act_inv_scale = 1.f;
-  P.n_tiles = (M + kTileM - 1) / kTileM;
+  P.n_tiles = 2 * ((M + 127) / 128);
   P.err = d_err;
   P.has_emit = 1; P.emit = io;
   P.mode = 2; P.dz_in = dz_in; P.dz_ld = dz_ld; P.dout = dout; P.emit_mn = emit_mn;
-  static_assert(kEpiWarps * 8192u <= kPeTotal, "the pack staging blocks live in the (unused) encoding buffers");
   return launch_prepared(P, num_sms, st, launches);
 }
 

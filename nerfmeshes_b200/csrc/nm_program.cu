@@ -70,15 +70,11 @@ static bool is_skip(const NmNetDesc& d, int i) {  // src/nerf/models.py:36-42,64
 // bookkeeping and n_blocks from each layer's n_out / k_act / pe_src / k_pe.
 static int schedule_blocks(NetProgram* p) {
   const int nl = p->n_layers;
-  // tensor-core schedule.  Block (k,n) needs epilogue chunks 0..max(k,n) of the previous layer (group): chunk k
-  // supplies activation K-block k, chunk n frees accumulator chunk n.  The TMEM A region is single-buffered and is
-  // overwritten in place by the epilogue; the kernel's kb_free barriers (not the block order) make that safe.
-  // Issuer assignment.  policy 1 (default): the issuer owns an accumulator chunk, so a chunk's blocks are issued by
-  // one warp in schedule order -> deterministic accumulation order, first block overwrites.  policy 0: round-robin
-  // over the schedule (better balanced, but accumulation order across issuers is timing dependent, and the
-  // accumulator must be re-zeroed by the epilogue).  NM_TC_POLICY overrides, for experiments.
-  int policy = 1;
-  if (const char* e = getenv("NM_TC_POLICY")) policy = atoi(e) ? 1 : 0;
+  // tensor-core schedule: the block order within a layer (row part first, then the column part of each j) is the order of
+  // the weight stream.  The wgmma kernel (nm_mlp_tc.cu) reads only src / kb / nc / ksteps of each block, in this order, and
+  // blk_begin / blk_end of each layer.  The rest (group, first / last, the per-issuer flags / next / first_blk / none_d /
+  // none_k and accumulate_only) is bookkeeping the kernel does not use; the CPU schedule tests check it.
+  const int policy = 1;   // a block's "issuer" owns its accumulator chunk
   p->accumulate_only = policy == 0 ? 1 : 0;
   int nb = 0;
   for (int li = 0; li < nl; ++li) {

@@ -1,5 +1,5 @@
 // Layer "program" of one FlexibleNeRFModel (reference: src/nerf/models.py:5-80) as the fused kernels consume it.
-// Built once on the host at weight-load time (nm_program.cu); read by the tcgen05 kernel (nm_mlp_tc.cu) and
+// Built once on the host at weight-load time (nm_program.cu); read by the wgmma kernel (nm_mlp_tc.cu) and
 // the fp32 CUDA-core kernel (nm_mlp_simt.cu).
 #pragma once
 #include <stdint.h>
@@ -11,8 +11,8 @@ constexpr int kMaxBlocks = 200;
 constexpr int kMaxFreq = 16;
 
 // tensor-core tiling constants
-constexpr int kIssuers = 4;           // MMA-issuing warps; a block's issuer is BlockProg.flags >> 4
-constexpr int kTileM = 128;          // points per tile (= TMEM lanes)
+constexpr int kIssuers = 4;           // schedule bookkeeping only (BlockProg.flags >> 4); the wgmma kernel does not read it
+constexpr int kTileM = 64;           // points per tile (= rows of one warpgroup MMA)
 constexpr int kChunk = 64;           // N-chunk / K-block width
 constexpr int kStageBytes = 16384;   // one weight stage: [hi 64x64 fp16 | lo 64x64 fp16], 128B-swizzled K-major
 constexpr int kHalfStage = 8192;
@@ -51,7 +51,7 @@ struct LayerProg {
 // One (K-block, N-chunk) step of the tensor-core schedule == one 16 KB weight stage.
 struct BlockProg {
   uint8_t src;     // SRC_*
-  uint8_t kb;      // K-block index within the source (activation TMEM columns kb*32..)
+  uint8_t kb;      // K-block index within the source (activation K-block kb of the shared-memory A operand)
   uint8_t nc;      // N-chunk: accumulator columns nc*64..
   uint8_t ksteps;  // 1..4 MMAs of K=16
   uint8_t group;   // needs epilogue chunks 0..group of the previous layer done

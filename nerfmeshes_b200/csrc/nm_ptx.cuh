@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, bulk async copy (TMA engine, 1-D), tcgen05 (alloc / mma / ld / st /
-// commit / fences).  Encodings follow the PTX ISA; descriptor bit layouts follow cute/arch/mma_sm100_desc.hpp.
+// Thin inline-PTX wrappers for sm_90a: mbarrier, bulk async copy (TMA engine, 1-D), warpgroup MMA (wgmma) and its
+// shared-memory descriptors.  Encodings follow the PTX ISA.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -71,22 +71,6 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uin
                "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
-// ---- cluster of two CTAs sharing one weight stream --------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// one L2 read, the same shared-memory offset written (and the same mbarrier offset credited) in every CTA of `mask`
-__device__ __forceinline__ void bulk_g2s_multicast(uint32_t dst_smem, const void* src, uint32_t bytes, uint32_t bar, uint16_t mask) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::"r"(dst_smem),
-               "l"(src), "r"(bytes), "r"(bar), "h"(mask)
-               : "memory");
-}
-
 // shared -> global bulk store (bulk async-group completion): the issuing thread commits a group and, before the shared-memory
 // source is rewritten (or the kernel exits), waits for the group's reads (or writes) to finish
 __device__ __forceinline__ void bulk_s2g(void* dst, uint32_t src_smem, uint32_t bytes) {
@@ -96,267 +80,66 @@ __device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bul
 __device__ __forceinline__ void bulk_wait_group_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_group0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// ---- tcgen05 ---------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]
-__device__ __forceinline__ void mma_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]
-__device__ __forceinline__ void mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-// Warp-converged variants: every lane of the issuing warp executes the statement, one elected lane issues.  Keeping
-// the issuing warp converged matters: a lone diverged lane pays ~200 cycles per tcgen05.mma, a converged warp ~100
-// (measured, tools/umma_bench.cu), and several issuing warps overlap that cost.
-__device__ __forceinline__ void mma_ss_elect(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred pe, p;\n\telect.sync _|pe, 0xffffffff;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void mma_ts_elect(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred pe, p;\n\telect.sync _|pe, 0xffffffff;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-// One schedule block (64x64, K=64) as ONE asm statement: a single elect, operands converted to uniform registers once,
-// descriptor increments in PTX.  Issuing the 12 (exact) / 4 (fast) MMAs one statement at a time costs ~85 cycles each
-// (five R2UR + elect per MMA); fused they approach the 32-cycle execution time of an N=64 MMA.
-// Order (exact): a_hi*b_hi, a_lo*b_hi, a_hi*b_lo; the first MMA overwrites when acc_first == 0.
-__device__ __forceinline__ void mma_block_ts3(uint32_t d_tmem, uint32_t a_hi, uint32_t a_lo, uint64_t b_hi, uint64_t b_lo,
-                                              uint32_t idesc, uint32_t acc_first) {
-  asm volatile(
-      "{\n\t.reg .pred pe, pacc, pt;\n\t.reg .b32 a;\n\t.reg .b64 b;\n\t"
-      "elect.sync _|pe, 0xffffffff;\n\tsetp.ne.b32 pacc, %6, 0;\n\tsetp.eq.b32 pt, 0, 0;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %3, %5, pacc;\n\t"
-      "add.u32 a, %1, 8;\n\tadd.u64 b, %3, 2;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], [a], b, %5, pt;\n\t"
-      "add.u32 a, %1, 16;\n\tadd.u64 b, %3, 4;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], [a], b, %5, pt;\n\t"
-      "add.u32 a, %1, 24;\n\tadd.u64 b, %3, 6;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], [a], b, %5, pt;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], [%2], %3, %5, pt;\n\t"
-      "add.u32 a, %2, 8;\n\tadd.u64 b, %3, 2;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], [a], b, %5, pt;\n\t"
-      "add.u32 a, %2, 16;\n\tadd.u64 b, %3, 4;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], [a], b, %5, pt;\n\t"
-      "add.u32 a, %2, 24;\n\tadd.u64 b, %3, 6;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], [a], b, %5, pt;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %4, %5, pt;\n\t"
-      "add.u32 a, %1, 8;\n\tadd.u64 b, %4, 2;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], [a], b, %5, pt;\n\t"
-      "add.u32 a, %1, 16;\n\tadd.u64 b, %4, 4;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], [a], b, %5, pt;\n\t"
-      "add.u32 a, %1, 24;\n\tadd.u64 b, %4, 6;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], [a], b, %5, pt;\n\t"
-      "}"
-      ::"r"(d_tmem), "r"(a_hi), "r"(a_lo), "l"(b_hi), "l"(b_lo), "r"(idesc), "r"(acc_first)
-      : "memory");
-}
-__device__ __forceinline__ void mma_block_ts1(uint32_t d_tmem, uint32_t a_hi, uint32_t a_lo, uint64_t b_hi, uint64_t b_lo,
-                                              uint32_t idesc, uint32_t acc_first) {
-  asm volatile(
-      "{\n\t.reg .pred pe, pacc, pt;\n\t.reg .b32 a;\n\t.reg .b64 b;\n\t"
-      "elect.sync _|pe, 0xffffffff;\n\tsetp.ne.b32 pacc, %6, 0;\n\tsetp.eq.b32 pt, 0, 0;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %3, %5, pacc;\n\t"
-      "add.u32 a, %1, 8;\n\tadd.u64 b, %3, 2;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], [a], b, %5, pt;\n\t"
-      "add.u32 a, %1, 16;\n\tadd.u64 b, %3, 4;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], [a], b, %5, pt;\n\t"
-      "add.u32 a, %1, 24;\n\tadd.u64 b, %3, 6;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], [a], b, %5, pt;\n\t"
-      "}"
-      ::"r"(d_tmem), "r"(a_hi), "r"(a_lo), "l"(b_hi), "l"(b_lo), "r"(idesc), "r"(acc_first)
-      : "memory");
-}
-// same for an encoding block (A from shared memory), ksteps (1..4) K=16 steps per pass
-__device__ __forceinline__ void mma_block_ss3(uint32_t d_tmem, uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo,
-                                              uint32_t idesc, uint32_t acc_first, uint32_t ksteps) {
-  asm volatile(
-      "{\n\t.reg .pred pe, pk, pacc, pt;\n\t.reg .b64 a, b;\n\t"
-      "elect.sync _|pe, 0xffffffff;\n\tsetp.ne.b32 pacc, %6, 0;\n\tsetp.eq.b32 pt, 0, 0;\n\t"
-      "setp.gt.u32 pk, %7, 0;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, %1, 0;\n\tadd.u64 b, %3, 0;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pacc;\n\t"
-      "setp.gt.u32 pk, %7, 1;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, %1, 2;\n\tadd.u64 b, %3, 2;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "setp.gt.u32 pk, %7, 2;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, %1, 4;\n\tadd.u64 b, %3, 4;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "setp.gt.u32 pk, %7, 3;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, %1, 6;\n\tadd.u64 b, %3, 6;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "setp.gt.u32 pk, %7, 0;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, %2, 0;\n\tadd.u64 b, %3, 0;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "setp.gt.u32 pk, %7, 1;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, %2, 2;\n\tadd.u64 b, %3, 2;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "setp.gt.u32 pk, %7, 2;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, %2, 4;\n\tadd.u64 b, %3, 4;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "setp.gt.u32 pk, %7, 3;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, %2, 6;\n\tadd.u64 b, %3, 6;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "setp.gt.u32 pk, %7, 0;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, %1, 0;\n\tadd.u64 b, %4, 0;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "setp.gt.u32 pk, %7, 1;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, %1, 2;\n\tadd.u64 b, %4, 2;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "setp.gt.u32 pk, %7, 2;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, %1, 4;\n\tadd.u64 b, %4, 4;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "setp.gt.u32 pk, %7, 3;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, %1, 6;\n\tadd.u64 b, %4, 6;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "}"
-      ::"r"(d_tmem), "l"(a_hi), "l"(a_lo), "l"(b_hi), "l"(b_lo), "r"(idesc), "r"(acc_first), "r"(ksteps)
-      : "memory");
-}
-__device__ __forceinline__ void mma_block_ss1(uint32_t d_tmem, uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo,
-                                              uint32_t idesc, uint32_t acc_first, uint32_t ksteps) {
-  asm volatile(
-      "{\n\t.reg .pred pe, pk, pacc, pt;\n\t.reg .b64 a, b;\n\t"
-      "elect.sync _|pe, 0xffffffff;\n\tsetp.ne.b32 pacc, %6, 0;\n\tsetp.eq.b32 pt, 0, 0;\n\t"
-      "setp.gt.u32 pk, %7, 0;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, %1, 0;\n\tadd.u64 b, %3, 0;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pacc;\n\t"
-      "setp.gt.u32 pk, %7, 1;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, %1, 2;\n\tadd.u64 b, %3, 2;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "setp.gt.u32 pk, %7, 2;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, %1, 4;\n\tadd.u64 b, %3, 4;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "setp.gt.u32 pk, %7, 3;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, %1, 6;\n\tadd.u64 b, %3, 6;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "}"
-      ::"r"(d_tmem), "l"(a_hi), "l"(a_lo), "l"(b_hi), "l"(b_lo), "r"(idesc), "r"(acc_first), "r"(ksteps)
-      : "memory");
-}
-// The same blocks with the per-k16 descriptor advance given by the caller (>>4 units): K-major SWIZZLE_128B operands step
-// by 32 B (2), MN-major ones by two 8-row groups = 2048 B (128).
-__device__ __forceinline__ void mma_block_ss3g(uint32_t d_tmem, uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo,
-                                               uint32_t idesc, uint32_t acc_first, uint32_t ksteps, uint64_t a_step, uint64_t b_step) {
-  asm volatile(
-      "{\n\t.reg .pred pe, pk, pacc, pt;\n\t.reg .b64 a, b;\n\t"
-      "elect.sync _|pe, 0xffffffff;\n\tsetp.ne.b32 pacc, %6, 0;\n\tsetp.eq.b32 pt, 0, 0;\n\t"
-      "setp.gt.u32 pk, %7, 0;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, %1, 0;\n\tadd.u64 b, %3, 0;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pacc;\n\t"
-      "setp.gt.u32 pk, %7, 1;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, a, %8;\n\tadd.u64 b, b, %9;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "setp.gt.u32 pk, %7, 2;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, a, %8;\n\tadd.u64 b, b, %9;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "setp.gt.u32 pk, %7, 3;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, a, %8;\n\tadd.u64 b, b, %9;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "setp.gt.u32 pk, %7, 0;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, %2, 0;\n\tadd.u64 b, %3, 0;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "setp.gt.u32 pk, %7, 1;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, a, %8;\n\tadd.u64 b, b, %9;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "setp.gt.u32 pk, %7, 2;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, a, %8;\n\tadd.u64 b, b, %9;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "setp.gt.u32 pk, %7, 3;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, a, %8;\n\tadd.u64 b, b, %9;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "setp.gt.u32 pk, %7, 0;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, %1, 0;\n\tadd.u64 b, %4, 0;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "setp.gt.u32 pk, %7, 1;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, a, %8;\n\tadd.u64 b, b, %9;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "setp.gt.u32 pk, %7, 2;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, a, %8;\n\tadd.u64 b, b, %9;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "setp.gt.u32 pk, %7, 3;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, a, %8;\n\tadd.u64 b, b, %9;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %5, pt;\n\t"
-      "}"
-      ::"r"(d_tmem), "l"(a_hi), "l"(a_lo), "l"(b_hi), "l"(b_lo), "r"(idesc), "r"(acc_first), "r"(ksteps), "l"(a_step), "l"(b_step)
-      : "memory");
-}
-__device__ __forceinline__ void mma_block_ss1g(uint32_t d_tmem, uint64_t a_hi, uint64_t b_hi, uint32_t idesc, uint32_t acc_first,
-                                               uint32_t ksteps, uint64_t a_step, uint64_t b_step) {
-  asm volatile(
-      "{\n\t.reg .pred pe, pk, pacc, pt;\n\t.reg .b64 a, b;\n\t"
-      "elect.sync _|pe, 0xffffffff;\n\tsetp.ne.b32 pacc, %4, 0;\n\tsetp.eq.b32 pt, 0, 0;\n\t"
-      "setp.gt.u32 pk, %5, 0;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, %1, 0;\n\tadd.u64 b, %2, 0;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %3, pacc;\n\t"
-      "setp.gt.u32 pk, %5, 1;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, a, %6;\n\tadd.u64 b, b, %7;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %3, pt;\n\t"
-      "setp.gt.u32 pk, %5, 2;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, a, %6;\n\tadd.u64 b, b, %7;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %3, pt;\n\t"
-      "setp.gt.u32 pk, %5, 3;\n\tand.pred pk, pk, pe;\n\tadd.u64 a, a, %6;\n\tadd.u64 b, b, %7;\n\t"
-      "@pk tcgen05.mma.cta_group::1.kind::f16 [%0], a, b, %3, pt;\n\t"
-      "}"
-      ::"r"(d_tmem), "l"(a_hi), "l"(b_hi), "r"(idesc), "r"(acc_first), "r"(ksteps), "l"(a_step), "l"(b_step)
-      : "memory");
-}
-__device__ __forceinline__ void tc_commit_elect(uint32_t bar) {
-  asm volatile(
-      "{\n\t.reg .pred pe;\n\telect.sync _|pe, 0xffffffff;\n\t"
-      "@pe tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(bar)
-      : "memory");
-}
-// the same arrival delivered to the mbarrier at this offset in every CTA of `mask`
-__device__ __forceinline__ void tc_commit_elect_multicast(uint32_t bar, uint16_t mask) {
-  asm volatile(
-      "{\n\t.reg .pred pe;\n\telect.sync _|pe, 0xffffffff;\n\t"
-      "@pe tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n\t}" ::"r"(bar), "h"(mask)
-      : "memory");
-}
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start>>4 [0,14), LBO>>4
-// [16,30) (unused for swizzled K-major, set to 1), SBO>>4 [32,46) = 1024 B between 8-row groups, version=1 [46,48),
-// layout_type=2 (SWIZZLE_128B) [61,64).  Tile base must be 1024-byte aligned; advancing K by 16 fp16 = +32 B = +2.
+// ---- wgmma (sm_90a warpgroup MMA) ----------------------------------------------------------------------------------
+// Shared-memory matrix descriptor (PTX ISA "matrix-descriptor-format" for wgmma): start>>4 [0,14), LBO>>4 [16,30),
+// SBO>>4 [32,46), base offset [49,52) = 0 (tile bases are 1024-byte aligned), layout type [62,64) = 1 (SWIZZLE_128B).
+// K-major: rows of 128 B (64 16-bit K elements, 16-byte chunks XOR-swizzled by row % 8), SBO = 1024 B between 8-row
+// groups, LBO unused (1); advancing K by 16 = +32 B = +2.
 __device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) |
-         ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
+  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
 // MN-major, SWIZZLE_128B descriptor of a 128 (M or N) x 64 (K) tile of 16-bit elements stored as [MN group of 64][K row][128 B]:
-// the 64 MN elements of one K index are one 128-byte line (16-byte chunks XOR-swizzled by the K row % 8, as in the K-major
-// case), 8 K rows make a 1024-byte group (SBO), the second MN group of 64 follows at LBO = 64 rows * 128 B = 8192 B.
-// Canonical form ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte units (cute mma_traits_sm100.hpp).  Advancing K by 16 = +2048 B.
+// the 64 MN elements of one K index are one 128-byte line (16-byte chunks XOR-swizzled by the K row % 8), 8 K rows make a
+// 1024-byte group (SBO), the second MN group of 64 follows at LBO = 64 rows * 128 B = 8192 B.  Advancing K by 16 = +2048 B.
 __device__ __forceinline__ uint64_t make_mnmajor_sw128_desc(uint32_t smem_addr) {
   return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)(8192 >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) |
-         ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
+         ((uint64_t)1 << 62);
 }
-// kind::f16 instruction descriptor (cute::UMMA::InstrDescriptor): D fp32 (bits 4-5 = 1), A/B fp16 (0), both K-major,
-// N>>3 at [17,23), M>>4 at [24,29).
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N) {
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Keeps the compiler from moving accesses of accumulator registers across an asynchronous wgmma's issue and its wait.
+template <int N>
+__device__ __forceinline__ void fence_regs(float* d) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-
-#define NM_TMEM_LD32(taddr, r)                                                                                          \
-  asm volatile(                                                                                                         \
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,"  \
-      "%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"                                                        \
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),     \
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),          \
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),         \
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])                       \
-      : "r"(taddr)                                                                                                      \
-      : "memory")
-#define NM_TMEM_LD16(taddr, r)                                                                                          \
-  asm volatile(                                                                                                         \
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"          \
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),     \
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])                        \
-      : "r"(taddr)                                                                                                      \
-      : "memory")
-#define NM_TMEM_ST16(taddr, r)                                                                                         \
-  asm volatile(                                                                                                        \
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(  \
-          taddr),                                                                                                      \
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),    \
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])                                           \
-      : "memory")
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+// D (64 x N fp32, registers of the warpgroup) (+)= A (64 x 16, smem desc) * B (N x 16, smem desc)^T.  acc == 0 overwrites.
+// TA / TB: 0 = K-major, 1 = MN-major operand tile; BF16: operands are bf16 (else fp16).  Accumulator fragment: register i
+// of thread t holds row 16 * (t / 32 % 4) + (t % 32) / 4 + 8 * ((i / 2) % 2), column 8 * (i / 4) + 2 * (t % 4) + i % 2.
+template <int TA, int TB, int BF16>
+__device__ __forceinline__ void wgmma_m64n64(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+  if (BF16) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(adesc), "l"(bdesc), "r"(acc), "n"(TA), "n"(TB));
+  } else {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(adesc), "l"(bdesc), "r"(acc), "n"(TA), "n"(TB));
+  }
+}
+template <int TA, int TB, int BF16>
+__device__ __forceinline__ void wgmma_m64n128(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+  if (BF16) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(acc), "n"(TA), "n"(TB));
+  } else {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(acc), "n"(TA), "n"(TB));
+  }
+}
 
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");

@@ -783,7 +783,7 @@ int mlp_backward(NetDev& net, const MlpInput& in, const float* dout, float* ws_b
   grad_layout(G, gw_off, gw_ld);
   if (tc && !layerwise) {
     // Fused: the SIMT heads produce dZ of the last layer; ONE launch of the fused kernel on the backward program walks the
-    // data gradient down the whole network with dZ in TMEM (W^T streamed through shared memory, relu masks from the recompute,
+    // data gradient down the whole network with dZ in shared memory (W^T streamed through shared memory, relu masks from the recompute,
     // the rank-1 d sigma term, bias gradients as column sums) and leaves every layer's dZ as the point-major pack the
     // long-K weight-gradient GEMMs consume — no per-layer round trip of dZ / masks / row packs through HBM.
     if (!net.bwd_valid)

@@ -63,7 +63,7 @@ class Engine:
     def __init__(self, coarse: dict, fine: Optional[dict], settings: RenderSettings, device: int = 0):
         self.lib = L.load()
         if not torch.cuda.is_available():
-            raise L.NmError("nerfmeshes_b200 needs a CUDA device (sm_100a); there is no CPU path")
+            raise L.NmError("nerfmeshes_b200 needs a CUDA device (sm_90a); there is no CPU path")
         self.device = torch.device("cuda", device)
         self.settings = settings
         self.has_fine = fine is not None
@@ -367,7 +367,7 @@ class Engine:
 
     def check_flags(self):
         """Synchronise the current stream and raise if a kernel of this handle flagged an error (AABB hit-list overflow,
-        tcgen05 watchdog)."""
+        tensor-core pipeline watchdog)."""
         L.check(self.lib.nm_check_flags(self._h, self._stream()))
 
     def grid_sigma(self, lins, x0=0, x1=None, with_rgb=False, out=None):

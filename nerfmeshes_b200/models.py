@@ -8,7 +8,7 @@ Same names, constructor arguments, call conventions and state-dict keys as
   src/models/model_base.py:65-73   BaseModel.sample_points
 but every computation is a call into libnerfmeshes_b200.so through nerfmeshes_b200.engine.Engine.  The classes are
 torch.nn.Modules only so that parameters / state_dict / load_state_dict / train() / eval() behave as the reference's
-callers expect (PyTorch-Lightning itself is not required).  There is no torch fallback: without a B200 the forward
+callers expect (PyTorch-Lightning itself is not required).  There is no torch fallback: without an H100 the forward
 raises.
 """
 from __future__ import annotations

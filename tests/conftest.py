@@ -12,16 +12,16 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
     config.addinivalue_line("markers", "multigpu: gpu test that spawns one process per GPU (needs >= 2 devices)")
 
 
 def pytest_collection_modifyitems(config, items):
-    """`gpu` tests need the B200: skip (not fail) them on a machine without CUDA; `multigpu` tests need >= 2 devices."""
+    """`gpu` tests need an H100: skip (not fail) them on a machine without CUDA; `multigpu` tests need >= 2 devices."""
     n = torch.cuda.device_count() if torch.cuda.is_available() else 0
     for item in items:
         if "gpu" in item.keywords and n == 0:
-            item.add_marker(pytest.mark.skip(reason="no CUDA device (run on the B200 box with -m gpu)"))
+            item.add_marker(pytest.mark.skip(reason="no CUDA device (run on an H100 with -m gpu)"))
         elif "multigpu" in item.keywords and n < 2:
             item.add_marker(pytest.mark.skip(reason="needs >= 2 CUDA devices"))
 

@@ -1,152 +1,30 @@
-"""Functional model of tc_gemm_kernel's mbarrier protocol (nm_gemm_tc.cu): stage ring full[s] / empty[s] across the tiles
-of a persistent CTA and the double-buffered accumulator hand-off acc_full[b] / acc_empty[b], with the hardware's ONE
-parity bit per wait (tools/protocol_sim.Bar).  Agents are generators that yield when they would block; the test checks
-that every schedule finishes (no deadlock, no arrival overflow) and that data moves in order: the MMA warp consumes exactly
-the K blocks the producer loaded for that tile, and every epilogue warp reads the accumulator of the tile it expects."""
+"""Functional model of tc_gemm_kernel's mbarrier protocol (nm_gemm_tc.cu): one producer fills the stage ring full[s] /
+empty[s] with the K blocks of every tile of a persistent CTA; the two consumer warpgroups (rows 0-63 / 64-127 of the tile)
+each take every stage in order, release a stage once their wgmmas on it have completed, and run the epilogue of a tile from
+their registers after the tile's last K block.  Modelled by tools/protocol_sim.run_ring with the hardware's ONE parity bit
+per wait: every schedule finishes (no deadlock, no arrival overflow) and each warpgroup reads exactly the K blocks the
+producer loaded, in order."""
 import itertools
 import os
-import random
 import sys
 
 from conftest import ROOT
 
 sys.path.insert(0, os.path.join(ROOT, "tools"))
-from protocol_sim import Bar  # noqa: E402
-
-EPI_WARPS = 16
-
-
-def run(NS, nk, tiles, seed):
-    full = [Bar(f"full{s}", 1) for s in range(NS)]
-    empty = [Bar(f"empty{s}", 1) for s in range(NS)]
-    acc_full = [Bar(f"acc_full{b}", 1) for b in range(2)]
-    acc_empty = [Bar(f"acc_empty{b}", EPI_WARPS) for b in range(2)]
-    stage = [None] * NS            # what the producer last loaded into each stage
-    acc = [None, None]             # which tile's sum sits in each TMEM buffer, and how many K blocks went in
-    log = []
-
-    def wait(bar, k):
-        while not bar.done(k):
-            yield
-
-    def producer():
-        it = 0
-        for t in range(tiles):
-            for kk in range(nk):
-                s = it % NS
-                if it >= NS:
-                    yield from wait(empty[s], it // NS - 1)
-                stage[s] = (t, kk)
-                full[s].arrive()                       # expect_tx + complete_tx of the bulk copies
-                it += 1
-                yield
-
-    def mma():
-        it = 0
-        for i in range(tiles):
-            b = i & 1
-            if i >= 2:
-                yield from wait(acc_empty[b], (i >> 1) - 1)
-            for kk in range(nk):
-                s = it % NS
-                yield from wait(full[s], it // NS)
-                assert stage[s] == (i, kk), f"MMA of tile {i} k {kk} found {stage[s]} in stage {s}"
-                acc[b] = (i, kk + 1) if kk else (i, 1)  # first K block overwrites
-                empty[s].arrive()                      # tcgen05.commit -> empty[s]
-                it += 1
-                yield
-            acc_full[b].arrive()                       # tcgen05.commit -> acc_full[b]
-
-    def epilogue(w):
-        for i in range(tiles):
-            b = i & 1
-            yield from wait(acc_full[b], i >> 1)
-            assert acc[b] == (i, nk), f"epilogue warp {w} expected tile {i} complete, buffer {b} holds {acc[b]}"
-            yield                                       # TMEM reads, stores
-            log.append((w, i))
-            acc_empty[b].arrive()
-
-    agents = [producer(), mma()] + [epilogue(w) for w in range(EPI_WARPS)]
-    rng = random.Random(seed)
-    alive = list(range(len(agents)))
-    for _ in range(200000):
-        if not alive:
-            break
-        a = rng.choice(alive)                           # adversarial interleaving
-        try:
-            next(agents[a])
-        except StopIteration:
-            alive.remove(a)
-    assert not alive, f"deadlock / livelock: NS={NS} nk={nk} tiles={tiles}, agents left {alive}"
-    assert sorted(log) == sorted(itertools.product(range(EPI_WARPS), range(tiles)))
+from protocol_sim import run_ring  # noqa: E402
 
 
 def test_persistent_gemm_protocol_all_small_shapes():
     for NS, nk, tiles in itertools.product((2, 3), (1, 2, 3, 4, 5, 7), (1, 2, 3, 5, 16)):
         for seed in range(3):
-            run(NS, nk, tiles, seed)
-
-
-def run_split_k_with_row_sums(NS, nk, seed):
-    """The split-K (weight-gradient) variant with a_rowsum: one tile per CTA, and the 16 epilogue warps first walk the stage
-    ring as READERS of the A tiles (row sums = bias gradient), arriving on empty[s] next to the MMA warp's commit — so
-    empty[s] counts 1 + 16 arrivals and the producer may only refill a stage once both kinds of consumer are done."""
-    full = [Bar(f"full{s}", 1) for s in range(NS)]
-    empty = [Bar(f"empty{s}", 1 + EPI_WARPS) for s in range(NS)]
-    acc_full = Bar("acc_full", 1)
-    stage = [None] * NS
-    summed = [[] for _ in range(EPI_WARPS)]
-    done = []
-
-    def wait(bar, k):
-        while not bar.done(k):
-            yield
-
-    def producer():
-        for it in range(nk):
-            s = it % NS
-            if it >= NS:
-                yield from wait(empty[s], it // NS - 1)
-            stage[s] = it
-            full[s].arrive()
-            yield
-
-    def mma():
-        for it in range(nk):
-            s = it % NS
-            yield from wait(full[s], it // NS)
-            assert stage[s] == it
-            empty[s].arrive()
-            yield
-        acc_full.arrive()
-
-    def epilogue(w):
-        for it in range(nk):                            # row-sum readers
-            s = it % NS
-            yield from wait(full[s], it // NS)
-            assert stage[s] == it, f"row-sum warp {w} expected K block {it}, stage {s} holds {stage[s]}"
-            summed[w].append(it)
-            yield
-            empty[s].arrive()
-        yield from wait(acc_full, 0)
-        done.append(w)
-
-    agents = [producer(), mma()] + [epilogue(w) for w in range(EPI_WARPS)]
-    rng = random.Random(seed)
-    alive = list(range(len(agents)))
-    for _ in range(400000):
-        if not alive:
-            break
-        a = rng.choice(alive)
-        try:
-            next(agents[a])
-        except StopIteration:
-            alive.remove(a)
-    assert not alive, f"deadlock: NS={NS} nk={nk}, agents left {alive}"
-    assert sorted(done) == list(range(EPI_WARPS)) and all(x == list(range(nk)) for x in summed)
+            ok, info = run_ring(NS, tiles, [nk], lambda wg, r: True, seed)
+            assert ok, (NS, nk, tiles, seed, info)
 
 
 def test_split_k_row_sum_readers_share_the_stage_ring():
+    """The split-K (weight-gradient) variant with a_rowsum: one tile per CTA; each consumer warpgroup sums the rows of its half
+    of the staged A tile before it releases the stage, so a stage is refilled only after both have read it."""
     for NS, nk in itertools.product((2, 3), (1, 2, 3, 4, 7, 9, 16)):
         for seed in range(3):
-            run_split_k_with_row_sums(NS, nk, seed)
+            ok, info = run_ring(NS, 1, [nk], lambda wg, r: True, seed)
+            assert ok, (NS, nk, seed, info)

@@ -1,4 +1,4 @@
-"""Per-launch time of the backward's tcgen05 GEMM (nm_gemm_tc.cu) through nm_debug_gemm: the pack kernels run once,
+"""Per-launch time of the backward's wgmma GEMM (nm_gemm_tc.cu) through nm_debug_gemm: the pack kernels run once,
 the GEMM NM_GEMM_REPEAT times; (t(repeat=R) - t(repeat=1)) / (R-1).  NM_GEMM_DBG=1/2/4 knocks out MMAs / loads / stores.
 Run each configuration in its own process (the env knobs are read once)."""
 import os, sys

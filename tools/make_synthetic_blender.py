@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Write a tiny Blender-format dataset (transforms_{train,val,test}.json + PNGs) and a config in the reference's live schema
 (config/nerf-synthetic-lego.yml) so that train_nerf.py / eval_nerf.py can be driven without the real datasets (none ship
-with the reference).  Images are rendered from the lego checkpoint re-packed under tests/golden/ when a B200 is available
+with the reference).  Images are rendered from the lego checkpoint re-packed under tests/golden/ when an H100 is available
 (`--render`), else filled with noise (enough for the no-GPU plumbing test, which stops at the first compute call).
 
     python tools/make_synthetic_blender.py OUT_DIR [--size 40] [--views 6 2 2] [--render] [--tiny-net]

@@ -1,13 +1,22 @@
-"""Functional simulation of the tcgen05 kernel's mbarrier protocol (nm_mlp_tc.cu) on the real layer program.
+"""Functional model of the weight / operand stage ring both tensor-core kernels use (nm_mlp_tc.cu, nm_gemm_tc.cu), with the
+hardware's ONE parity bit per mbarrier wait.
 
-Agents (producer, 4 MMA issuers, 2 epilogue sets, front-end) are generators that yield when they would block; a
-round-robin scheduler runs them until everyone finishes (ok) or nobody can move (deadlock -> prints who waits on what).
-Timing is not modelled, only ordering / phase correctness.  Commits are modelled as completing immediately.
+One producer fills a ring of NS stages in a fixed order (full[s]: one arrival per fill, the bulk copies' transaction bytes
+completing it; empty[s]: one arrival per consumer warpgroup).  Two consumer warpgroups each take EVERY stage in that order.
+A consumer releases a stage only once the wgmmas reading it have completed: it waits for the next stage, issues on it, and
+then (wgmma.wait_group 1) releases the previous one; the last stage of a run of blocks is released after wait_group 0.  In
+the MLP kernel each warpgroup has its own tiles; when warpgroup 1 has no tile left in a round that warpgroup 0 still runs,
+it walks that round's stages as a "ghost" (wait, release) so that both walk the ring the same number of times.
 
-    NM_TC_POLICY=1 python tools/protocol_sim.py [--tiles 3] [--stages 5]
+Agents are generators that yield when they would block; a seeded random scheduler runs them until everyone finishes (ok) or
+the step budget is spent (deadlock).  Every stage read is checked against what the producer put there, so a stage refilled
+before both consumers released it is caught.  Timing is not modelled, only ordering and phase correctness.
+
+    python tools/protocol_sim.py [--tiles 3] [--stages 5]
 """
 import argparse
 import os
+import random
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -30,291 +39,93 @@ class Bar:
         return (self.phase & 1) != (k & 1)   # phases away from the barrier's current phase aliases (this is what is modelled)
 
 
-def simulate(prog, tiles, NS, verbose=False, armed_counter=True, fe_emit=False):
-    L = [prog.layers[i] for i in range(prog.n_layers)]
-    w_full = [Bar(f"w_full{i}", 1) for i in range(NS)]
-    w_empty = [Bar(f"w_empty{i}", 1) for i in range(NS)]
-    pe_full = [Bar(f"pe_full{i}", 1) for i in range(2)]
-    pe_empty = [Bar(f"pe_empty{i}", 4) for i in range(2)]
-    chunk = [Bar(f"chunk_ready{i}", 1) for i in range(4)]       # one arrival per epilogue set (4 warps act together)
-    d_full = [Bar(f"d_full{i}", 4) for i in range(4)]
-    kb_free = [Bar(f"kb_free{i}", 4) for i in range(4)]
-    dir_full, dir_empty = Bar("dir_full", 1), Bar("dir_empty", 4)
-    emit_done = [Bar(f"emit_done{i}", 1) for i in range(2)]      # fe_emit (mode 1): the front end answers chunk_ready[2..3] per layer
-    uses_dir = any(L[i].pe_src == 2 for i in range(len(L)))
-    waiting = {}
-    armed = [0]
+def run_ring(NS, rounds, runs, own, seed, release_count=2, max_steps=400000):
+    """rounds: how many times the producer walks its stage sequence; runs: lengths of the consecutive runs of stages a consumer
+    issues before a wait_group 0 (an MLP layer's blocks / a GEMM tile's K blocks), summing to one round; own(wg, r): whether
+    warpgroup wg has its own work in round r (else a ghost round).  Returns (ok, info)."""
+    per_round = sum(runs)
+    full = [Bar(f"full{s}", 1) for s in range(NS)]
+    empty = [Bar(f"empty{s}", release_count) for s in range(NS)]
+    stage = [None] * NS
+    seen = [[], []]
     errors = []
 
-    def wait(me, bar, k):
+    def wait(bar, k):
         while not bar.done(k):
-            waiting[me] = f"{bar.name} completion #{k} (phase now {bar.phase}, pending {bar.pending})"
             yield
-        waiting.pop(me, None)
 
     def producer():
-        g = 0
-        for t in range(tiles):
-            for b in range(prog.n_blocks):
-                slot, rnd = g % NS, g // NS
-                if rnd > 0:
-                    yield from wait("producer", w_empty[slot], rnd - 1)
-                w_full[slot].arrive()
-                g += 1
-                armed[0] = g
-
-    def fe_emit_tile(T):
-        for li in range(len(L)):
-            gl = T * len(L) + li
-            for n in (2, 3):
-                yield from wait("frontend", chunk[n], gl)
-                emit_done[n - 2].arrive()
-
-    def frontend():
-        for t in range(tiles):
-            buf = t & 1
-            if t >= 2:
-                yield from wait("frontend", pe_empty[buf], t // 2 - 1)
-            pe_full[buf].arrive()
-            if fe_emit and t > 0:
-                yield from fe_emit_tile(t - 1)
-            if uses_dir:
-                if t >= 1:
-                    yield from wait("frontend", dir_empty, t - 1)
-                dir_full.arrive()
-        if fe_emit:
-            yield from fe_emit_tile(tiles - 1)
-
-    def issuer(w):
-        me = f"issuer{w}"
-        g = 0
-        gl = 0
-        for t in range(tiles):
-            buf = t & 1
-            yield from wait(me, pe_full[buf], t // 2)
-            for li, Lp in enumerate(L):
-                waited = -1
-
-                def pass_group(gr):
-                    nonlocal waited
-                    while waited < gr:
-                        waited += 1
-                        if gl > 0:
-                            yield from wait(me, chunk[waited], gl - 1)
-                        if (Lp.none_d >> (4 * w + waited)) & 1:
-                            d_full[waited].arrive()
-                        if (Lp.none_k >> (4 * w + waited)) & 1:
-                            kb_free[waited].arrive()
-                for b in range(Lp.blk_begin, Lp.blk_end):
-                    B = prog.blocks[b]
-                    slot, rnd = g % NS, g // NS
-                    if (B.flags >> 4) == w:
-                        yield from pass_group(B.group)
-                        if B.src == 2:
-                            yield from wait(me, dir_full, t)
-                        while armed_counter and armed[0] <= g:
-                            waiting[me] = f"armed counter > {g}"
-                            yield
-                        yield from wait(me, w_full[slot], rnd)
-                        if w_full[slot].phase != rnd + 1:
-                            errors.append(f"{me}: consumed slot {slot} for block {g} (round {rnd}) while the barrier had completed {w_full[slot].phase} rounds")
-                        w_empty[slot].arrive()
-                        if B.flags & 1:
-                            d_full[B.nc].arrive()
-                        if B.flags & 2:
-                            kb_free[B.kb].arrive()
-                    g += 1
-                yield from pass_group(3)
-                gl += 1
-            pe_empty[buf].arrive()
-            dir_empty.arrive()
-
-    def epilogue(s):
-        me = f"epi_set{s}"
-        gl = 0
-        for t in range(tiles):
-            for li, Lp in enumerate(L):
-                for nn in range(2):
-                    n = s + 2 * nn
-                    yield from wait(me, d_full[n], gl)
-                    yield from wait(me, kb_free[n], gl)
-                    if fe_emit and nn == 1 and gl > 0:
-                        yield from wait(me, emit_done[n - 2], gl - 1)
-                    chunk[n].arrive()
-                gl += 1
-
-    agents = {"producer": producer(), "frontend": frontend(), **{f"issuer{w}": issuer(w) for w in range(4)},
-              **{f"epi_set{s}": epilogue(s) for s in range(2)}}
-    alive = dict(agents)
-    steps = 0
-    while alive:
-        progressed = False
-        for name in list(alive):
-            before = (tuple(b.phase for b in w_full + w_empty + pe_full + pe_empty + chunk + d_full + kb_free + emit_done + [dir_full, dir_empty]),
-                      tuple(b.pending for b in w_full + w_empty + pe_full + pe_empty + chunk + d_full + kb_free + emit_done + [dir_full, dir_empty]))
-            try:
-                next(alive[name])
-            except StopIteration:
-                del alive[name]
-                progressed = True
-                continue
-            after = (tuple(b.phase for b in w_full + w_empty + pe_full + pe_empty + chunk + d_full + kb_free + emit_done + [dir_full, dir_empty]),
-                     tuple(b.pending for b in w_full + w_empty + pe_full + pe_empty + chunk + d_full + kb_free + emit_done + [dir_full, dir_empty]))
-            progressed |= before != after
-        steps += 1
-        if not progressed:
-            return False, dict(waiting, errors=errors[:3])
-    return (not errors), dict(errors=errors[:3])
-
-
-def simulate_pair(prog, tiles, NS, ghost=False):
-    """Two CTAs of a cluster sharing ONE weight stream (nm_mlp_tc.cu, P.cluster == 2): rank 0's producer multicasts every
-    stage into both rings; each CTA's producer arms its own w_full (modelled as a second arrival: arm + copy completion); a
-    stage is released into BOTH CTAs' w_empty barriers (count 2) by the consuming issuer of each CTA.  ghost=True: rank 1 has
-    one tile less and its issuers run a ghost iteration for the last round (wait for the stage, release it).  Only the ring
-    protocol and the tile-level barriers that gate it are modelled per CTA; returns (ok, info)."""
-    L = [prog.layers[i] for i in range(prog.n_layers)]
-    uses_dir = any(L[i].pe_src == 2 for i in range(len(L)))
-    waiting, errors = {}, []
-
-    class Cta:
-        def __init__(self, r):
-            self.r = r
-            self.w_full = [Bar(f"c{r}.w_full{i}", 2) for i in range(NS)]
-            self.w_empty = [Bar(f"c{r}.w_empty{i}", 2) for i in range(NS)]
-            self.pe_full = [Bar(f"c{r}.pe_full{i}", 1) for i in range(2)]
-            self.pe_empty = [Bar(f"c{r}.pe_empty{i}", 4) for i in range(2)]
-            self.chunk = [Bar(f"c{r}.chunk{i}", 1) for i in range(4)]
-            self.d_full = [Bar(f"c{r}.d_full{i}", 4) for i in range(4)]
-            self.kb_free = [Bar(f"c{r}.kb_free{i}", 4) for i in range(4)]
-            self.dir_full, self.dir_empty = Bar(f"c{r}.dir_full", 1), Bar(f"c{r}.dir_empty", 4)
-            self.armed = 0
-            self.real = tiles - (1 if (ghost and r == 1) else 0)
-
-        def bars(self):
-            return self.w_full + self.w_empty + self.pe_full + self.pe_empty + self.chunk + self.d_full + self.kb_free + [self.dir_full, self.dir_empty]
-    C = [Cta(0), Cta(1)]
-
-    def wait(me, bar, k):
-        while not bar.done(k):
-            waiting[me] = f"{bar.name} completion #{k} (phase now {bar.phase}, pending {bar.pending})"
+        for it in range(rounds * per_round):
+            s, ph = it % NS, (it // NS) & 1
+            yield from wait(empty[s], ph ^ 1)
+            stage[s] = it
+            full[s].arrive()
             yield
-        waiting.pop(me, None)
 
-    def producer(c):
-        me = f"c{c.r}.producer"
-        g = 0
-        for t in range(tiles):                       # both ranks: the SAME number of rounds (iter_exists)
-            for b in range(prog.n_blocks):
-                slot, rnd = g % NS, g // NS
-                if rnd > 0:
-                    yield from wait(me, c.w_empty[slot], rnd - 1)
-                c.w_full[slot].arrive()              # arm (expect_tx)
-                if c.r == 0:                         # the multicast copy lands in both rings
-                    C[0].w_full[slot].arrive()
-                    C[1].w_full[slot].arrive()
-                g += 1
-                c.armed = g
+    def consumer(wg):
+        it = 0
+        for r in range(rounds):
+            real = own(wg, r)
+            for n in runs:
+                prev = None
+                for _ in range(n):
+                    s = it % NS
+                    yield from wait(full[s], it // NS)
+                    if stage[s] != it:
+                        errors.append(f"warpgroup {wg} expected stage content {it}, slot {s} holds {stage[s]}")
+                    seen[wg].append(it)
+                    yield
+                    if not real:                   # ghost: hand the stage straight back
+                        empty[s].arrive()
+                    else:                          # wait_group 1: the previous stage's wgmmas are complete
+                        if prev is not None:
+                            empty[prev].arrive()
+                        prev = s
+                    it += 1
+                if real and prev is not None:      # wait_group 0 at the end of the run
+                    empty[prev].arrive()
                 yield
 
-    def frontend(c):
-        me = f"c{c.r}.frontend"
-        for t in range(c.real):
-            buf = t & 1
-            if t >= 2:
-                yield from wait(me, c.pe_empty[buf], t // 2 - 1)
-            c.pe_full[buf].arrive()
-            if uses_dir:
-                if t >= 1:
-                    yield from wait(me, c.dir_empty, t - 1)
-                c.dir_full.arrive()
-
-    def issuer(c, w):
-        me = f"c{c.r}.issuer{w}"
-        g = gl = 0
-        for t in range(tiles):
-            is_ghost = t >= c.real
-            buf = t & 1
-            if not is_ghost:
-                yield from wait(me, c.pe_full[buf], t // 2)
-            for li, Lp in enumerate(L):
-                waited = -1
-
-                def pass_group(gr):
-                    nonlocal waited
-                    while waited < gr:
-                        waited += 1
-                        if gl > 0:
-                            yield from wait(me, c.chunk[waited], gl - 1)
-                        if (Lp.none_d >> (4 * w + waited)) & 1:
-                            c.d_full[waited].arrive()
-                        if (Lp.none_k >> (4 * w + waited)) & 1:
-                            c.kb_free[waited].arrive()
-                for b in range(Lp.blk_begin, Lp.blk_end):
-                    B = prog.blocks[b]
-                    slot, rnd = g % NS, g // NS
-                    if (B.flags >> 4) == w:
-                        if not is_ghost:
-                            yield from pass_group(B.group)
-                            if B.src == 2:
-                                yield from wait(me, c.dir_full, t)
-                        while c.armed <= g:
-                            waiting[me] = f"armed counter > {g}"
-                            yield
-                        yield from wait(me, c.w_full[slot], rnd)
-                        if c.w_full[slot].phase != rnd + 1:
-                            errors.append(f"{me}: consumed slot {slot} for block {g} (round {rnd}) while the barrier had completed {c.w_full[slot].phase} rounds")
-                        C[0].w_empty[slot].arrive()      # multicast commit: both CTAs' barriers
-                        C[1].w_empty[slot].arrive()
-                        if not is_ghost:
-                            if B.flags & 1:
-                                c.d_full[B.nc].arrive()
-                            if B.flags & 2:
-                                c.kb_free[B.kb].arrive()
-                    g += 1
-                if not is_ghost:
-                    yield from pass_group(3)
-                    gl += 1
-            if not is_ghost:
-                c.pe_empty[buf].arrive()
-                c.dir_empty.arrive()
-
-    def epilogue(c, s_):
-        me = f"c{c.r}.epi_set{s_}"
-        gl = 0
-        for t in range(c.real):
-            for li, Lp in enumerate(L):
-                for nn in range(2):
-                    n = s_ + 2 * nn
-                    yield from wait(me, c.d_full[n], gl)
-                    yield from wait(me, c.kb_free[n], gl)
-                    c.chunk[n].arrive()
-                gl += 1
-
-    agents = {}
-    for c in C:
-        agents[f"c{c.r}.producer"] = producer(c)
-        agents[f"c{c.r}.frontend"] = frontend(c)
-        for w in range(4):
-            agents[f"c{c.r}.issuer{w}"] = issuer(c, w)
-        for s_ in range(2):
-            agents[f"c{c.r}.epi{s_}"] = epilogue(c, s_)
-    alive = dict(agents)
-    allbars = C[0].bars() + C[1].bars()
-    while alive:
-        progressed = False
-        for name in list(alive):
-            before = (tuple(b.phase for b in allbars), tuple(b.pending for b in allbars), C[0].armed, C[1].armed)
+    agents = [producer(), consumer(0), consumer(1)]
+    rng = random.Random(seed)
+    alive = list(range(len(agents)))
+    try:
+        for _ in range(max_steps):
+            if not alive:
+                break
+            a = rng.choice(alive)
             try:
-                next(alive[name])
+                next(agents[a])
             except StopIteration:
-                del alive[name]
-                progressed = True
-                continue
-            progressed |= before != (tuple(b.phase for b in allbars), tuple(b.pending for b in allbars), C[0].armed, C[1].armed)
-        if not progressed:
-            return False, dict(waiting, errors=errors[:3])
-    return (not errors), dict(errors=errors[:3])
+                alive.remove(a)
+    except AssertionError as e:
+        return False, str(e)
+    if alive:
+        return False, f"deadlock: agents left {alive}"
+    if errors:
+        return False, errors[0]
+    want = list(range(rounds * per_round))
+    if seen[0] != want or seen[1] != want:
+        return False, "a consumer skipped or repeated a stage"
+    return True, "ok"
+
+
+def layer_runs(prog):
+    """Blocks per layer of an MLP layer program (layers without blocks issue nothing)."""
+    return [prog.layers[i].blk_end - prog.layers[i].blk_begin for i in range(prog.n_layers)
+            if prog.layers[i].blk_end > prog.layers[i].blk_begin]
+
+
+def simulate(prog, tiles, NS, seeds=(0, 1, 2), release_count=2):
+    """The MLP kernel on one CTA processing `tiles` 64-point tiles: warpgroup 0 takes tiles 0, 2, 4, ..., warpgroup 1 tiles
+    1, 3, ...; rounds = ceil(tiles / 2), warpgroup 1 ghosts the last round when tiles is odd."""
+    rounds = (tiles + 1) // 2
+    own = lambda wg, r: 2 * r + wg < tiles
+    for seed in seeds:
+        ok, info = run_ring(NS, rounds, layer_runs(prog), own, seed, release_count)
+        if not ok:
+            return False, f"seed {seed}: {info}"
+    return True, "ok"
 
 
 if __name__ == "__main__":
@@ -324,12 +135,6 @@ if __name__ == "__main__":
     a = ap.parse_args()
     from oracle import nerf_oracle as O
     from test_host_logic import debug_pack
-    for arch in (dict(), dict(num_layers=4, hidden_size=128, num_encoding_fn_xyz=6), dict(num_layers=3, hidden_size=128, use_viewdirs=False)):
-        cfg = O.NetCfg(**{**O.NetCfg().__dict__, **arch})
-        for sigma_only in (False, True):
-            prog, _ = debug_pack(cfg, O.init_weights(cfg, 1), sigma_only)
-            for ns in sorted({2, 3, a.stages}):
-                ok, who = simulate(prog, a.tiles, ns)
-                ok0, who0 = simulate(prog, a.tiles, ns, armed_counter=False)
-                print(f"arch={arch} sigma_only={sigma_only} stages={ns}: {'ok' if ok else 'FAIL ' + str(who)}"
-                      f"   [without the armed counter: {'ok' if ok0 else 'FAIL ' + str(who0)[:160]}]")
+    cfg = O.NetCfg()
+    prog, _ = debug_pack(cfg, O.init_weights(cfg, 1))
+    print(simulate(prog, a.tiles, a.stages))

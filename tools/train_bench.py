@@ -1,5 +1,5 @@
 """Time one training step of the lego configuration (two 8x256 nets, 64+128 samples) through the fused forward +
-backward: nm_loss_backward alone, and the full step with torch.optim.Adam + weight re-upload.  Run on a B200."""
+backward: nm_loss_backward alone, and the full step with torch.optim.Adam + weight re-upload.  Run on an H100."""
 import sys, os, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
