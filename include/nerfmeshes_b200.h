@@ -235,13 +235,12 @@ int nm_ray_voxel_indices_ex(NmHandle h, const float* origins_dev, int o_stride, 
 int nm_tree_integrate(NmHandle h, const int32_t* idx_dev, const float* weights_dev, const float* mask_weights_dev, int64_t n,
                       float* memm_dev, int32_t V, int32_t counter, void* stream);
 
-/* Test hook for the tensor-core GEMM of the backward pass (nm_gemm_tc.cu): D (M,N) = A (M,K) B (N,K)^T from fp32
- * row-major device arrays through the bf16 hi/lo operand packs.  a_cols / b_cols: that operand is given transposed
- * ((K,M) / (K,N)) and packed along its rows (the weight-gradient operands; 1 = K-major tiles, 2 = MN-major tiles read
- * through MN-major shared-memory descriptors); k_split: feed K as two segments;
- * fp16: fp16 halves instead of bf16; atomic: D += with K split over CTAs. */
-int nm_debug_gemm(NmHandle h, const float* a_dev, const float* b_dev, int M, int N, int K, int a_cols, int b_cols,
-                  int k_split, int n_passes, int fp16, int atomic, float* d_dev, void* stream);
+/* Test hook for the weight-gradient GEMM of the backward pass (nm_gemm_tc.cu): D (M,N) += A B^T, i.e.
+ * d[m][n] += sum_k a[k][m] b[k][n], from fp32 row-major device arrays a (K,M) and b (K,N) (K = points), packed into the
+ * bf16 hi/lo operand layouts the backward uses and reduced over K splits with atomics.  n_passes: 3 (hi*hi + lo*hi +
+ * hi*lo) or 1 (hi*hi). */
+int nm_debug_gemm(NmHandle h, const float* a_dev, const float* b_dev, int M, int N, int K, int n_passes, float* d_dev,
+                  void* stream);
 
 /* ---- host-only debugging aid (no CUDA): the layer program + tensor-core weight stream nm_load_weights would
  * upload, for CPU tests of the schedule / swizzle logic.  program_out receives the internal NetProgram struct

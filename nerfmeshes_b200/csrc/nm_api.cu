@@ -7,6 +7,7 @@
 #include <vector>
 
 #include "nm_common.h"
+#include "nm_gemm.h"
 
 namespace nm {
 const char* last_error();
@@ -316,7 +317,7 @@ int train_chunk(NmHandle h, const RayBatch& rb, int flags, uint64_t seed, const 
   const bool use_tc = c.precision != NM_PREC_FP32;
   const char* dg_env = getenv("NM_TRAIN_DIRECT_GB");      // read per call: the tests flip it to cover both walks
   const double direct_gb = dg_env ? atof(dg_env) : 48.0;
-  const size_t ws_main = train_fused(use_tc) && c.act_scale_log2 == 0 ? train_ws_bytes(h->nets[two ? NM_NET_FINE : NM_NET_COARSE].full, R * S, true) + 1024 : 0;
+  const size_t ws_main = use_tc && c.act_scale_log2 == 0 ? train_ws_bytes(h->nets[two ? NM_NET_FINE : NM_NET_COARSE].full, R * S, true) + 1024 : 0;
   const size_t ws_coarse = (ws_main && two) ? train_ws_bytes(h->nets[NM_NET_COARSE].full, R * Nc, true) + 1024 : 0;
   const bool direct = ws_main > 0 && (double)(ws_main + ws_coarse) <= direct_gb * 1e9 && (d_rgb || target) && (!two || d_rgb_coarse || target);
   float *ws_m = nullptr, *ws_c = nullptr;
@@ -368,7 +369,7 @@ int train_chunk(NmHandle h, const RayBatch& rb, int flags, uint64_t seed, const 
       if (int e = mlp_backward(h->nets[P.which], in, h->dout.as<float>(), wsp, &gd, h->num_sms, md, st, &h->launches, 1)) return e;
       continue;
     }
-    // sub-chunks of `waves` full waves of 128-point row blocks (148 SMs): bounds the activation workspace (~20 KB per point)
+    // sub-chunks of `waves` full waves of 128-point row blocks (one per SM): bounds the activation workspace (~20 KB per point)
     static const int waves = [] { const char* e = getenv("NM_TRAIN_WAVES"); int v = e ? atoi(e) : 0; return v > 0 ? v : 16; }();
     long long rays_sub = ((long long)h->num_sms * 128 * waves) / P.s;
     if (rays_sub < 1) rays_sub = 1;
@@ -646,15 +647,16 @@ int nm_get_grad(NmHandle h, int which, const char* name, float* out_dev, int64_t
   return -1;
 }
 
-int nm_debug_gemm(NmHandle h, const float* a_dev, const float* b_dev, int M, int N, int K, int a_cols, int b_cols,
-                  int k_split, int n_passes, int fp16, int atomic, float* d_dev, void* stream) {
+int nm_debug_gemm(NmHandle h, const float* a_dev, const float* b_dev, int M, int N, int K, int n_passes, float* d_dev,
+                  void* stream) {
   if (int e = bind_device(h)) return e;
   NM_CHECK(a_dev && b_dev && d_dev && M > 0 && N > 0 && K > 0, "bad arguments");
-  const size_t need = 3 * ((size_t)((M > N ? M : N) + 127) / 128 * ((K + 63) / 64) * 32768 + 1024) + 1024;
-  if (int e = h->train_ws.ensure(need)) return e;
+  NM_CHECK(n_passes == 1 || n_passes == 3, "n_passes must be 1 or 3");
+  const size_t need = pack_bytes(M, K) + pack_bytes(N, K);
+  if (int e = h->train_ws.ensure(need + 1024)) return e;
   uint8_t* ws = reinterpret_cast<uint8_t*>(((uintptr_t)h->train_ws.p + 1023) & ~(uintptr_t)1023);
-  return debug_tc_gemm(a_dev, b_dev, M, N, K, a_cols, b_cols, k_split, n_passes, fp16, atomic, d_dev, ws, need - 1024, h->num_sms,
-                       h->d_err, (cudaStream_t)stream, &h->launches);
+  return debug_tc_gemm(a_dev, b_dev, M, N, K, n_passes, d_dev, ws, need, h->num_sms, h->d_err, (cudaStream_t)stream,
+                       &h->launches);
 }
 
 // ---------------------------------------------------------------------------------------------- BuFF tree maintenance

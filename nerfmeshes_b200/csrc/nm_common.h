@@ -44,12 +44,6 @@ struct NetDev {
   float* d_wt = nullptr;             // transposed fp32 weights (CUDA-core kernel)
   float* d_w = nullptr;              // the same weights in the reference's (out,in) layout, same per-layer offsets
   size_t n_wt = 0;                   // floats in d_wt
-  // training backward on the tensor cores (nm_gemm_tc.cu): bf16 hi/lo operand packs of W (forward) and W^T (data
-  // gradient) per layer, rebuilt lazily after every weight load
-  uint8_t* d_tcw = nullptr;
-  size_t tcw_bytes = 0;
-  size_t tcw_fwd_off[kMaxLayers] = {}, tcw_bwd_off[kMaxLayers] = {};
-  bool tcw_valid = false;
   // fused data-gradient chain (nm_mlp_tc.cu, mode 2): backward program + W^T stages (bf16 hi/lo), rebuilt lazily
   NetProgram bwd{};
   NetProgram* d_bwd = nullptr;
@@ -98,7 +92,8 @@ struct MlpInput {
 
 // Optional by-products of a fused-MLP launch for the training backward (nm_train.cu): per layer (nullptr = not wanted)
 //   packT  the layer's output as the point-major bf16 hi/lo operand pack of the weight-gradient GEMM (nm_gemm.h: tiles of
-//          128 features x 64 points, [feature block][point block], `kbt` point blocks per feature block; rows >= M zero)
+//          128 features x 64 points, [feature block][point block], `kbt` point blocks per feature block; rows >= M zero),
+//          K-major from the training forward (mode 1), MN-major from the data-gradient chain (mode 2)
 //   bits   its relu mask, one bit per element (halfword [m * n_out/16 + n/16], bit n%16)
 //   act    its fp32 value (M, n_out) row-major (the layers the SIMT head kernels read)
 struct MlpEmit {
@@ -106,7 +101,6 @@ struct MlpEmit {
   uint32_t* bits[kMaxLayers];
   float* act[kMaxLayers];
   int kbt;
-  int mn;      // packT as MN-major tiles (bulk stores from a shared-memory staging block) instead of K-major ones
 };
 
 int build_programs(const NmNetDesc& d, NetProgram* full, NetProgram* sigma);
@@ -135,7 +129,7 @@ int launch_mlp_tc(const NetDev& net, bool sigma_only, int n_passes, int act_scal
                   int num_sms, int* d_err, cudaStream_t st, int64_t* launches, const MlpEmit* emit = nullptr,
                   const CompositeArgs* comp = nullptr);
 int launch_mlp_tc_bwd(const NetDev& net, long long M, const float* dz_in, int dz_ld, const float* dout,
-                      const MlpEmit& io, int n_passes, int num_sms, int* d_err, cudaStream_t st, int64_t* launches, int emit_mn = 0);
+                      const MlpEmit& io, int n_passes, int num_sms, int* d_err, cudaStream_t st, int64_t* launches);
 int launch_mlp_simt(const NetDev& net, bool sigma_only, const MlpInput& in, float* out, cudaStream_t st,
                     int64_t* launches);
 
@@ -182,11 +176,7 @@ size_t train_ws_bytes(const NetProgram& full, long long points, bool use_tc);
 struct TrainMode { int use_tc; int n_passes; int* d_err; };
 int mlp_backward(NetDev& net, const MlpInput& in, const float* dout, float* ws, NetGrads* g, int num_sms,
                  const TrainMode& mode, cudaStream_t st, int64_t* launches, int have_acts = 0);
-bool train_fused(bool use_tc);
 void train_emit_setup(const NetProgram& full, long long points, float* ws, MlpEmit* emit);
-int debug_tc_gemm(const float* A, const float* B, int M, int N, int K, int a_cols, int b_cols, int k_split, int n_passes,
-                  int fp16, int atomic, float* D, uint8_t* scratch, size_t scratch_bytes, int num_sms, int* d_err, cudaStream_t st,
-                  int64_t* launches);
 int launch_composite_backward(const float* raw, const float* t, const float* dirs, const float* d_rgb, long long R, int S,
                               float noise_std, uint64_t seed, int white_bg, float* scratch, float* dout,
                               cudaStream_t st, int64_t* launches);

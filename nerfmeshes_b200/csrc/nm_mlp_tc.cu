@@ -75,7 +75,6 @@ struct TcParams {
   const float* dz_in;     // (M, dz_ld) fp32: dZ of the last forward layer
   int dz_ld;
   const float* dout;      // (M, 4): compositor adjoint, column 3 = d sigma
-  int emit_mn;            // modes 1 / 2: packs as MN-major tiles instead of K-major ones
   // fused compositor (mode 0, ray inputs): the last layer's (rgb, sigma) of a tile are staged in shared memory instead of
   // going to `out`; the warpgroup composites every ray in sample order (nm_composite.cuh) and writes the per-ray maps.
   int comp_on;
@@ -310,11 +309,12 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
   };
 
   // point-major bf16 hi/lo pack of the weight-gradient GEMM: features f, f+1 of point pt (nm_gemm.h ptiles of 128 features
-  // x 64 points, K-major: row f % 128, 16-byte chunk ((pt % 64) / 8) ^ (f % 8); MN-major: feature group (f % 128) / 64,
-  // point row pt % 64, chunk ((f % 64) / 8) ^ (pt % 8))
+  // x 64 points).  Mode 2 (dZ, the GEMM's A operand) writes MN-major tiles: feature group (f % 128) / 64, point row pt % 64,
+  // chunk ((f % 64) / 8) ^ (pt % 8); mode 1 (activations, its B operand) K-major ones: row f % 128, 16-byte chunk
+  // ((pt % 64) / 8) ^ (f % 8)
   auto emit_pack = [&](uint8_t* packT, int f, long long pt, uint32_t hi2, uint32_t lo2) {
     uint8_t* tb = packT + ((size_t)(f >> 7) * (size_t)P.emit.kbt + (size_t)(pt >> 6)) * 32768u;
-    if (P.emit_mn) {
+    if (MODE == 2) {
       const uint32_t off = (uint32_t)((f & 127) >> 6) * 8192u + (uint32_t)(pt & 63) * 128u +
                            ((((uint32_t)(f & 63) >> 3) ^ (uint32_t)(pt & 7)) << 4) + (uint32_t)(f & 7) * 2u;
       *reinterpret_cast<uint32_t*>(tb + off) = hi2;
@@ -632,7 +632,7 @@ int launch_mlp_tc(const NetDev& net, bool sigma_only, int n_passes, int act_scal
   P.n_tiles = (in.M + kTileM - 1) / kTileM;
   P.err = d_err;
   if (emit) {
-    P.has_emit = 1; P.emit = *emit; P.emit_mn = emit->mn;
+    P.has_emit = 1; P.emit = *emit;
     P.n_tiles = 2 * ((in.M + 127) / 128);      // the packs hold whole 128-point blocks: their zero rows are written too
   }
   P.tile_group = 1;
@@ -650,7 +650,7 @@ int launch_mlp_tc(const NetDev& net, bool sigma_only, int n_passes, int act_scal
 // forward layer; for every backward layer li (net.bwd): io.bits[li] = relu mask to apply (input), io.packT[li] = where dZ
 // goes as the weight-gradient operand (its row sums there are the bias gradients: launch_tc_gemm a_rowsum).
 int launch_mlp_tc_bwd(const NetDev& net, long long M, const float* dz_in, int dz_ld, const float* dout,
-                      const MlpEmit& io, int n_passes, int num_sms, int* d_err, cudaStream_t st, int64_t* launches, int emit_mn) {
+                      const MlpEmit& io, int n_passes, int num_sms, int* d_err, cudaStream_t st, int64_t* launches) {
   if (M <= 0) return 0;
   NM_CHECK(net.bwd_valid && net.d_wpack_bwd, "backward weight stream not built");
   NM_CHECK((dz_ld & 1) == 0 && (reinterpret_cast<uintptr_t>(dz_in) & 7) == 0, "dz_in must be 8-byte aligned rows");
@@ -665,7 +665,7 @@ int launch_mlp_tc_bwd(const NetDev& net, long long M, const float* dz_in, int dz
   P.n_tiles = 2 * ((M + 127) / 128);
   P.err = d_err;
   P.has_emit = 1; P.emit = io;
-  P.mode = 2; P.dz_in = dz_in; P.dz_ld = dz_ld; P.dout = dout; P.emit_mn = emit_mn;
+  P.mode = 2; P.dz_in = dz_in; P.dz_ld = dz_ld; P.dout = dout;
   return launch_prepared(P, num_sms, st, launches);
 }
 

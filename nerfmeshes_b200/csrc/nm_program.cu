@@ -292,7 +292,7 @@ int debug_pack(const NmNetDesc& d, const WeightSource& src, bool sigma_only, Net
 
 void free_network(NetDev* net) {
   cudaFree(net->d_full); cudaFree(net->d_sigma); cudaFree(net->d_wpack_full); cudaFree(net->d_wpack_sigma);
-  cudaFree(net->d_bias); cudaFree(net->d_head); cudaFree(net->d_wt); cudaFree(net->d_w); cudaFree(net->d_tcw);
+  cudaFree(net->d_bias); cudaFree(net->d_head); cudaFree(net->d_wt); cudaFree(net->d_w);
   cudaFree(net->d_bwd); cudaFree(net->d_wpack_bwd);
   *net = NetDev{};
 }
@@ -487,7 +487,6 @@ int load_network_dev(const NmNetDesc& d, const WeightSource& src, NetDev* net, c
   pack_stream_kernel<<<sig.n_blocks, 256, 0, st>>>(net->d_sigma, net->d_w, net->d_wpack_sigma);
   NM_CUDA(cudaGetLastError());
   if (launches) *launches += 2;
-  net->tcw_valid = false;
   net->bwd_valid = false;
   net->loaded = true;
   return 0;

@@ -3,22 +3,20 @@
 // through VolumeRenderer (src/nerf/modules.py:67-121), the network (src/nerf/models.py:60-80) and nothing else
 // (SamplePDF is detached, modules.py:201; sample positions do not depend on θ).
 //
-// Default (tensor cores, DESIGN.md 4.4): the training forward is the fused kernel in its emitting mode (nm_mlp_tc.cu mode 1:
-// relu masks, head activations, point-major operand packs of every hidden activation) — for the whole chunk when its
+// Tensor cores (default, DESIGN.md 4.4): the training forward is the fused kernel in its emitting mode (nm_mlp_tc.cu mode 1:
+// relu masks, head activations, K-major operand packs of every hidden activation) — for the whole chunk when its
 // workspace fits (no recompute), else per sub-chunk of points; the data-gradient chain
 //     dZ_{l-1} = (dZ_l W_l (+ dsigma w_alpha)) * relu'_{l-1}
-// of ALL layers is one more launch of that kernel (mode 2); the weight gradients
+// of ALL layers is one more launch of that kernel (mode 2, MN-major operand packs of every dZ); the weight gradients
 //     dW_l += dZ_l^T [act_{l-1} | PE]                    (K = points: split over CTAs, fp32 atomics)
 // are long-K launches of tc_gemm_kernel (nm_gemm_tc.cu) on the packs, which also take the bias gradients (row sums of the
-// staged dZ^T tiles).  NM_TRAIN_LAYERWISE=1: round 1's walk, every layer's forward / data gradient as its own tc_gemm launch.
-// NM_PREC_FP32: the same walk in plain fp32 FMAs on the CUDA cores (sgemm_kernel / sgemm_tn_kernel below; the
-// reference trains in fp32, TF32 off) — the numerical yard-stick the tensor-core path is tested against.
+// staged dZ^T tiles).
+// NM_PREC_FP32: the network walked layer by layer in plain fp32 FMAs on the CUDA cores (sgemm_kernel / sgemm_tn_kernel
+// below; the reference trains in fp32, TF32 off) — the numerical yard-stick the tensor-core path is tested against.
 // Small SIMT kernels around them: encodings, the 3-/4-row heads, the compositor adjoint, the MSE gradient.
 // Gradients accumulate in the reference's (out,in) orientation (rows padded to 4 floats, grad_layout()); nm_get_grad
 // returns them per state-dict tensor.
 #include <math_constants.h>
-
-#include <cstdlib>
 
 #include <cuda_bf16.h>
 
@@ -100,6 +98,18 @@ __global__ void __launch_bounds__(256) encode_pack_kernel(const __grid_constant_
 // ------------------------------------------------------------------------------------------------ SGEMM  C = A * op(B)
 // A (M,K) row-major.  BT=false: B (K,N) row-major;  BT=true: B (N,K) row-major (C = A B^T).
 // CTA tile 128 x (16*TN), 256 threads, 8 x TN micro-tile, BK = 16, register prefetch of the next K tile.
+
+// fused epilogue: v = acc (+C) (+bias[n]) (+r1_vec[m]*r1_w[n]); relu; relu-mask of another tensor
+struct GemmEpi {
+  int accumulate;          // C += (else C =)
+  const float* bias;       // + bias[n]
+  int relu;                // max(.,0)
+  const float* r1_vec;     // + r1_vec[m * r1_stride] * r1_w[n]
+  int r1_stride;
+  const float* r1_w;
+  const float* mask;       // * (mask[m*ldmask + n] > 0)
+  int ldmask;
+};
 
 template <int TN, bool BT>
 __global__ void __launch_bounds__(256) sgemm_kernel(const float* __restrict__ A, int lda, const float* __restrict__ B,
@@ -568,6 +578,7 @@ __global__ void mse_grad_kernel(const float* __restrict__ rgb, const float* __re
 
 }  // namespace
 
+
 // ------------------------------------------------------------------------------------------------ host side
 namespace {
 
@@ -577,86 +588,43 @@ size_t up(size_t x) { return (x + kAlign - 1) / kAlign * kAlign; }
 // workspace carving for one sub-chunk of P points (all regions 1 KB aligned; ptile packs need it)
 struct TrainWs {
   float *pe_x, *pe_d, *dbuf[2], *act[kMaxLayers];
-  uint8_t *pk_a[2], *pk_pex, *pk_ped, *pkt_a, *pkt_act[kMaxLayers], *pkt_pex, *pkt_ped;
-  uint8_t* pkt_dz[kMaxLayers];    // point-major bf16 packs of every layer's dZ (fused data-gradient chain: A operands of dW)
-  uint16_t* bits[kMaxLayers];     // relu masks of the recomputed activations, 1 bit per element (tensor-core path)
+  uint8_t *pkt_act[kMaxLayers], *pkt_pex, *pkt_ped;   // K-major bf16 packs of the activations / encodings (B operands of dW)
+  uint8_t* pkt_dz[kMaxLayers];    // MN-major bf16 packs of every layer's dZ (A operands of dW)
+  uint16_t* bits[kMaxLayers];     // relu masks of the forward's activations, 1 bit per element
   size_t bytes;
 };
-bool train_layerwise() {
-  static const bool v = [] { const char* e = getenv("NM_TRAIN_LAYERWISE"); return e && atoi(e) != 0; }();
-  return v;
-}
 
 TrainWs carve(const NetProgram& G, long long P, bool use_tc, uint8_t* base) {
   TrainWs w{};
   size_t off = 0;
   auto take = [&](size_t bytes) { uint8_t* p = base ? base + off : nullptr; off += up(bytes); return p; };
   const int h = G.hidden;
-  const bool fused = use_tc && !train_layerwise();    // fused chains: no row packs, fp32 activations only where the heads read them
-  if (!fused) {
-    w.pe_x = (float*)take((size_t)P * kPeLd * 4);
-    w.pe_d = (float*)take((size_t)P * kPeLd * 4);
-  }
-  w.dbuf[0] = (float*)take((size_t)P * h * 4);
-  if (!fused) w.dbuf[1] = (float*)take((size_t)P * h * 4);
-  for (int l = 0; l < G.n_layers; ++l)
-    if (!fused || G.layers[l].kind != KIND_HIDDEN) w.act[l] = (float*)take((size_t)P * G.layers[l].n_out * 4);
   if (use_tc) {
-    if (!fused) {
-      w.pk_a[0] = take(pack_bytes((int)P, h));
-      w.pk_a[1] = take(pack_bytes((int)P, h));
-      w.pk_pex = take(pack_bytes((int)P, kPeLd));
-      w.pk_ped = take(pack_bytes((int)P, kPeLd));
-    }
+    // fp32 only where the SIMT head kernels read or write (dZ of the last layer, the activations under a head); the rest
+    // lives in the operand packs and relu masks
+    w.dbuf[0] = (float*)take((size_t)P * h * 4);
+    for (int l = 0; l < G.n_layers; ++l)
+      if (G.layers[l].kind != KIND_HIDDEN) w.act[l] = (float*)take((size_t)P * G.layers[l].n_out * 4);
     const int P128 = (int)((P + 127) / 128) * 128;     // K blocks of the point-major packs come in pairs (one per 128-row tile)
-    if (!fused) w.pkt_a = take(pack_bytes(h, P128));
     for (int l = 0; l + 1 < G.n_layers; ++l) w.pkt_act[l] = take(pack_bytes(G.layers[l].n_out, P128));
     w.pkt_pex = take(pack_bytes(kPeLd, P128));
     w.pkt_ped = take(pack_bytes(kPeLd, P128));
     for (int l = 0; l < G.n_layers; ++l) w.bits[l] = (uint16_t*)take((size_t)P * (G.layers[l].n_out / 16) * 2);
     for (int l = 0; l < G.n_layers; ++l) w.pkt_dz[l] = take(pack_bytes(G.layers[l].n_out, P128));
+  } else {
+    w.pe_x = (float*)take((size_t)P * kPeLd * 4);
+    w.pe_d = (float*)take((size_t)P * kPeLd * 4);
+    w.dbuf[0] = (float*)take((size_t)P * h * 4);
+    w.dbuf[1] = (float*)take((size_t)P * h * 4);
+    for (int l = 0; l < G.n_layers; ++l) w.act[l] = (float*)take((size_t)P * G.layers[l].n_out * 4);
   }
   w.bytes = off;
   return w;
 }
 
-// bf16 hi/lo packs of W (rows = out features, K = in features) and of W^T restricted to the activation inputs
-// (rows = in features, K = out features) for every layer
-int build_weight_packs(NetDev& net, cudaStream_t st, int64_t* launches) {
-  const NetProgram& G = net.full;
-  size_t total = 0;
-  for (int l = 0; l < G.n_layers; ++l) {
-    const LayerProg& L = G.layers[l];
-    net.tcw_fwd_off[l] = total; total += pack_bytes(L.n_out, L.k_act + L.k_pe);
-    net.tcw_bwd_off[l] = total; total += L.k_act > 0 ? pack_bytes(L.k_act, L.n_out) : 0;
-  }
-  if (net.tcw_bytes < total) {
-    cudaFree(net.d_tcw);
-    net.d_tcw = nullptr; net.tcw_bytes = 0;
-    NM_CUDA(cudaMalloc(&net.d_tcw, total));
-    net.tcw_bytes = total;
-  }
-  for (int l = 0; l < G.n_layers; ++l) {
-    const LayerProg& L = G.layers[l];
-    const int K = L.k_act + L.k_pe;
-    if (int e = launch_pack_rows(net.d_w + L.wt_off, K, L.n_out, K, net.d_tcw + net.tcw_fwd_off[l], 1, st, launches)) return e;
-    if (L.k_act > 0)
-      if (int e = launch_pack_rows(net.d_wt + L.wt_off, L.n_out, L.k_act, L.n_out, net.d_tcw + net.tcw_bwd_off[l], 0, st, launches)) return e;
-  }
-  net.tcw_valid = true;
-  return 0;
-}
-
 }  // namespace
 
 size_t train_ws_bytes(const NetProgram& G, long long points, bool use_tc) { return carve(G, points, use_tc, nullptr).bytes; }
-
-bool train_fused(bool use_tc) { return use_tc && !train_layerwise(); }
-// NM_TRAIN_ACT_MN=1: the training forward writes its activation packs as MN-major tiles too (64 KB of staging out of the weight ring)
-int train_act_mn() {
-  static const int v = [] { const char* e = getenv("NM_TRAIN_ACT_MN"); return (e && atoi(e) != 0) ? 1 : 0; }();
-  return v;
-}
 
 // The by-products a training forward must leave in `ws` (same carving as mlp_backward) so that the backward can skip its
 // recompute launch: see MlpEmit.
@@ -664,7 +632,6 @@ void train_emit_setup(const NetProgram& G, long long P, float* ws_base, MlpEmit*
   const TrainWs W = carve(G, P, true, reinterpret_cast<uint8_t*>(ws_base));
   *E = MlpEmit{};
   E->kbt = 2 * (int)((P + 127) / 128);
-  E->mn = train_act_mn();
   for (int l = 0; l < G.n_layers; ++l) {
     const LayerProg& L = G.layers[l];
     if (l + 1 < G.n_layers) E->packT[l] = W.pkt_act[l];
@@ -694,156 +661,117 @@ int launch_mse_grad(const float* rgb, const float* target, long long n, long lon
   return 0;
 }
 
-// Backward of one network over P = in.M points.  dout (P,4).  ws: train_ws_bytes(full, P, use_tc) bytes, 1 KB aligned.
-// Weight gradients accumulate in the reference's (out,in) layout at the offsets of NetDev.d_w.
-int mlp_backward(NetDev& net, const MlpInput& in, const float* dout, float* ws_base, NetGrads* g, int num_sms,
-                 const TrainMode& mode, cudaStream_t st, int64_t* launches, int have_acts) {
+namespace {
+
+// Tensor cores: ONE launch of the fused forward kernel (nm_mlp_tc.cu, mode 1) leaves what the backward needs — relu masks,
+// the bf16 packs of every hidden activation and the fp32 activations the head kernels read — unless the training forward
+// already did (have_acts); the SIMT heads produce dZ of the last layer; ONE launch of the fused kernel on the backward
+// program (mode 2) walks the data gradient down the whole network with dZ in shared memory (W^T streamed through shared
+// memory, relu masks from the forward, the rank-1 d sigma term) and leaves every layer's dZ as the pack the long-K
+// weight-gradient GEMMs consume — no per-layer round trip of dZ through HBM.
+int backward_tc(NetDev& net, const MlpInput& in, const float* dout, float* ws_base, NetGrads* g, int num_sms,
+                const TrainMode& mode, cudaStream_t st, int64_t* launches, int have_acts) {
   const NetProgram& G = net.full;
   const int P = (int)in.M;
-  if (P <= 0) return 0;
-  const bool tc = mode.use_tc != 0;
-  TrainWs W = carve(G, P, tc, reinterpret_cast<uint8_t*>(ws_base));
-  if (tc && !net.tcw_valid)
-    if (int e = build_weight_packs(net, st, launches)) return e;
+  const TrainWs W = carve(G, P, true, reinterpret_cast<uint8_t*>(ws_base));
   const int kbtP = 2 * ((P + 127) / 128);      // K blocks of the point-major packs (zero-filled beyond P)
-
-  if (tc && !train_layerwise()) {               // fused chains: the encodings are needed as weight-gradient operands only
-    NM_CHECK(G.dim_xyz <= kPeLd && G.dim_dir <= kPeLd, "encoding wider than %d", kPeLd);
-    encode_pack_kernel<<<kbtP, 256, 0, st>>>(in, net.d_full, W.pkt_pex, W.pkt_ped);
-    NM_CUDA(cudaGetLastError());
-    if (launches) ++*launches;
-  } else {
-    encode_kernel<<<(P + 127) / 128, 128, 0, st>>>(in, net.d_full, W.pe_x, W.pe_d);
-    NM_CUDA(cudaGetLastError());
-    if (launches) ++*launches;
-    if (tc) {                                   // layer-wise chain: row packs feed the forward GEMMs, column packs the dW GEMMs
-      if (int e = launch_pack_rows(W.pe_x, kPeLd, P, G.dim_xyz, W.pk_pex, 1, st, launches)) return e;
-      if (int e = launch_pack_cols(W.pe_x, kPeLd, P, G.dim_xyz, W.pkt_pex, kbtP, 0, st, launches)) return e;
-      if (G.dim_dir > 0) {
-        if (int e = launch_pack_rows(W.pe_d, kPeLd, P, G.dim_dir, W.pk_ped, 1, st, launches)) return e;
-        if (int e = launch_pack_cols(W.pe_d, kPeLd, P, G.dim_dir, W.pkt_ped, kbtP, 0, st, launches)) return e;
-      }
-    }
-  }
-  auto pe_of = [&](const LayerProg& L) { return L.pe_src == SRC_PE_XYZ ? W.pe_x : W.pe_d; };
-  auto pk_pe_of = [&](const LayerProg& L) { return L.pe_src == SRC_PE_XYZ ? W.pk_pex : W.pk_ped; };
-  auto pkt_pe_of = [&](const LayerProg& L) { return L.pe_src == SRC_PE_XYZ ? W.pkt_pex : W.pkt_ped; };
-  auto tc_base = [&]() { TcGemmParams T{}; T.n_passes = mode.n_passes; T.err = mode.d_err; return T; };
-
-  // ---- forward recompute: act[l] = act_l([act[l-1] | PE] W^T + b)
-  // Tensor-core path: ONE launch of the fused forward kernel (nm_mlp_tc.cu) whose epilogue also emits what the backward
-  // needs — relu masks, the point-major bf16 packs of every hidden activation (B operand of the weight-gradient GEMMs) and
-  // the fp32 activations the head kernels read — instead of a chain of layer GEMMs round-tripping through HBM.  The masks
-  // are by construction the forward pass's own.  NM_TRAIN_LAYERWISE=1 keeps the layer-by-layer GEMM chain (debugging).
-  const bool layerwise = train_layerwise();
-  if (tc && !layerwise && !have_acts) {       // have_acts: the training forward itself already left them in `ws` (nm_api.cu)
+  NM_CHECK(G.dim_xyz <= kPeLd && G.dim_dir <= kPeLd, "encoding wider than %d", kPeLd);
+  encode_pack_kernel<<<kbtP, 256, 0, st>>>(in, net.d_full, W.pkt_pex, W.pkt_ped);
+  NM_CUDA(cudaGetLastError());
+  if (launches) ++*launches;
+  if (!have_acts) {
     MlpEmit E{};
     train_emit_setup(G, P, ws_base, &E);
     if (int e = launch_mlp_tc(net, false, mode.n_passes, 0, in, nullptr, num_sms, mode.d_err, st, launches, &E)) return e;
   }
-  for (int l = 0; l < G.n_layers && !(tc && !layerwise); ++l) {
-    const LayerProg& L = G.layers[l];
-    const int N = L.n_out, Kt = L.k_act + L.k_pe;
-    GemmEpi fin{};
-    fin.bias = net.d_bias + L.bias_off; fin.relu = L.relu;
-    if (tc) {
-      TcGemmParams T = tc_base();
-      const uint8_t* wp = net.d_tcw + net.tcw_fwd_off[l];
-      const int kbtW = (Kt + 63) / 64;
-      int ns = 0;
-      if (L.k_act > 0)      // the previous layer's epilogue left its output here as an fp16 row pack
-        T.seg[ns++] = TcSeg{W.pk_a[l & 1], L.k_act / 64, wp, kbtW, L.k_act / 64};
-      if (L.pe_src) T.seg[ns++] = TcSeg{pk_pe_of(L), 1, wp + (size_t)(L.k_act / 64) * kPtileBytes, kbtW, 1};
-      T.nseg = ns; T.D = W.act[l]; T.ldd = N; T.M = P; T.N = N; T.epi = fin;
-      T.fp16 = 1;      // forward recompute in the forward kernel's precision class (relu masks must agree with it)
-      if (l + 1 < G.n_layers) {      // the next layer's A operand, and the B^T operand of its weight gradient
-        T.pack_out = W.pk_a[(l + 1) & 1]; T.pack_kbt = N / 64; T.pack_fp16 = 1;
-        T.packT_out = W.pkt_act[l]; T.packT_kbt = kbtP;
-      }
-      if (L.relu) { T.bits_out = W.bits[l]; T.bits_ld = N / 16; }
-      // fp32 activations are only read by the SIMT head kernels (trunk output for fc_alpha, last layer for fc_rgb / fc_out)
-      T.skip_d = (L.kind == KIND_HIDDEN) ? 1 : 0;
-      if (int e = launch_tc_gemm(T, num_sms, st, launches)) return e;
-    } else {
-      const float* Wt = net.d_wt + L.wt_off;
-      if (L.k_act > 0) {
-        GemmEpi e0 = L.pe_src ? GemmEpi{} : fin;
-        if (int rc = sgemm<false>(W.act[l - 1], G.layers[l - 1].n_out, Wt, N, W.act[l], N, P, N, L.k_act, e0, st, launches)) return rc;
-      }
-      if (L.pe_src) {
-        fin.accumulate = L.k_act > 0 ? 1 : 0;
-        if (int rc = sgemm<false>(pe_of(L), kPeLd, Wt + (size_t)L.k_act * N, N, W.act[l], N, P, N, L.k_pe, fin, st, launches)) return rc;
-      }
-    }
-  }
 
-  // ---- backward
   size_t gw_off[kMaxLayers];
   int gw_ld[kMaxLayers];
   grad_layout(G, gw_off, gw_ld);
-  if (tc && !layerwise) {
-    // Fused: the SIMT heads produce dZ of the last layer; ONE launch of the fused kernel on the backward program walks the
-    // data gradient down the whole network with dZ in shared memory (W^T streamed through shared memory, relu masks from the recompute,
-    // the rank-1 d sigma term, bias gradients as column sums) and leaves every layer's dZ as the point-major pack the
-    // long-K weight-gradient GEMMs consume — no per-layer round trip of dZ / masks / row packs through HBM.
-    if (!net.bwd_valid)
-      if (int e = build_backward_stream(&net, st, launches)) return e;
-    const int last = G.n_layers - 1;
-    const LayerProg& Ltop = G.layers[last];
-    NM_CHECK(Ltop.kind == KIND_RGB || Ltop.kind == KIND_OUT4, "the last layer must carry the colour head");
-    const int p_per_block = (P + 8 * num_sms - 1) / (8 * num_sms);
-    const int hb_blocks = (P + p_per_block - 1) / p_per_block;
-    NM_CHECK((Ltop.n_out & 3) == 0 && Ltop.n_out <= 1024 && (G.hidden & 3) == 0 && G.hidden <= 1024, "head widths must be multiples of 4, <= 1024");
-    float* dZ = W.dbuf[0];
-    head_backward_kernel<<<hb_blocks, 256, 0, st>>>(dout, 0, Ltop.kind == KIND_RGB ? 3 : 4, W.act[last], Ltop.n_out, P,
-                                                   net.d_head + Ltop.head_off, g->head + Ltop.head_off, dZ, Ltop.relu, p_per_block,
-                                                   g->bias + Ltop.bias_off);
+  if (!net.bwd_valid)
+    if (int e = build_backward_stream(&net, st, launches)) return e;
+  const int last = G.n_layers - 1;
+  const LayerProg& Ltop = G.layers[last];
+  NM_CHECK(Ltop.kind == KIND_RGB || Ltop.kind == KIND_OUT4, "the last layer must carry the colour head");
+  const int p_per_block = (P + 8 * num_sms - 1) / (8 * num_sms);
+  const int hb_blocks = (P + p_per_block - 1) / p_per_block;
+  NM_CHECK((Ltop.n_out & 3) == 0 && Ltop.n_out <= 1024 && (G.hidden & 3) == 0 && G.hidden <= 1024, "head widths must be multiples of 4, <= 1024");
+  float* dZ = W.dbuf[0];
+  head_backward_kernel<<<hb_blocks, 256, 0, st>>>(dout, 0, Ltop.kind == KIND_RGB ? 3 : 4, W.act[last], Ltop.n_out, P,
+                                                 net.d_head + Ltop.head_off, g->head + Ltop.head_off, dZ, Ltop.relu, p_per_block,
+                                                 g->bias + Ltop.bias_off);
+  NM_CUDA(cudaGetLastError());
+  if (launches) ++*launches;
+  for (int l = 0; l < last; ++l) {
+    const LayerProg& L = G.layers[l];
+    if (L.kind != KIND_SIGMA) continue;       // weight / bias gradient of fc_alpha (its data-gradient term is in the chain)
+    head_backward_kernel<<<hb_blocks, 256, 0, st>>>(dout, 3, 1, W.act[l], L.n_out, P, net.d_head + L.head_off,
+                                                   g->head + L.head_off, nullptr, 0, p_per_block, nullptr);
     NM_CUDA(cudaGetLastError());
     if (launches) ++*launches;
-    for (int l = 0; l < last; ++l) {
-      const LayerProg& L = G.layers[l];
-      if (L.kind != KIND_SIGMA) continue;       // weight / bias gradient of fc_alpha (its data-gradient term is in the chain)
-      head_backward_kernel<<<hb_blocks, 256, 0, st>>>(dout, 3, 1, W.act[l], L.n_out, P, net.d_head + L.head_off,
-                                                     g->head + L.head_off, nullptr, 0, p_per_block, nullptr);
-      NM_CUDA(cudaGetLastError());
-      if (launches) ++*launches;
-    }
-    MlpEmit io{};
-    io.kbt = kbtP;
-    io.packT[0] = W.pkt_dz[last];               // the chain's load stage emits the top dZ's pack too
-    for (int li = 1; li < net.bwd.n_layers; ++li) {
-      const int l = net.bwd.layers[li].aux;      // this backward layer streams W_l^T and produces dZ of forward layer l-1
-      io.packT[li] = W.pkt_dz[l - 1];
-      if (G.layers[l - 1].relu) io.bits[li] = reinterpret_cast<uint32_t*>(W.bits[l - 1]);
-    }
-    // dZ packs as MN-major tiles through per-warp bulk stores (NM_TRAIN_DZ_MN=0: K-major tiles, 2-byte stores)
-    const char* dz_env = getenv("NM_TRAIN_DZ_MN");       // read per call: the tests cover both layouts
-    const int dz_mn = (!dz_env || atoi(dz_env) != 0) ? 1 : 0;
-    if (int e = launch_mlp_tc_bwd(net, P, dZ, Ltop.n_out, dout, io, mode.n_passes, num_sms, mode.d_err, st, launches, dz_mn)) return e;
-    for (int l = last; l >= 0; --l) {            // weight gradients dW (N, Kt) += dZ^T [act[l-1] | PE]: long-K GEMMs, fp32 atomics
-      const LayerProg& L = G.layers[l];
-      TcGemmParams T = tc_base();
-      T.nseg = 1; T.atomic = 1; T.ldd = gw_ld[l]; T.M = L.n_out;
-      // bias gradient = row sums of dZ^T, taken by the first GEMM that stages this layer's dZ pack (the top layer's comes
-      // from head_backward_kernel)
-      T.a_rowsum = l < last ? g->bias + L.bias_off : nullptr;
-      if (L.k_act > 0) {
-        T.seg[0] = TcSeg{W.pkt_dz[l], kbtP, W.pkt_act[l - 1], kbtP, kbtP, dz_mn | (train_act_mn() << 1)};
-        T.D = g->w + gw_off[l]; T.N = L.k_act;
-        if (int e = launch_tc_gemm(T, num_sms, st, launches)) return e;
-        T.a_rowsum = nullptr;
-      }
-      if (L.pe_src) {
-        T.seg[0] = TcSeg{W.pkt_dz[l], kbtP, pkt_pe_of(L), kbtP, kbtP, dz_mn};
-        T.D = g->w + gw_off[l] + L.k_act; T.N = L.k_pe;
-        if (int e = launch_tc_gemm(T, num_sms, st, launches)) return e;
-      }
-    }
-    return 0;
   }
+  MlpEmit io{};
+  io.kbt = kbtP;
+  io.packT[0] = W.pkt_dz[last];               // the chain's load stage emits the top dZ's pack too
+  for (int li = 1; li < net.bwd.n_layers; ++li) {
+    const int l = net.bwd.layers[li].aux;      // this backward layer streams W_l^T and produces dZ of forward layer l-1
+    io.packT[li] = W.pkt_dz[l - 1];
+    if (G.layers[l - 1].relu) io.bits[li] = reinterpret_cast<uint32_t*>(W.bits[l - 1]);
+  }
+  if (int e = launch_mlp_tc_bwd(net, P, dZ, Ltop.n_out, dout, io, mode.n_passes, num_sms, mode.d_err, st, launches)) return e;
+  for (int l = last; l >= 0; --l) {            // weight gradients dW (N, Kt) += dZ^T [act[l-1] | PE]: long-K GEMMs, fp32 atomics
+    const LayerProg& L = G.layers[l];
+    TcGemmParams T{};
+    T.a = W.pkt_dz[l]; T.kbt = kbtP; T.n_passes = mode.n_passes; T.err = mode.d_err;
+    T.ldd = gw_ld[l]; T.M = L.n_out;
+    // bias gradient = row sums of dZ^T, taken by the first GEMM that stages this layer's dZ pack (the top layer's comes
+    // from head_backward_kernel)
+    T.a_rowsum = l < last ? g->bias + L.bias_off : nullptr;
+    if (L.k_act > 0) {
+      T.b = W.pkt_act[l - 1]; T.D = g->w + gw_off[l]; T.N = L.k_act;
+      if (int e = launch_tc_gemm(T, num_sms, st, launches)) return e;
+      T.a_rowsum = nullptr;
+    }
+    if (L.pe_src) {
+      T.b = L.pe_src == SRC_PE_XYZ ? W.pkt_pex : W.pkt_ped; T.D = g->w + gw_off[l] + L.k_act; T.N = L.k_pe;
+      if (int e = launch_tc_gemm(T, num_sms, st, launches)) return e;
+    }
+  }
+  return 0;
+}
+
+// NM_PREC_FP32: forward recompute act[l] = act_l([act[l-1] | PE] W^T + b) and the backward layer by layer, every GEMM in
+// fp32 FMAs on the CUDA cores.
+int backward_fp32(NetDev& net, const MlpInput& in, const float* dout, float* ws_base, NetGrads* g, int num_sms,
+                  cudaStream_t st, int64_t* launches) {
+  const NetProgram& G = net.full;
+  const int P = (int)in.M;
+  const TrainWs W = carve(G, P, false, reinterpret_cast<uint8_t*>(ws_base));
+  encode_kernel<<<(P + 127) / 128, 128, 0, st>>>(in, net.d_full, W.pe_x, W.pe_d);
+  NM_CUDA(cudaGetLastError());
+  if (launches) ++*launches;
+  auto pe_of = [&](const LayerProg& L) { return L.pe_src == SRC_PE_XYZ ? W.pe_x : W.pe_d; };
+
+  for (int l = 0; l < G.n_layers; ++l) {
+    const LayerProg& L = G.layers[l];
+    const int N = L.n_out;
+    GemmEpi fin{};
+    fin.bias = net.d_bias + L.bias_off; fin.relu = L.relu;
+    const float* Wt = net.d_wt + L.wt_off;
+    if (L.k_act > 0) {
+      GemmEpi e0 = L.pe_src ? GemmEpi{} : fin;
+      if (int rc = sgemm<false>(W.act[l - 1], G.layers[l - 1].n_out, Wt, N, W.act[l], N, P, N, L.k_act, e0, st, launches)) return rc;
+    }
+    if (L.pe_src) {
+      fin.accumulate = L.k_act > 0 ? 1 : 0;
+      if (int rc = sgemm<false>(pe_of(L), kPeLd, Wt + (size_t)L.k_act * N, N, W.act[l], N, P, N, L.k_pe, fin, st, launches)) return rc;
+    }
+  }
+
+  size_t gw_off[kMaxLayers];
+  int gw_ld[kMaxLayers];
+  grad_layout(G, gw_off, gw_ld);
   int cur = 0;
-  bool dz_packed = false;      // W.pk_a[cur] already holds the bf16 row pack of dbuf[cur]
-  bool dz_colpacked = false;   // W.pkt_a already holds the point-major bf16 pack of dbuf[cur]
   bool bias_done = false;      // the kernel that produced dbuf[cur] already accumulated its column sums (bias gradient)
   const int p_per_block = (P + 8 * num_sms - 1) / (8 * num_sms);      // 8 CTAs per SM keep enough loads in flight
   const int hb_blocks = (P + p_per_block - 1) / p_per_block;
@@ -871,27 +799,10 @@ int mlp_backward(NetDev& net, const MlpInput& in, const float* dout, float* ws_b
     // weight gradient dW (N, Kt) += dZ^T [act[l-1] | PE], bias gradient
     float* gW = g->w + gw_off[l];
     const int ldg = gw_ld[l];
-    if (tc) {
-      if (!dz_colpacked)
-        if (int e = launch_pack_cols(dZ, N, P, N, W.pkt_a, kbtP, 0, st, launches)) return e;
-      TcGemmParams T = tc_base();
-      T.nseg = 1; T.atomic = 1; T.ldd = ldg; T.M = N;
-      if (L.k_act > 0) {
-        T.seg[0] = TcSeg{W.pkt_a, kbtP, W.pkt_act[l - 1], kbtP, kbtP};
-        T.D = gW; T.N = L.k_act;
-        if (int e = launch_tc_gemm(T, num_sms, st, launches)) return e;
-      }
-      if (L.pe_src) {
-        T.seg[0] = TcSeg{W.pkt_a, kbtP, pkt_pe_of(L), kbtP, kbtP};
-        T.D = gW + L.k_act; T.N = L.k_pe;
-        if (int e = launch_tc_gemm(T, num_sms, st, launches)) return e;
-      }
-    } else {
-      if (L.k_act > 0)
-        if (int rc = sgemm_tn(dZ, N, W.act[l - 1], G.layers[l - 1].n_out, gW, ldg, P, N, L.k_act, num_sms, st, launches)) return rc;
-      if (L.pe_src)
-        if (int rc = sgemm_tn(dZ, N, pe_of(L), kPeLd, gW + L.k_act, ldg, P, N, L.k_pe, num_sms, st, launches)) return rc;
-    }
+    if (L.k_act > 0)
+      if (int rc = sgemm_tn(dZ, N, W.act[l - 1], G.layers[l - 1].n_out, gW, ldg, P, N, L.k_act, num_sms, st, launches)) return rc;
+    if (L.pe_src)
+      if (int rc = sgemm_tn(dZ, N, pe_of(L), kPeLd, gW + L.k_act, ldg, P, N, L.k_pe, num_sms, st, launches)) return rc;
     if (!bias_done) {
       const int ppb = (P + 63) / 64;
       dim3 grid((N + 31) / 32, (P + ppb - 1) / ppb);
@@ -905,66 +816,25 @@ int mlp_backward(NetDev& net, const MlpInput& in, const float* dout, float* ws_b
       NM_CHECK(L.k_act == Lp.n_out, "layer chain mismatch");
       GemmEpi e{};
       if (Lp.kind == KIND_SIGMA) { e.r1_vec = dout + 3; e.r1_stride = 4; e.r1_w = net.d_head + Lp.head_off; }
-      if (Lp.relu && !tc) { e.mask = W.act[l - 1]; e.ldmask = Lp.n_out; }
-      if (tc) {
-        // A = row pack of dZ: written by the previous data-gradient epilogue, or packed here at the head of the chain
-        if (!dz_packed)
-          if (int rc = launch_pack_rows(dZ, N, P, N, W.pk_a[cur], 0, st, launches)) return rc;
-        TcGemmParams T = tc_base();
-        const int kb = (N + 63) / 64;
-        T.nseg = 1; T.seg[0] = TcSeg{W.pk_a[cur], kb, net.d_tcw + net.tcw_bwd_off[l], kb, kb};
-        T.D = W.dbuf[cur ^ 1]; T.ldd = L.k_act; T.M = P; T.N = L.k_act; T.epi = e;
-        if (Lp.relu) { T.bits_in = W.bits[l - 1]; T.bits_ld = Lp.n_out / 16; }
-        if (l - 1 > 0) { T.pack_out = W.pk_a[cur ^ 1]; T.pack_kbt = L.k_act / 64; T.pack_fp16 = 0; dz_packed = true; }
-        T.colsum = g->bias + Lp.bias_off;
-        bias_done = true;
-        T.packT_out = W.pkt_a; T.packT_kbt = kbtP; dz_colpacked = true;
-        T.skip_d = 1;      // dZ is consumed only through its two packs and the column sums
-        if (int rc = launch_tc_gemm(T, num_sms, st, launches)) return rc;
-      } else {
-        // W[n][k] = Wt[k][n]  ->  B = Wt rows 0..k_act-1 viewed (k_act, N), read transposed
-        if (int rc = sgemm<true>(dZ, N, net.d_wt + L.wt_off, N, W.dbuf[cur ^ 1], L.k_act, P, L.k_act, N, e, st, launches)) return rc;
-        bias_done = false;
-      }
+      if (Lp.relu) { e.mask = W.act[l - 1]; e.ldmask = Lp.n_out; }
+      // W[n][k] = Wt[k][n]  ->  B = Wt rows 0..k_act-1 viewed (k_act, N), read transposed
+      if (int rc = sgemm<true>(dZ, N, net.d_wt + L.wt_off, N, W.dbuf[cur ^ 1], L.k_act, P, L.k_act, N, e, st, launches)) return rc;
+      bias_done = false;
       cur ^= 1;
     }
   }
   return 0;
 }
 
-// standalone entry for tests of the tensor-core GEMM: D (M,N) = A (M,K) B (N,K)^T from fp32 row-major device
-// arrays.  a_cols / b_cols != 0: the operand is given transposed ((K,M) / (K,N) row-major) and packed with
-// pack_cols (1: K-major tiles, 2: MN-major tiles consumed through MN-major descriptors).  k_split > 0 (multiple of 64, row-packed operands only): the K range is fed as two segments.
-int debug_tc_gemm(const float* A, const float* B, int M, int N, int K, int a_cols, int b_cols, int k_split, int n_passes,
-                  int fp16, int atomic, float* D, uint8_t* scratch, size_t scratch_bytes, int num_sms, int* d_err, cudaStream_t st,
-                  int64_t* launches) {
-  const size_t need = up(pack_bytes(M, K)) + up(pack_bytes(N, K)) + (k_split > 0 ? up(pack_bytes(M, K)) : 0);
-  NM_CHECK(scratch_bytes >= need, "scratch too small: need %zu bytes", need);
-  uint8_t* pa = scratch;
-  uint8_t* pb = pa + up(pack_bytes(M, K));
-  uint8_t* pa2 = pb + up(pack_bytes(N, K));
-  TcGemmParams T{};
-  T.n_passes = n_passes; T.fp16 = fp16; T.err = d_err; T.atomic = atomic; T.D = D; T.ldd = N; T.M = M; T.N = N;
-  const int kbt = (K + 63) / 64;
-  if (int e = b_cols ? launch_pack_cols(B, N, K, N, pb, 0, fp16, st, launches, b_cols == 2) : launch_pack_rows(B, K, N, K, pb, fp16, st, launches)) return e;
-  if (k_split > 0) {
-    NM_CHECK(!a_cols && !b_cols && k_split % 64 == 0 && k_split < K && !atomic, "bad k_split");
-    if (int e = launch_pack_rows(A, K, M, k_split, pa, fp16, st, launches)) return e;
-    if (int e = launch_pack_rows(A + k_split, K, M, K - k_split, pa2, fp16, st, launches)) return e;
-    const int kb0 = k_split / 64, kb1 = kbt - kb0;
-    T.nseg = 2;
-    T.seg[0] = TcSeg{pa, kb0, pb, kbt, kb0};
-    T.seg[1] = TcSeg{pa2, kb1, pb + (size_t)kb0 * kPtileBytes, kbt, kb1};
-  } else {
-    if (int e = a_cols ? launch_pack_cols(A, M, K, M, pa, 0, fp16, st, launches, a_cols == 2) : launch_pack_rows(A, K, M, K, pa, fp16, st, launches)) return e;
-    T.nseg = 1;
-    T.seg[0] = TcSeg{pa, kbt, pb, kbt, kbt, (a_cols == 2 ? 1 : 0) | (b_cols == 2 ? 2 : 0)};
-  }
-  int repeat = 1;
-  if (const char* e = getenv("NM_GEMM_REPEAT")) repeat = atoi(e) > 0 ? atoi(e) : 1;     // timing aid (tools/gemm_bench.py)
-  for (int i = 0; i < repeat; ++i)
-    if (int e = launch_tc_gemm(T, num_sms, st, launches)) return e;
-  return 0;
+}  // namespace
+
+// Backward of one network over P = in.M points.  dout (P,4).  ws: train_ws_bytes(full, P, use_tc) bytes, 1 KB aligned.
+// Weight gradients accumulate in the reference's (out,in) layout at the offsets of NetDev.d_w.
+int mlp_backward(NetDev& net, const MlpInput& in, const float* dout, float* ws_base, NetGrads* g, int num_sms,
+                 const TrainMode& mode, cudaStream_t st, int64_t* launches, int have_acts) {
+  if (in.M <= 0) return 0;
+  if (mode.use_tc) return backward_tc(net, in, dout, ws_base, g, num_sms, mode, st, launches, have_acts);
+  return backward_fp32(net, in, dout, ws_base, g, num_sms, st, launches);
 }
 
 }  // namespace nm

@@ -303,15 +303,14 @@ class Engine:
         L.check(self.lib.nm_tree_integrate(self._h, _ptr(idx), _ptr(w), _ptr(mw), idx.numel(), _ptr(memm), memm.numel(),
                                            int(counter), self._stream()))
 
-    def debug_gemm(self, a, b, *, a_cols=False, b_cols=False, k_split=0, n_passes=3, fp16=False, atomic=False, out=None):
-        """Test hook (nm_debug_gemm): D = A B^T on the backward pass's tensor-core GEMM.  a: (M,K) or (K,M) if a_cols;
-        b: (N,K) or (K,N) if b_cols."""
+    def debug_gemm(self, a, b, *, n_passes=3, out=None):
+        """Test hook (nm_debug_gemm): D += a^T b on the backward pass's weight-gradient GEMM.  a: (K,M), b: (K,N);
+        D: `out` (M,N), or a new zero tensor."""
         a, b = _f32c(a, self.device), _f32c(b, self.device)
-        M, K = (a.shape[1], a.shape[0]) if a_cols else a.shape
-        N = b.shape[1] if b_cols else b.shape[0]
+        (K, M), N = a.shape, b.shape[1]
+        assert b.shape[0] == K, (a.shape, b.shape)
         d = out if out is not None else torch.zeros((M, N), dtype=torch.float32, device=self.device)
-        L.check(self.lib.nm_debug_gemm(self._h, _ptr(a), _ptr(b), M, N, K, int(a_cols), int(b_cols), k_split, n_passes,
-                                       int(fp16), int(atomic), _ptr(d), self._stream()))
+        L.check(self.lib.nm_debug_gemm(self._h, _ptr(a), _ptr(b), M, N, K, n_passes, _ptr(d), self._stream()))
         return d
 
     def render_image(self, pose, H, W, focal, near, far, *, ndc=False, rows=None, training=False, buff=False, seed=0,

@@ -197,10 +197,6 @@ def test_direct_and_subchunk_walks_agree(monkeypatch):
     l_dir, c_dir, f_dir = run()
     monkeypatch.setenv("NM_TRAIN_DIRECT_GB", "0")
     l_sub, c_sub, f_sub = run()
-    monkeypatch.setenv("NM_TRAIN_DZ_MN", "0")            # ... and with the dZ packs as K-major tiles (2-byte stores, K-major row sums)
-    l_k, c_k, f_k = run()
-    compare(c_k, c_dir, rel_max=ATOMIC_NOISE, name="K-major dZ packs coarse")
-    compare(f_k, f_dir, rel_max=ATOMIC_NOISE, name="K-major dZ packs fine")
     assert all(abs(a - b) <= 1e-6 * abs(a) for a, b in zip(l_dir, l_sub))      # the loss is an atomic sum of block partials
     compare(c_sub, c_dir, rel_max=ATOMIC_NOISE, name="walks coarse")
     compare(f_sub, f_dir, rel_max=ATOMIC_NOISE, name="walks fine")
@@ -276,21 +272,15 @@ def test_device_side_weight_load_is_bit_identical():
 
 
 @pytest.mark.parametrize("shape", [
-    dict(M=300, N=256, K=319, k_split=256),          # forward of the skip layer: [activations | encoding]
-    dict(M=1000, N=128, K=64),
-    dict(M=77, N=64, K=283, k_split=256),            # tiny net's direction layer
-    dict(M=5000, N=256, K=128),                      # data gradient shape
-    dict(M=256, N=63, K=5000, cols=True),            # weight gradient (encoding part): K = points, split + atomics
-    dict(M=128, N=256, K=70001, cols=True),
-    dict(M=256, N=63, K=5000, cols=2),               # the same operands as MN-major tiles (MN-major smem descriptors)
-    dict(M=128, N=256, K=70001, cols=2),
+    dict(M=256, N=63, K=5000),                       # weight gradient (encoding part): K = points, split + atomics
+    dict(M=128, N=256, K=70001),
 ])
 def test_tc_gemm_matches_fp64(shape):
-    """The backward's wgmma GEMM (operand split x = hi + lo, 3 MMAs per product) against an fp64 product.  Errors are
-    measured against the random-walk scale s = sqrt((A*A)(B*B)^T): bf16 halves (16 significand bits per operand) must stay
-    within 1e-4*s (expected ~2^-17 per term), fp16 halves (22 bits) within 2e-5*s, and
-    the one-pass variant (bf16's 8 bits) must be at least 30x worse than the three-pass one — i.e. the two correction
-    passes really contribute."""
+    """The backward's weight-gradient GEMM (operand split x = hi + lo, 3 MMAs per product; A as MN-major, B as K-major
+    tiles) against an fp64 product.  Errors are measured against the random-walk scale s = sqrt((A*A)(B*B)^T): bf16
+    halves (16 significand bits per operand) must stay within 1e-4*s (expected ~2^-17 per term), and the one-pass variant
+    (bf16's 8 bits) must be at least 30x worse than the three-pass one — i.e. the two correction passes really
+    contribute."""
     import nerfmeshes_b200 as nm
     eng = nm.Engine(O.NetCfg().__dict__, None, nm.RenderSettings())
     M, N, K = shape["M"], shape["N"], shape["K"]
@@ -299,19 +289,15 @@ def test_tc_gemm_matches_fp64(shape):
     b = torch.randn(N, K, generator=g)
     ref = a.double() @ b.double().T
     scale = ((a.double() ** 2) @ (b.double() ** 2).T).sqrt()
-    cols = int(shape.get("cols", 0))      # 1: point-major source packed as K-major tiles, 2: as MN-major tiles
-    A = a.T.contiguous().cuda() if cols else a.cuda()
-    B = b.T.contiguous().cuda() if cols else b.cuda()
-    kw = dict(a_cols=cols, b_cols=cols, k_split=shape.get("k_split", 0), atomic=bool(cols))
+    A, B = a.T.contiguous().cuda(), b.T.contiguous().cuda()                       # point-major, like dZ and the activations
     worst = {}
-    for name, opts in (("bf16x3", dict(n_passes=3)), ("bf16x1", dict(n_passes=1)), ("fp16x3", dict(n_passes=3, fp16=True))):
-        d = eng.debug_gemm(A, B, **kw, **opts)
+    for name, n_passes in (("bf16x3", 3), ("bf16x1", 1)):
+        d = eng.debug_gemm(A, B, n_passes=n_passes)
         worst[name] = float(((d.cpu().double() - ref).abs() / scale).max())
-    assert worst["bf16x3"] <= 1e-4 and worst["fp16x3"] <= 2e-5 and worst["bf16x1"] >= 30 * worst["bf16x3"], (shape, worst)
-    if cols:                                                                       # atomic: a second call accumulates
-        d1 = eng.debug_gemm(A, B, **kw, n_passes=3)
-        d2 = eng.debug_gemm(A, B, **kw, n_passes=3, out=d1.clone())
-        assert float(((d2.cpu().double() - 2 * ref).abs() / scale).max()) <= 2e-4
+    assert worst["bf16x3"] <= 1e-4 and worst["bf16x1"] >= 30 * worst["bf16x3"], (shape, worst)
+    d1 = eng.debug_gemm(A, B, n_passes=3)                                          # atomic: a second call accumulates
+    d2 = eng.debug_gemm(A, B, n_passes=3, out=d1.clone())
+    assert float(((d2.cpu().double() - 2 * ref).abs() / scale).max()) <= 2e-4
 
 
 def test_backward_tensor_core_vs_cuda_core_yardstick():

@@ -1,6 +1,8 @@
-"""Per-launch time of the backward's wgmma GEMM (nm_gemm_tc.cu) through nm_debug_gemm: the pack kernels run once,
-the GEMM NM_GEMM_REPEAT times; (t(repeat=R) - t(repeat=1)) / (R-1).  NM_GEMM_DBG=1/2/4 knocks out MMAs / loads / stores.
-Run each configuration in its own process (the env knobs are read once)."""
+"""Per-launch time of the backward's weight-gradient GEMM (nm_gemm_tc.cu) through nm_debug_gemm: the pack kernels run
+once, the GEMM NM_GEMM_REPEAT times; (t(repeat=R) - t(repeat=1)) / (R-1).
+
+    python tools/gemm_bench.py M N K REPEAT        (A: (K,M), B: (K,N), K = points)
+"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -11,23 +13,23 @@ ARCH = dict(num_layers=8, hidden_size=256, skip_step=4, num_encoding_fn_xyz=10, 
             include_input_dir=True, log_sampling_xyz=True, log_sampling_dir=True, use_viewdirs=True)
 
 
-def run(M, N, K, cols, rep):
+def run(M, N, K, rep):
     os.environ["NM_GEMM_REPEAT"] = str(rep)
     eng = nm.Engine(ARCH, None, nm.RenderSettings())
-    a = torch.randn((K, M) if cols else (M, K), device="cuda")
-    b = torch.randn((K, N) if cols else (N, K), device="cuda")
+    a = torch.randn((K, M), device="cuda")
+    b = torch.randn((K, N), device="cuda")
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
     out = torch.zeros(M, N, device="cuda")
     ts = []
     for _ in range(3):
         ev[0].record()
-        eng.debug_gemm(a, b, a_cols=cols, b_cols=cols, atomic=cols, out=out)
+        eng.debug_gemm(a, b, out=out)
         ev[1].record(); torch.cuda.synchronize()
         ts.append(ev[0].elapsed_time(ev[1]))
     return min(ts)
 
 
 if __name__ == "__main__":
-    M, N, K, cols, rep = int(sys.argv[1]), int(sys.argv[2]), int(sys.argv[3]), int(sys.argv[4]), int(sys.argv[5])
-    t = run(M, N, K, bool(cols), rep)
-    print(f"M={M} N={N} K={K} cols={cols} repeat={rep} dbg={os.environ.get('NM_GEMM_DBG', '0')}: {t * 1e3:.1f} us total")
+    M, N, K, rep = int(sys.argv[1]), int(sys.argv[2]), int(sys.argv[3]), int(sys.argv[4])
+    t = run(M, N, K, rep)
+    print(f"M={M} N={N} K={K} repeat={rep}: {t * 1e3:.1f} us total")
