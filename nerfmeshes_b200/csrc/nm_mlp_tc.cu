@@ -83,8 +83,22 @@ struct TcParams {
 };
 static_assert(sizeof(TcParams) <= 4096, "TcParams must fit the 4 KB kernel-parameter window");
 
-// barrier slots (8 B each) relative to off_bars
-constexpr uint32_t kBarWFull = 0, kBarWEmpty = 64, kBarBytes = 128;
+// NM_MLP_STALLS=1 (diagnostic build: NM_NVCC_EXTRA=-DNM_MLP_STALLS=1): thread 0 of each consumer warpgroup splits its
+// clock64() time into weight-ring full waits, the MMA main loop (its waits excluded) and the rest (encodings, epilogues,
+// compositor), and the first two and the last CTA of a launch printf the totals at exit.  The counters live in shared
+// memory after the barriers to keep register pressure down; the instrumented kernel still spills more than the shipped
+// one, so its split is approximate.
+#ifndef NM_MLP_STALLS
+#define NM_MLP_STALLS 0
+#endif
+#if NM_MLP_STALLS
+#define NM_ST(...) __VA_ARGS__
+#else
+#define NM_ST(...)
+#endif
+
+// barrier slots (8 B each) relative to off_bars (+ the NM_MLP_STALLS counters: wait, mma, start per warpgroup)
+constexpr uint32_t kBarWFull = 0, kBarWEmpty = 64, kBarStalls = 128, kBarBytes = 128 + (NM_MLP_STALLS ? 64 : 0);
 
 enum : int { ERR_ALIGN = 1, ERR_W_EMPTY = 2, ERR_W_FULL = 3 };
 
@@ -195,6 +209,8 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
   int slot = 0;
   uint32_t ph = 0;
   float acc[4][32];
+  NM_ST(volatile long long* const st = reinterpret_cast<volatile long long*>(smem + P.off_bars + kBarStalls) + 4 * wg;
+        if (t == 0) { st[0] = 0; st[1] = 0; st[2] = clock64(); })
 
   // encoding of this tile's points (xyz or view direction) -> the encoding buffer, columns past the width zeroed
   auto encode = [&](long long tile, bool dir) {
@@ -339,7 +355,9 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
       // hand it straight back
       for (int b = 0; b < n_blocks; ++b) {
         if (t == 0) {
+          NM_ST(const long long c0 = clock64();)
           ptx::mbar_wait(bars + kBarWFull + 8 * slot, ph, P.err, ERR_W_FULL);
+          NM_ST(st[0] += clock64() - c0;)
           ptx::mbar_arrive(bars + kBarWEmpty + 8 * slot);
         }
         if (++slot == NS) { slot = 0; ph ^= 1; }
@@ -359,10 +377,13 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
 #pragma unroll
           for (int i = 0; i < 32; ++i) acc[c][i] = 0.f;
         ptx::wgmma_fence();
+        NM_ST(if (t == 0) st[1] -= clock64() - st[0];)      // + (loop end - loop start) - (waits inside the loop)
         int prev = -1;
         for (int b = L.blk_begin; b < L.blk_end; ++b) {
           const BlockProg& B = P.net.blocks[b];
-          ptx::mbar_wait(bars + kBarWFull + 8 * slot, ph, P.err, ERR_W_FULL);
+          NM_ST(const long long c0 = clock64();)
+          ptx::mbar_wait_warp(bars + kBarWFull + 8 * slot, ph, P.err, ERR_W_FULL);
+          NM_ST(if (t == 0) st[0] += clock64() - c0;)
           const uint32_t wst = sbase + (uint32_t)slot * kStageBytes;
           const uint64_t b_hi = ptx::make_kmajor_sw128_desc(wst), b_lo = ptx::make_kmajor_sw128_desc(wst + (uint32_t)kHalfStage);
           const uint32_t a_t = (B.src == SRC_ACT) ? act_s + (uint32_t)B.kb * kKBlock : pe_s;
@@ -382,6 +403,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
         }
         ptx::wgmma_wait<0>();
         if (prev >= 0 && t == 0) ptx::mbar_arrive(bars + kBarWEmpty + 8 * prev);
+        NM_ST(if (t == 0) st[1] += clock64() - st[0];)
 #pragma unroll
         for (int c = 0; c < 4; ++c) ptx::fence_regs<32>(acc[c]);
       }
@@ -555,6 +577,9 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
     }
     if (MODE == 0 && P.comp_on) composite_tile(it, tile);
   }
+  NM_ST(if (t == 0 && (blockIdx.x < 2 || blockIdx.x + 1 == gridDim.x))
+          printf("mlp_stalls mode %d cta %d wg %d wait %lld mma %lld other %lld\n", MODE, (int)blockIdx.x, wg, st[0], st[1],
+                 clock64() - st[2] - st[0] - st[1]);)
 }
 
 }  // namespace

@@ -64,6 +64,21 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int* er
   }
 }
 
+// The same for a whole warp that waits together, with warp-uniform control flow (votes).  A wgmma issued after a wait
+// whose loop branches per thread sits in a divergent path, and ptxas then serialises every wgmma of the kernel (C7520: a
+// wait for completion after each one).
+__device__ __forceinline__ void mbar_wait_warp(uint32_t bar, uint32_t parity, int* err, int code) {
+  if (__all_sync(0xffffffffu, mbar_try_wait(bar, parity))) return;
+  const long long t0 = clock64();
+  while (!__all_sync(0xffffffffu, mbar_try_wait_hint(bar, parity, NM_WAIT_HINT_NS))) {
+    if (__any_sync(0xffffffffu, clock64() - t0 > 4000000000LL)) {  // ~2 s
+      if (err) atomicExch(err, code);
+      __threadfence_system();
+      __trap();
+    }
+  }
+}
+
 // ---- async-proxy fences / bulk copy ---------------------------------------------------------------------------
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uint32_t bytes, uint32_t bar) {
