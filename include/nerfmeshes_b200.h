@@ -242,6 +242,14 @@ int nm_tree_integrate(NmHandle h, const int32_t* idx_dev, const float* weights_d
 int nm_debug_gemm(NmHandle h, const float* a_dev, const float* b_dev, int M, int N, int K, int n_passes, float* d_dev,
                   void* stream);
 
+/* Test hook for the network backward alone (no compositor): runs it on M points built like nm_point_mlp's, with
+ * dout_dev (M,4) = [d rgb logits (before the sigmoid), d raw sigma] per point, and ACCUMULATES dL/dtheta of network
+ * `which` into the handle's gradient buffers (nm_zero_grad clears them, nm_get_grad reads them).  The handle's precision
+ * selects the path: tensor cores (training forward that emits the backward's operands, heads, data-gradient chain,
+ * weight-gradient GEMMs) or NM_PREC_FP32.  dout_dev must be 16-byte aligned. */
+int nm_debug_mlp_backward(NmHandle h, int which, const float* pts_dev, const float* dirs_dev, int64_t M, const float* dout_dev,
+                          void* stream);
+
 /* ---- host-only debugging aid (no CUDA): the layer program + tensor-core weight stream nm_load_weights would
  * upload, for CPU tests of the schedule / swizzle logic.  program_out receives the internal NetProgram struct
  * (nerfmeshes_b200/csrc/nm_program.h). */

@@ -659,6 +659,27 @@ int nm_debug_gemm(NmHandle h, const float* a_dev, const float* b_dev, int M, int
                        &h->launches);
 }
 
+int nm_debug_mlp_backward(NmHandle h, int which, const float* pts_dev, const float* dirs_dev, int64_t M, const float* dout_dev,
+                          void* stream) {
+  if (int e = bind_checked(h)) return e;
+  NM_CHECK(which == NM_NET_COARSE || (which == NM_NET_FINE && h->has_fine), "network slot %d not present", which);
+  NM_CHECK(pts_dev && dout_dev && M > 0 && M <= INT32_MAX, "bad arguments");
+  NM_CHECK((reinterpret_cast<uintptr_t>(dout_dev) & 15) == 0, "dout must be 16-byte aligned (M,4) rows");
+  NetDev& net = h->nets[which];
+  NM_CHECK(net.loaded, "weights of network %d not loaded", which);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (!h->grads_ready) if (int e = ensure_grads(h, st, true)) return e;
+  if (int e = ensure_grads(h, st, false)) return e;
+  const bool use_tc = h->cfg.precision != NM_PREC_FP32;
+  if (int e = h->train_ws.ensure(train_ws_bytes(net.full, M, use_tc) + 1024)) return e;
+  float* ws = reinterpret_cast<float*>(((uintptr_t)h->train_ws.p + 1023) & ~(uintptr_t)1023);
+  MlpInput in{};
+  in.mode = IN_POINTS; in.pts = pts_dev; in.dirs = dirs_dev; in.M = M;
+  NetGrads g{h->g_wt[which].as<float>(), h->g_bias[which].as<float>(), h->g_head[which].as<float>()};
+  TrainMode mode{use_tc ? 1 : 0, h->cfg.precision == NM_PREC_FAST ? 1 : 3, h->d_err};
+  return mlp_backward(net, in, dout_dev, ws, &g, h->num_sms, mode, st, &h->launches, 0);
+}
+
 // ---------------------------------------------------------------------------------------------- BuFF tree maintenance
 int nm_ray_voxel_indices(NmHandle h, const float* origins_dev, int o_stride, const float* dirs_dev, int64_t R,
                          const float* near_far_host, float* z_out_dev, int32_t* idx_out_dev, void* stream) {

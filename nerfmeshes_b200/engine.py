@@ -313,6 +313,16 @@ class Engine:
         L.check(self.lib.nm_debug_gemm(self._h, _ptr(a), _ptr(b), M, N, K, n_passes, _ptr(d), self._stream()))
         return d
 
+    def debug_mlp_backward(self, which: int, pts, dirs, dout):
+        """Test hook (nm_debug_mlp_backward): accumulate the gradients of network `which` for per-point adjoints
+        dout (M,4) = [d rgb logits, d raw sigma] at points pts (M,3) with view directions dirs (M,3) or None."""
+        p = _f32c(pts, self.device).reshape(-1, 3)
+        d = None if dirs is None else _f32c(dirs, self.device).reshape(-1, 3)
+        g = _f32c(dout, self.device)
+        M = p.shape[0]
+        assert g.shape == (M, 4) and (d is None or d.shape == (M, 3)), (p.shape, g.shape)
+        L.check(self.lib.nm_debug_mlp_backward(self._h, which, _ptr(p), _ptr(d), M, _ptr(g), self._stream()))
+
     def render_image(self, pose, H, W, focal, near, far, *, ndc=False, rows=None, training=False, buff=False, seed=0,
                      want=None, to_host=False, host_out=None, out=None) -> Dict[str, torch.Tensor]:
         """Rays generated on the device from a 3x4 / 4x4 camera-to-world pose (get_ray_bundle [+ ndc_rays])."""
