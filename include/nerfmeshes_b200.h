@@ -177,6 +177,21 @@ int nm_mc_count(NmHandle h, const float* vol_dev, int nb, int ny, int nz, float 
                 int64_t* counts_host, void* stream);
 int nm_mc_emit(NmHandle h, const float* vol_dev, int nb, int ny, int nz, float iso, int g_x0, int g_nx, int p_lo, int p_hi,
                int64_t v_base, float* verts_dev, float* normals_dev, int32_t* faces_dev, void* stream);
+/* Super-sampled emit step (the --super-sampling branch of mesh_nerf.py:95-128): called after nm_mc_count with the same
+ * shard arguments, like nm_mc_emit, whose faces, normals and centre vertices it reproduces bit for bit.  Each vertex on the
+ * axis-a edge from global grid point (I,J,K) to its neighbour along a is re-placed from s >= 0 extra samples along that
+ * edge: v_0 = vol(point), v_{s+1} = vol(neighbour), and for m = 1..s v_m = sigma of the finest network (the one
+ * nm_grid_sigma sweeps, at the handle's precision, directions = positions) at fine_a[idx_a*(s+1)+m] along a and
+ * lin_b[idx_b] along the other axes.  With the smallest m in [0,s] where (v_m > iso) != (v_{m+1} > iso), in double:
+ *   w0 = 1/(FLT_EPSILON + |v_m - iso|),  w1 = 1/(FLT_EPSILON + |v_{m+1} - iso|),  pos[a] = base[a] + (m + w1/(w0+w1))/(s+1);
+ * s = 0 is nm_mc_emit's formula.  lin0 / fine0 cover the GLOBAL grid (g_nx and (g_nx-1)(s+1)+1 entries), lin1 / lin2 have
+ * ny / nz entries, fine1 / fine2 (ny-1)(s+1)+1 / (nz-1)(s+1)+1: torch.linspace(-limit, limit, n) and
+ * torch.linspace(-limit, limit, n + (n-1)*s).  Host tables.  0 <= s <= 64.  The network sees s points per owned vertex
+ * (centre vertices are padded with their grid point), in launches of at most NM_SS_CHUNK_POINTS points (default 4 Mi). */
+int nm_mc_emit_ss(NmHandle h, const float* vol_dev, int nb, int ny, int nz, float iso, int g_x0, int g_nx, int p_lo, int p_hi,
+                  int64_t v_base, int s, const float* lin0_host, const float* lin1_host, const float* lin2_host,
+                  const float* fine0_host, const float* fine1_host, const float* fine2_host,
+                  float* verts_dev, float* normals_dev, int32_t* faces_dev, void* stream);
 
 /* Replaces export_obj (src/nerf/nerf_helpers.py:86-111): `v x y z [r g b]`, `vn x y z`, `f i//i j//j k//k` (1-based) with
  * byte-identical number formatting (python repr of the float32 widened to double).  Host arrays, no GPU involved;

@@ -63,12 +63,21 @@ struct NmHandle_t {
   size_t mc_ws2_bytes = 0;
   void* mc_ws2_ptr = nullptr;
   int64_t mc_counts[2] = {0, 0};   // {vertices, triangles} of the last count step: sizes of the emit step
+  Buf ss_tab, ss_ws;               // super-sampled emit: the six coordinate tables; chunk points (M,3) + sigma (M,)
   // training (nm_train.cu): gradient accumulators per network + scratch
   Buf g_wt[2], g_bias[2], g_head[2], train_ws, dout, trans, tr_rgb[2], tr_drgb[2];
   bool grads_ready = false;
 };
 
 namespace {
+
+// points per network launch of the super-sampled mesh emit (16 B of workspace each: 64 MB at 4 Mi); NM_SS_CHUNK_POINTS
+// overrides it, read per call (the tests cross chunk boundaries with small values)
+long long ss_chunk_points() {
+  const char* e = getenv("NM_SS_CHUNK_POINTS");
+  const long long x = e ? atoll(e) : 0;
+  return x > 0 ? x : (1ll << 22);
+}
 
 // rays per internal chunk (bounds the per-sample workspace: 20 B x 192 samples x 1 Mi rays = 4 GB); NM_CHUNK_RAYS overrides (tests)
 long long chunk_rays() {
@@ -473,6 +482,7 @@ int nm_destroy(NmHandle h) {
   for (Buf& b : h->stage_out) b.release();
   for (int i = 0; i < 2; ++i) { h->g_wt[i].release(); h->g_bias[i].release(); h->g_head[i].release(); h->tr_rgb[i].release(); h->tr_drgb[i].release(); }
   h->train_ws.release(); h->dout.release(); h->trans.release();
+  h->ss_tab.release(); h->ss_ws.release();
   if (h->mc_ws_ptr) cudaFree(h->mc_ws_ptr);
   if (h->mc_ws2_ptr) cudaFree(h->mc_ws2_ptr);
   if (h->h_err) cudaFreeHost(h->h_err);
@@ -777,6 +787,55 @@ int nm_mc_emit(NmHandle h, const float* vol_dev, int nb, int ny, int nz, float i
   const McShard s{vol_dev, nb, ny, nz, iso, g_x0, g_nx, p_lo, p_hi, 0};
   return mc_emit(s, h->mc_ws_ptr, h->mc_ws_bytes, &h->mc_ws2_ptr, &h->mc_ws2_bytes, v_base, h->mc_counts[0], h->mc_counts[1],
                  verts_dev, normals_dev, faces_dev, (cudaStream_t)stream, &h->launches);
+}
+
+int nm_mc_emit_ss(NmHandle h, const float* vol_dev, int nb, int ny, int nz, float iso, int g_x0, int g_nx, int p_lo, int p_hi,
+                  int64_t v_base, int s, const float* lin0_host, const float* lin1_host, const float* lin2_host,
+                  const float* fine0_host, const float* fine1_host, const float* fine2_host, float* verts_dev, float* normals_dev,
+                  int32_t* faces_dev, void* stream) {
+  if (int e = bind_checked(h)) return e;
+  NM_CHECK(s >= 0 && s <= kMcMaxSuperSampling, "super-sampling factor %d outside [0, %d]", s, kMcMaxSuperSampling);
+  NM_CHECK(lin0_host && lin1_host && lin2_host && fine0_host && fine1_host && fine2_host, "null coordinate table");
+  NM_CHECK(vol_dev && verts_dev && faces_dev && h->mc_ws_ptr, "bad arguments (call nm_mc_count first)");
+  NM_CHECK(ny >= 2 && nz >= 2 && g_nx >= 2, "marching cubes: bad volume shape");
+  const int64_t nv = h->mc_counts[0], nt = h->mc_counts[1];
+  const McShard sh{vol_dev, nb, ny, nz, iso, g_x0, g_nx, p_lo, p_hi, 0};
+  cudaStream_t st = (cudaStream_t)stream;
+  McSuperSampling ss;
+  ss.s = s;
+  if (nv > 0) {
+    // the six tables in one buffer: lin0 | lin1 | lin2 | fine0 | fine1 | fine2
+    const long long n[3] = {g_nx, ny, nz};
+    const float* hs[6] = {lin0_host, lin1_host, lin2_host, fine0_host, fine1_host, fine2_host};
+    long long len[6], off[6], tot = 0;
+    for (int a = 0; a < 6; ++a) {
+      len[a] = a < 3 ? n[a] : (n[a - 3] - 1) * (s + 1) + 1;
+      off[a] = tot;
+      tot += len[a];
+    }
+    if (int e = h->ss_tab.ensure((size_t)tot * 4)) return e;
+    for (int a = 0; a < 6; ++a)
+      NM_CUDA(cudaMemcpyAsync(h->ss_tab.as<float>() + off[a], hs[a], (size_t)len[a] * 4, cudaMemcpyHostToDevice, st));
+    NM_CUDA(cudaStreamSynchronize(st));      // pageable sources: the copies must finish before the host arrays may change
+    for (int a = 0; a < 3; ++a) { ss.lin[a] = h->ss_tab.as<float>() + off[a]; ss.fine[a] = h->ss_tab.as<float>() + off[a + 3]; }
+    if (s > 0) {
+      ss.chunk_points = ss_chunk_points();
+      ss.chunk_vertices = ss.chunk_points >= s ? ss.chunk_points / s : 1;
+      if (ss.chunk_vertices > nv) ss.chunk_vertices = nv;
+      const long long m = ss.chunk_vertices * s;
+      if (int e = h->ss_ws.ensure((size_t)m * 16 + 256)) return e;
+      ss.pts = h->ss_ws.as<float>();
+      ss.sig = reinterpret_cast<float*>(reinterpret_cast<char*>(h->ss_ws.p) + ((size_t)m * 12 + 255) / 256 * 256);
+      const int which = h->has_fine ? NM_NET_FINE : NM_NET_COARSE;     // the net nm_grid_sigma sweeps
+      ss.eval = [h, which, st](const float* pts, long long M, float* sigma) -> int {
+        MlpInput in{};
+        in.mode = IN_POINTS; in.pts = pts; in.dirs = nullptr; in.M = M;   // directions = positions, as in the grid sweep
+        return run_mlp(h, which, true, in, sigma, st);
+      };
+    }
+  }
+  return mc_emit_ss(sh, h->mc_ws_ptr, h->mc_ws_bytes, &h->mc_ws2_ptr, &h->mc_ws2_bytes, v_base, nv, nt, ss, verts_dev,
+                    normals_dev, faces_dev, st, &h->launches);
 }
 
 int nm_marching_cubes_count(NmHandle h, const float* vol_dev, int nx, int ny, int nz, float iso, int64_t* counts_host,

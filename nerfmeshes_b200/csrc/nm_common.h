@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <functional>
 #include <string>
 #include <vector>
 
@@ -195,5 +196,21 @@ struct McShard {
 int mc_count(const McShard& s, void** ws, size_t* ws_bytes, int64_t* counts_host, cudaStream_t st, int64_t* launches);
 int mc_emit(const McShard& s, void* ws, size_t ws_bytes, void** ws2, size_t* ws2_bytes, long long v_base, int64_t nv, int64_t nt,
             float* verts, float* normals, int32_t* faces, cudaStream_t st, int64_t* launches);
+// super-sampled emit (nm_mc_emit_ss): mc_emit, then every edge vertex is re-placed from s network samples along its edge.
+// The vertices are walked in chunks of chunk_vertices; each chunk's chunk_vertices*s points go to `pts` (M,3), are
+// evaluated by `eval` (sigma only, at most chunk_points per call) into `sig` (M,), and the chunk's vertices are refined.
+constexpr int kMcMaxSuperSampling = 64;
+struct McSuperSampling {
+  int s = 0;
+  const float* lin[3] = {nullptr, nullptr, nullptr};    // device: the coarse tables, g_nx / ny / nz entries
+  const float* fine[3] = {nullptr, nullptr, nullptr};   // device: the fine tables, (n-1)(s+1)+1 entries
+  float* pts = nullptr;
+  float* sig = nullptr;
+  long long chunk_vertices = 0, chunk_points = 0;
+  std::function<int(const float* pts, long long M, float* sigma)> eval;
+};
+int mc_emit_ss(const McShard& s, void* ws, size_t ws_bytes, void** ws2, size_t* ws2_bytes, long long v_base, int64_t nv,
+               int64_t nt, const McSuperSampling& ss, float* verts, float* normals, int32_t* faces, cudaStream_t st,
+               int64_t* launches);
 
 }  // namespace nm

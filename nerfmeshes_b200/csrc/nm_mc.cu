@@ -13,6 +13,8 @@
 //   5. mc_emit_vertices / mc_emit_triangles   one thread per OUTPUT vertex / triangle (perfectly balanced, coalesced
 //                        stores); a vertex id anywhere in the grid is prefix[word] + popcount(bits below) — no dense
 //                        per-point id array.
+//   6. mc_ss_points_kernel / mc_ss_refine_kernel   super-sampled emit (nm_mc_emit_ss, DESIGN.md 4.3): after 5., s network
+//                        points per vertex, the fused MLP sigma-only on them, then each edge vertex re-placed along its edge.
 //
 // Output contract (mirrors the Lewiner output the reference consumes at mesh_nerf.py:79-90): an INDEXED mesh, one vertex
 // per crossed grid edge plus Lewiner's cell-centre vertices, vertices (V,3) fp32 in index coordinates (axis0, axis1, axis2),
@@ -479,6 +481,68 @@ __global__ void __launch_bounds__(kBlock) mc_emit_triangles(const McGrid g, unsi
   faces[3 * (size_t)tid] = out[0]; faces[3 * (size_t)tid + 1] = out[1]; faces[3 * (size_t)tid + 2] = out[2];
 }
 
+// ------------------------------------------------------------------------------------------------ 6. super-sampling
+// (nm_mc_emit_ss, DESIGN 4.3)  The vertex on the axis-a edge from global grid point (I,J,K) to its neighbour has the
+// samples v_0 = vol(point), v_{s+1} = vol(neighbour) and, for m = 1..s, v_m = sigma at (fine_a[idx_a*(s+1)+m] along a,
+// lin_b[idx_b] along the other axes).  Vertices [v0, v0+n) of the chunk give n*s points, s per vertex; centre vertices
+// are padded with s copies of their grid point (kept flat: point q belongs to vertex v0 + q/s), their sigma is unused.
+struct SsTables {
+  const float* lin[3];
+  const float* fine[3];
+  int s;
+};
+
+__global__ void __launch_bounds__(kBlock) mc_ss_points_kernel(const McGrid g, const SsTables t, unsigned v0, unsigned n,
+                                                              float* __restrict__ pts) {
+  const unsigned long long q = (unsigned long long)blockIdx.x * kBlock + threadIdx.x;
+  if (q >= (unsigned long long)n * t.s) return;
+  const unsigned vq = (unsigned)(q / (unsigned)t.s);
+  const int m = (int)(q - (unsigned long long)vq * t.s) + 1;
+  const unsigned long long rec = g.vmap[v0 + vq];
+  const long long wl = (long long)(rec >> 7);
+  const int b = (int)((rec >> 2) & 31u), slot = (int)(rec & 3u);
+  int i, j, w;
+  word_coords(g, wl, &i, &j, &w);
+  const int idx[3] = {g.g_x0 + i, j, w * 32 + b};
+  float p[3] = {t.lin[0][idx[0]], t.lin[1][idx[1]], t.lin[2][idx[2]]};
+  if (slot < 3) p[slot] = t.fine[slot][(size_t)idx[slot] * (t.s + 1) + m];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) pts[3 * q + c] = p[c];
+}
+
+// refined position of the chunk's edge vertices: the first sub-interval [m, m+1] whose samples straddle iso, placed with
+// the same weights as mc_emit_vertices; only coordinate a of the vertex is rewritten (normals, centre vertices untouched)
+__global__ void __launch_bounds__(kBlock) mc_ss_refine_kernel(const McGrid g, int s, unsigned v0, unsigned n,
+                                                              const float* __restrict__ sig, float* __restrict__ verts) {
+  const unsigned q = blockIdx.x * kBlock + threadIdx.x;
+  if (q >= n) return;
+  const unsigned id = v0 + q;
+  const unsigned long long rec = g.vmap[id];
+  const int slot = (int)(rec & 3u);
+  if (slot == 3) return;
+  const long long wl = (long long)(rec >> 7);
+  const int b = (int)((rec >> 2) & 31u), a = slot;
+  int i, j, w;
+  word_coords(g, wl, &i, &j, &w);
+  const int k = w * 32 + b;
+  const size_t p = ((size_t)i * g.ny + j) * g.nz + k;
+  const size_t st = a == 0 ? (size_t)g.ny * g.nz : (a == 1 ? (size_t)g.nz : 1);
+  const float* vs = sig + (size_t)q * s;
+  float va = g.vol[p], vb = va;
+  const bool in0 = va > g.iso;
+  int m = 0;
+  for (; m <= s; ++m) {                          // v_{s+1} differs from v_0 in sign: the loop always breaks
+    vb = m < s ? vs[m] : g.vol[p + st];
+    if ((vb > g.iso) != in0) break;
+    va = vb;
+  }
+  const double iso = (double)g.iso;
+  const double w0 = 1.0 / (kEps + fabs((double)va - iso));
+  const double w1 = 1.0 / (kEps + fabs((double)vb - iso));
+  const double base = a == 0 ? (double)(g.g_x0 + i + g.x_shift) : (double)(a == 1 ? j : k);
+  verts[3 * (size_t)id + a] = (float)(base + ((double)m + w1 / (w0 + w1)) / (double)(s + 1));
+}
+
 size_t align_up(size_t x) { return (x + 255) / 256 * 256; }
 
 int carve(void* base, size_t bytes, McGrid* g, size_t* need) {
@@ -589,6 +653,43 @@ int mc_emit(const McShard& s, void* ws_ptr, size_t ws_bytes, void** ws2_ptr, siz
     NM_CUDA(cudaGetLastError());
   }
   if (launches) *launches += 3;
+  return 0;
+}
+
+int mc_emit_ss(const McShard& s, void* ws_ptr, size_t ws_bytes, void** ws2_ptr, size_t* ws2_bytes, long long v_base, int64_t nv,
+               int64_t nt, const McSuperSampling& ss, float* verts, float* normals, int32_t* faces, cudaStream_t st,
+               int64_t* launches) {
+  NM_CHECK(ss.s >= 0 && ss.s <= kMcMaxSuperSampling, "super-sampling factor %d outside [0, %d]", ss.s, kMcMaxSuperSampling);
+  // the s = 0 mesh (vertices, normals, faces, and the vertex records in the second workspace) ...
+  if (int e = mc_emit(s, ws_ptr, ws_bytes, ws2_ptr, ws2_bytes, v_base, nv, nt, verts, normals, faces, st, launches)) return e;
+  if (nv == 0) return 0;
+  NM_CHECK(ss.lin[0] && ss.lin[1] && ss.lin[2] && ss.fine[0] && ss.fine[1] && ss.fine[2], "super-sampling tables missing");
+  NM_CHECK(ss.s == 0 || (ss.pts && ss.sig && ss.chunk_vertices > 0 && ss.chunk_points > 0 && ss.eval),
+           "super-sampling workspace missing");
+  // ... then the edge vertices are moved, chunk by chunk
+  McGrid g{};
+  if (int e = make_grid(s, &g)) return e;
+  g.vmap = reinterpret_cast<unsigned long long*>(*ws2_ptr);
+  SsTables t{};
+  for (int a = 0; a < 3; ++a) { t.lin[a] = ss.lin[a]; t.fine[a] = ss.fine[a]; }
+  t.s = ss.s;
+  const long long per = ss.s ? ss.chunk_vertices : nv;
+  for (long long v0 = 0; v0 < nv; v0 += per) {
+    const long long n = nv - v0 < per ? nv - v0 : per;
+    if (ss.s) {
+      const long long npts = n * ss.s;
+      mc_ss_points_kernel<<<(unsigned)((npts + kBlock - 1) / kBlock), kBlock, 0, st>>>(g, t, (unsigned)v0, (unsigned)n, ss.pts);
+      NM_CUDA(cudaGetLastError());
+      if (launches) *launches += 1;
+      for (long long q0 = 0; q0 < npts; q0 += ss.chunk_points) {
+        const long long m = npts - q0 < ss.chunk_points ? npts - q0 : ss.chunk_points;
+        if (int e = ss.eval(ss.pts + 3 * q0, m, ss.sig + q0)) return e;
+      }
+    }
+    mc_ss_refine_kernel<<<(unsigned)((n + kBlock - 1) / kBlock), kBlock, 0, st>>>(g, ss.s, (unsigned)v0, (unsigned)n, ss.sig, verts);
+    NM_CUDA(cudaGetLastError());
+    if (launches) *launches += 1;
+  }
   return 0;
 }
 

@@ -447,6 +447,30 @@ class Engine:
                                         int(v_base), _ptr(verts), _ptr(normals), _ptr(faces), self._stream()))
         return verts, faces, normals
 
+    def mc_emit_ss(self, vol, iso, g_x0, g_nx, p_lo, p_hi, nv, nt, v_base, s, lins, fines, out=None):
+        """Super-sampled emit step (nm_mc_emit_ss): mc_emit's arrays, with every edge vertex re-placed from `s` network
+        samples along its edge.  lins: the coarse tables (g_nx, ny, nz entries), fines: the fine tables
+        ((n-1)(s+1)+1 entries; mesh.super_sampling_tables)."""
+        nb, ny, nz = vol.shape
+        if out is None:
+            verts = torch.empty((nv, 3), dtype=torch.float32, device=self.device)
+            normals = torch.empty((nv, 3), dtype=torch.float32, device=self.device)
+            faces = torch.empty((nt, 3), dtype=torch.int32, device=self.device)
+        else:
+            verts, normals, faces = out
+            assert verts.is_contiguous() and normals.is_contiguous() and faces.is_contiguous() and faces.dtype == torch.int32
+            assert verts.shape[0] >= nv and faces.shape[0] >= nt
+        want = (g_nx, ny, nz)
+        tabs = [np.ascontiguousarray(torch.as_tensor(t).detach().cpu().numpy(), dtype=np.float32) for t in (*lins, *fines)]
+        for a in range(3):                   # the library cannot see the host tables' lengths
+            if 0 <= s and (tabs[a].size != want[a] or tabs[3 + a].size != (want[a] - 1) * (s + 1) + 1):
+                raise L.NmError(f"super-sampling tables of axis {a}: {tabs[a].size} / {tabs[3 + a].size} entries, expected "
+                                f"{want[a]} / {(want[a] - 1) * (s + 1) + 1}")
+        L.check(self.lib.nm_mc_emit_ss(self._h, _ptr(vol), nb, ny, nz, float(iso), int(g_x0), int(g_nx), int(p_lo), int(p_hi),
+                                       int(v_base), int(s), *[t.ctypes.data for t in tabs], _ptr(verts), _ptr(normals),
+                                       _ptr(faces), self._stream()))
+        return verts, faces, normals
+
     # ------------------------------------------------------------------ introspection
     def kernel_flags(self):
         out = (C.c_int32 * 2)()

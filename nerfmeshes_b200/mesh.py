@@ -47,16 +47,42 @@ def marching_cubes(volume, level, engine=None):
     return verts.cpu().numpy(), faces.cpu().numpy(), normals.cpu().numpy(), values.numpy()
 
 
+def super_sampling_tables(limit, nums, s):
+    """Coordinate tables of super-sampled marching cubes (mesh_nerf.py:37,109): (lins, fines), per axis
+    torch.linspace(-limit, limit, n) and torch.linspace(-limit, limit, n + (n-1)*s)."""
+    if isinstance(nums, int):
+        nums = (nums,) * 3
+    lins = [torch.linspace(-limit, limit, n) for n in nums]
+    fines = [torch.linspace(-limit, limit, n + (n - 1) * s) for n in nums]
+    return lins, fines
+
+
 def extract_geometry(model, device, args):
-    """src/mesh_nerf.py:68-92: sigma sweep -> adaptive iso -> marching cubes -> rescale to (-limit, limit)."""
+    """src/mesh_nerf.py:68-92: sigma sweep -> adaptive iso -> marching cubes -> rescale to (-limit, limit).
+    With args.super_sampling = s >= 1 (mesh_nerf.py:95-128) the coarse grid's mesh keeps its topology, faces and normals,
+    and each edge vertex is placed from s extra network samples along its edge (nm_mc_emit_ss, DESIGN 4.3)."""
     eng = model._engine()
     density = extract_radiance(model, args, device, args.res, sigma_only=True)
     iso_value = extract_iso_level(density, args, eng)
-    verts, faces, normals = eng.marching_cubes(density, float(iso_value))
+    s = int(getattr(args, "super_sampling", 0) or 0)
+    if s == 0:
+        verts, faces, normals = eng.marching_cubes(density, float(iso_value))
+    else:
+        n0 = density.shape[0]
+        lins, fines = super_sampling_tables(args.limit, tuple(density.shape), s)
+        nv, nt = eng.mc_count(density, float(iso_value), 0, n0, 0, n0)
+        verts, faces, normals = eng.mc_emit_ss(density, float(iso_value), 0, n0, 0, n0, nv, nt, 0, s, lins, fines)
     # the reference rescales CPU tensors (:82-90); do the same on the host so the rounding is identical (torch's CUDA
     # division by a python scalar multiplies by the reciprocal, which differs in the last bit)
     vertices = args.limit * (verts.cpu() / (args.res / 2.0) - 1.0)    # keeps the reference's res/2 scale (:90)
     return vertices, faces.cpu(), normals.cpu(), density.cpu().numpy()
+
+
+def extract_geometry_with_super_sampling(model, device, args):
+    """src/mesh_nerf.py:95-128 (which raises NotImplementedError there): extract_geometry with
+    args.super_sampling (>= 1) network samples per crossed grid edge."""
+    assert int(getattr(args, "super_sampling", 0) or 0) >= 1, "super_sampling must be >= 1"
+    return extract_geometry(model, device, args)
 
 
 def _export_obj_python(vertices, triangles, diffuse, normals, filename):
@@ -134,7 +160,10 @@ def cached_geometry(args, build):
 
 
 def export_marching_cubes(model, args, cfg=None, device="cuda"):
-    """src/mesh_nerf.py:131-201 without the super-sampling branch (PyMCubes): geometry (or its cache) -> appearance -> OBJ."""
+    """src/mesh_nerf.py:131-201: geometry (or its cache) -> appearance -> OBJ.  With args.super_sampling >= 1 the geometry
+    comes from super-sampled marching cubes (extract_geometry) and the cache stores the refined vertices.  The reference's
+    branch would have written a geometry-only OBJ through PyMCubes but raises before it runs, so there is no behaviour to
+    match: the refined mesh goes through the same appearance pass and OBJ writer as s = 0."""
     import os
     vertices, triangles, normals, density = cached_geometry(args, lambda: extract_geometry(model, device, args))
     diffuse = mesh_appearance(model, vertices, normals, args)

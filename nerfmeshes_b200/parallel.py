@@ -249,7 +249,8 @@ def extract_geometry_sharded(model, args, group=None, to_host=True, timings=None
          [vertices | normals | faces] (padded to the largest slab) leaves the whole mesh on every rank.
     A vertex belongs to the rank that owns its grid point, and the last owned cell layer addresses the next rank's
     vertices by the ids that rank assigns (nm_mc_count / nm_mc_emit), so the concatenation IS the single-GPU mesh — same
-    arrays, bit for bit; there are no duplicates to remove.  Returns (vertices, triangles, normals, iso) like the single-GPU
+    arrays, bit for bit; there are no duplicates to remove.  args.super_sampling = s >= 1 emits through nm_mc_emit_ss
+    (super-sampled edge vertices, the same arrays as single-GPU extract_geometry with that s).  Returns (vertices, triangles, normals, iso) like the single-GPU
     function (vertices rescaled to (-limit, limit) when to_host).  Works without a process group (one slab)."""
     import numpy as np
     rank, world = _rank_world(group)
@@ -292,10 +293,17 @@ def extract_geometry_sharded(model, args, group=None, to_host=True, timings=None
     tm.mark("stats")
     shard = (iso, buf0, res, own0 - buf0, own1 - buf0)
     nv, nt = eng.mc_count(buf, *shard)
+    s = int(getattr(args, "super_sampling", 0) or 0)
+    if s:          # super-sampled vertices: the network is evaluated at the edge samples directly, no extra halo planes
+        from .mesh import super_sampling_tables
+        lins, fines = super_sampling_tables(args.limit, res, s)
+        emit = lambda *a, out: eng.mc_emit_ss(*a, s, lins, fines, out=out)
+    else:
+        emit = lambda *a, out: eng.mc_emit(*a, out=out)
     if world == 1:
         outs = (_scratch("v", 3 * nv, torch.float32, dev).view(nv, 3), _scratch("n", 3 * nv, torch.float32, dev).view(nv, 3),
                 _scratch("f", 3 * nt, torch.int32, dev).view(nt, 3))
-        v, f, n = eng.mc_emit(buf, *shard, nv, nt, 0, out=outs)
+        v, f, n = emit(buf, *shard, nv, nt, 0, out=outs)
         tm.mark("mc")
         tm.mark("gather")
     else:
@@ -312,7 +320,7 @@ def extract_geometry_sharded(model, args, group=None, to_host=True, timings=None
         local = _scratch("local", seg, torch.float32, dev)
         full = _scratch("full", world * seg, torch.float32, dev)
         views = (local[:3 * vmax].view(vmax, 3), local[3 * vmax:6 * vmax].view(vmax, 3), local[6 * vmax:].view(torch.int32).view(tmax, 3))
-        eng.mc_emit(buf, *shard, nv, nt, v_base, out=views)
+        emit(buf, *shard, nv, nt, v_base, out=views)
         tm.mark("mc")
         dist.all_gather_into_tensor(full, local, group=group)
         full = full.view(world, seg)
