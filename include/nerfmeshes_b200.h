@@ -193,6 +193,30 @@ int nm_mc_emit_ss(NmHandle h, const float* vol_dev, int nb, int ny, int nz, floa
                   const float* fine0_host, const float* fine1_host, const float* fine2_host,
                   float* verts_dev, float* normals_dev, int32_t* faces_dev, void* stream);
 
+/* ---- chamfer evaluation: the chamfer branch of validation_epoch_end (src/models/model_base.py:82-102) -------------------
+ * Argument errors (null pointers, negative sizes, empty point sets or meshes, sizes >= 2^31) are rejected before anything is
+ * launched; N = 0 (n = 0) succeeds and launches nothing.  Definitions: DESIGN §4.7.
+ *
+ * pytorch3d.ops.sample_points_from_meshes (model_base.py:94-96): n points on the mesh verts (V,3) fp32 / faces (F,3) int32,
+ * faces chosen with probability proportional to area (first f with cdf[f] > u * total, cdf the double prefix sum of the
+ * fp32 areas), barycentric weights w0 = 1 - sqrt(a), w1 = sqrt(a)(1 - b), w2 = sqrt(a) b; u, a, b = splitmix64 draws
+ * 3k, 3k+1, 3k+2 of `seed`.  points (n,3); face_idx (n,) int32 or NULL.  A face index outside [0,V) or a total area that
+ * is not positive and finite is reported through the device-side error word (nm_check_flags raises it, once). */
+int nm_mesh_sample(NmHandle h, const float* verts_dev, int64_t V, const int32_t* faces_dev, int64_t F, int64_t n, uint64_t seed,
+                   float* points_dev, int32_t* face_idx_dev_or_null, void* stream);
+/* The nearest-neighbour search inside pytorch3d.loss.chamfer_distance (model_base.py:99): for each of N queries q (N,3) the
+ * squared distance to the nearest of M >= 1 points p (M,3), dist2 (N,), and that point's index (N,) int32 or NULL, the
+ * lowest index on ties.  Exact (an fp32 distance, fmaf(dz,dz,fmaf(dy,dy,dx*dx))) by a uniform grid search. */
+int nm_nearest(NmHandle h, const float* q_dev, int64_t N, const float* p_dev, int64_t M, float* dist2_dev,
+               int32_t* idx_dev_or_null, void* stream);
+/* pytorch3d.loss.chamfer_distance(x, y) without weights or normals (model_base.py:99): means_dev (2 doubles, device) =
+ * {mean_i d2(x_i, Y), mean_j d2(y_j, X)}, reduced in double in a fixed order (the same bits on every run); the chamfer
+ * loss is their sum. */
+int nm_chamfer(NmHandle h, const float* x_dev, int64_t N, const float* y_dev, int64_t M, double* means_dev, void* stream);
+/* Test hook: nm_nearest by tiled brute force (the same distance function, same arguments). */
+int nm_debug_nearest_brute(NmHandle h, const float* q_dev, int64_t N, const float* p_dev, int64_t M, float* dist2_dev,
+                           int32_t* idx_dev_or_null, void* stream);
+
 /* Replaces export_obj (src/nerf/nerf_helpers.py:86-111): `v x y z [r g b]`, `vn x y z`, `f i//i j//j k//k` (1-based) with
  * byte-identical number formatting (python repr of the float32 widened to double).  Host arrays, no GPU involved;
  * diffuse may be NULL or shorter than the vertex list (vertices beyond it get no colour, like the reference's

@@ -10,8 +10,9 @@ from .engine import Engine, RenderSettings
 from .models import (BaseModel, BuFFModel, FlexibleNeRFModel, NeRFModel, OutputBundle, TreeSampling,
                      load_lightning_checkpoint)
 from .nerf_api import get_ray_bundle, meshgrid_xy, ndc_rays, pose_spherical
-from .mesh import (extract_geometry, extract_geometry_with_super_sampling, extract_iso_level, extract_radiance, marching_cubes,
-                   super_sampling_tables)
+from .mesh import (extract_geometry, extract_geometry_with_super_sampling, extract_iso_level, extract_radiance, load_obj,
+                   marching_cubes, super_sampling_tables)
+from .chamfer import Meshes, chamfer_distance, create_mesh, sample_points_from_meshes
 from .train import training_step
 
 __all__ = [n for n in dir() if not n.startswith("_")]

@@ -48,7 +48,9 @@ struct NmHandle_t {
   // workspace
   Buf t_c, raw_c, w_c, t_f, raw_f, t_u, dirs, origins, lin[3], small, stage_in[3], stage_out[12];
   int lin_n[3] = {0, 0, 0};
-  int* d_err = nullptr;       // [0] tensor-core pipeline watchdog code, [1] aabb hit-list overflow (device alias of h_err)
+  int* d_err = nullptr;       // [0] tensor-core pipeline watchdog code, [1] aabb hit-list overflow, [2] mesh sampler input
+                              // error (1: face index out of range, 2: total area not positive; cleared when reported)
+                              // (device alias of h_err)
   int* h_err = nullptr;       // mapped pinned host memory: still readable after a device-side trap
   double* d_stats = nullptr;
   cudaStream_t own_stream = nullptr;
@@ -64,6 +66,7 @@ struct NmHandle_t {
   void* mc_ws2_ptr = nullptr;
   int64_t mc_counts[2] = {0, 0};   // {vertices, triangles} of the last count step: sizes of the emit step
   Buf ss_tab, ss_ws;               // super-sampled emit: the six coordinate tables; chunk points (M,3) + sigma (M,)
+  Buf ms_ws, nn_ws;                // chamfer evaluation: surface sampler (areas, cdf); grid nearest-neighbour search
   // training (nm_train.cu): gradient accumulators per network + scratch
   Buf g_wt[2], g_bias[2], g_head[2], train_ws, dout, trans, tr_rgb[2], tr_drgb[2];
   bool grads_ready = false;
@@ -118,6 +121,10 @@ int check_kernel_flags(NmHandle h) {
   const volatile int* flags = h->h_err;
   NM_CHECK(flags[0] == 0, "tensor-core pipeline watchdog fired (code %d)", flags[0]);
   NM_CHECK(flags[1] == 0, "AABB sampler: more than 512 voxel hits on one ray (samples / voxel indices of that ray are truncated)");
+  if (const int c = flags[2]) {     // a bad input mesh, not a broken device: reported once
+    h->h_err[2] = 0;
+    NM_CHECK(false, c == 1 ? "mesh sampler: a face index lies outside [0, V)" : "mesh sampler: the total face area is not positive and finite");
+  }
   return 0;
 }
 
@@ -457,8 +464,8 @@ int nm_create(int device, const NmNetDesc* coarse, const NmNetDesc* fine, const 
     cudaDeviceProp p;
     NM_CUDA(cudaGetDeviceProperties(&p, device));
     h->num_sms = p.multiProcessorCount;
-    NM_CUDA(cudaHostAlloc(&h->h_err, 2 * sizeof(int), cudaHostAllocMapped));
-    h->h_err[0] = h->h_err[1] = 0;
+    NM_CUDA(cudaHostAlloc(&h->h_err, 3 * sizeof(int), cudaHostAllocMapped));
+    h->h_err[0] = h->h_err[1] = h->h_err[2] = 0;
     NM_CUDA(cudaHostGetDevicePointer(&h->d_err, h->h_err, 0));
     NM_CUDA(cudaMalloc(&h->d_stats, 4 * sizeof(double)));
     NM_CUDA(cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking));
@@ -482,7 +489,7 @@ int nm_destroy(NmHandle h) {
   for (Buf& b : h->stage_out) b.release();
   for (int i = 0; i < 2; ++i) { h->g_wt[i].release(); h->g_bias[i].release(); h->g_head[i].release(); h->tr_rgb[i].release(); h->tr_drgb[i].release(); }
   h->train_ws.release(); h->dout.release(); h->trans.release();
-  h->ss_tab.release(); h->ss_ws.release();
+  h->ss_tab.release(); h->ss_ws.release(); h->ms_ws.release(); h->nn_ws.release();
   if (h->mc_ws_ptr) cudaFree(h->mc_ws_ptr);
   if (h->mc_ws2_ptr) cudaFree(h->mc_ws2_ptr);
   if (h->h_err) cudaFreeHost(h->h_err);
@@ -836,6 +843,59 @@ int nm_mc_emit_ss(NmHandle h, const float* vol_dev, int nb, int ny, int nz, floa
   }
   return mc_emit_ss(sh, h->mc_ws_ptr, h->mc_ws_bytes, &h->mc_ws2_ptr, &h->mc_ws2_bytes, v_base, nv, nt, ss, verts_dev,
                     normals_dev, faces_dev, st, &h->launches);
+}
+
+// ---------------------------------------------------------------------------------------------- chamfer evaluation
+// Argument checks come before the handle is touched, so a bad call is rejected without a device.
+int nm_mesh_sample(NmHandle h, const float* verts_dev, int64_t V, const int32_t* faces_dev, int64_t F, int64_t n, uint64_t seed,
+                   float* points_dev, int32_t* face_idx_dev, void* stream) {
+  NM_CHECK(verts_dev && faces_dev, "mesh sampler: null mesh pointer");
+  NM_CHECK(V > 0 && F > 0, "mesh sampler: empty mesh (V = %lld, F = %lld)", (long long)V, (long long)F);
+  NM_CHECK(n >= 0, "mesh sampler: negative sample count %lld", (long long)n);
+  NM_CHECK(V < (1ll << 31) && F < (1ll << 31) && n < (1ll << 31), "mesh sampler: sizes must be below 2^31");
+  NM_CHECK(n == 0 || points_dev, "mesh sampler: null output pointer");
+  NM_CHECK(h != nullptr, "null handle");
+  if (n == 0) return 0;
+  if (int e = bind_checked(h)) return e;
+  return mesh_sample(verts_dev, V, faces_dev, F, n, seed, points_dev, face_idx_dev, h->d_err + 2, &h->ms_ws.p, &h->ms_ws.cap,
+                     (cudaStream_t)stream, &h->launches);
+}
+
+namespace {
+int check_nn_args(NmHandle h, const float* q, int64_t N, const float* p, int64_t M, const void* out) {
+  NM_CHECK(p, "nearest neighbour: null point pointer");
+  NM_CHECK(N >= 0 && M >= 0, "nearest neighbour: negative size (N = %lld, M = %lld)", (long long)N, (long long)M);
+  NM_CHECK(M > 0, "nearest neighbour: empty point set (M = 0)");
+  NM_CHECK(N < (1ll << 31) && M < (1ll << 31), "nearest neighbour: sizes must be below 2^31");
+  NM_CHECK(N == 0 || (q && out), "nearest neighbour: null query or output pointer");
+  NM_CHECK(h != nullptr, "null handle");
+  return 0;
+}
+}  // namespace
+
+int nm_nearest(NmHandle h, const float* q_dev, int64_t N, const float* p_dev, int64_t M, float* dist2_dev, int32_t* idx_dev,
+               void* stream) {
+  if (int e = check_nn_args(h, q_dev, N, p_dev, M, dist2_dev)) return e;
+  if (N == 0) return 0;
+  if (int e = bind_checked(h)) return e;
+  return nearest(q_dev, N, p_dev, M, dist2_dev, idx_dev, &h->nn_ws.p, &h->nn_ws.cap, (cudaStream_t)stream, &h->launches);
+}
+
+int nm_debug_nearest_brute(NmHandle h, const float* q_dev, int64_t N, const float* p_dev, int64_t M, float* dist2_dev,
+                           int32_t* idx_dev, void* stream) {
+  if (int e = check_nn_args(h, q_dev, N, p_dev, M, dist2_dev)) return e;
+  if (N == 0) return 0;
+  if (int e = bind_checked(h)) return e;
+  return nearest_brute(q_dev, N, p_dev, M, dist2_dev, idx_dev, (cudaStream_t)stream, &h->launches);
+}
+
+int nm_chamfer(NmHandle h, const float* x_dev, int64_t N, const float* y_dev, int64_t M, double* means_dev, void* stream) {
+  NM_CHECK(x_dev && y_dev && means_dev, "chamfer: null pointer");
+  NM_CHECK(N > 0 && M > 0, "chamfer: empty point set (N = %lld, M = %lld)", (long long)N, (long long)M);
+  NM_CHECK(N < (1ll << 31) && M < (1ll << 31), "chamfer: sizes must be below 2^31");
+  NM_CHECK(h != nullptr, "null handle");
+  if (int e = bind_checked(h)) return e;
+  return chamfer(x_dev, N, y_dev, M, means_dev, &h->nn_ws.p, &h->nn_ws.cap, (cudaStream_t)stream, &h->launches);
 }
 
 int nm_marching_cubes_count(NmHandle h, const float* vol_dev, int nx, int ny, int nz, float iso, int64_t* counts_host,

@@ -213,4 +213,18 @@ int mc_emit_ss(const McShard& s, void* ws, size_t ws_bytes, void** ws2, size_t* 
                int64_t nt, const McSuperSampling& ss, float* verts, float* normals, int32_t* faces, cudaStream_t st,
                int64_t* launches);
 
+// chamfer evaluation (nm_chamfer.cu).  ws / ws_bytes: a grow-only workspace of the handle.
+// mesh_sample: n area-weighted surface points (face index per point if face_idx != nullptr); a face index outside [0,V)
+// sets *d_err = 1, a total area that is not positive and finite *d_err = 2 (device-side, mapped memory)
+int mesh_sample(const float* verts, long long V, const int32_t* faces, long long F, long long n, uint64_t seed, float* pts,
+                int32_t* face_idx, int* d_err, void** ws, size_t* ws_bytes, cudaStream_t st, int64_t* launches);
+// exact nearest neighbour of each of N queries among M >= 1 points: squared distance (+ index, lowest on ties)
+int nearest(const float* q, long long N, const float* p, long long M, float* dist2, int32_t* idx, void** ws, size_t* ws_bytes,
+            cudaStream_t st, int64_t* launches);
+int nearest_brute(const float* q, long long N, const float* p, long long M, float* dist2, int32_t* idx, cudaStream_t st,
+                  int64_t* launches);
+// means[0] = mean_i d2(x_i, Y), means[1] = mean_j d2(y_j, X) (double, fixed summation order)
+int chamfer(const float* x, long long N, const float* y, long long M, double* means, void** ws, size_t* ws_bytes, cudaStream_t st,
+            int64_t* launches);
+
 }  // namespace nm

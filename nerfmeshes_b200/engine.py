@@ -471,6 +471,43 @@ class Engine:
                                        _ptr(faces), self._stream()))
         return verts, faces, normals
 
+    # ------------------------------------------------------------------ chamfer evaluation (DESIGN 4.7)
+    def mesh_sample(self, verts, faces, n: int, seed: int, want_faces=False):
+        """sample_points_from_meshes for one mesh (nm_mesh_sample): (n,3) area-weighted surface points [, (n,) int32 face
+        index].  Synchronises and raises if the mesh has a face index outside [0,V) or no area."""
+        v = _f32c(verts, self.device).reshape(-1, 3)
+        f = torch.as_tensor(faces).to(self.device, torch.int32).contiguous().reshape(-1, 3)
+        pts = torch.empty((n, 3), dtype=torch.float32, device=self.device)
+        fi = torch.empty((n,), dtype=torch.int32, device=self.device) if want_faces else None
+        L.check(self.lib.nm_mesh_sample(self._h, _ptr(v), v.shape[0], _ptr(f), f.shape[0], int(n), int(seed) & (2 ** 64 - 1),
+                                        _ptr(pts), _ptr(fi), self._stream()))
+        self.check_flags()
+        return (pts, fi) if want_faces else pts
+
+    def _nn(self, fn, q, p):
+        q, p = _f32c(q, self.device).reshape(-1, 3), _f32c(p, self.device).reshape(-1, 3)
+        d = torch.empty((q.shape[0],), dtype=torch.float32, device=self.device)
+        i = torch.empty((q.shape[0],), dtype=torch.int32, device=self.device)
+        L.check(fn(self._h, _ptr(q), q.shape[0], _ptr(p), p.shape[0], _ptr(d), _ptr(i), self._stream()))
+        return d, i
+
+    def nearest(self, q, p):
+        """Exact nearest neighbour (nm_nearest): for each query of q (N,3), the squared distance to the nearest point of
+        p (M,3) and its index (lowest on ties): ((N,) fp32, (N,) int32)."""
+        return self._nn(self.lib.nm_nearest, q, p)
+
+    def debug_nearest_brute(self, q, p):
+        """Test hook (nm_debug_nearest_brute): nearest() by brute force, the same distance function."""
+        return self._nn(self.lib.nm_debug_nearest_brute, q, p)
+
+    def chamfer(self, x, y) -> torch.Tensor:
+        """chamfer_distance without weights or normals (nm_chamfer): a (2,) float64 device tensor
+        [mean_i d2(x_i, Y), mean_j d2(y_j, X)]; the loss is their sum."""
+        x, y = _f32c(x, self.device).reshape(-1, 3), _f32c(y, self.device).reshape(-1, 3)
+        means = torch.empty((2,), dtype=torch.float64, device=self.device)
+        L.check(self.lib.nm_chamfer(self._h, _ptr(x), x.shape[0], _ptr(y), y.shape[0], _ptr(means), self._stream()))
+        return means
+
     # ------------------------------------------------------------------ introspection
     def kernel_flags(self):
         out = (C.c_int32 * 2)()

@@ -130,6 +130,32 @@ def export_obj(vertices, triangles, diffuse, normals, filename):
                                    ptr(n), n.shape[0]))
 
 
+def load_obj(path):
+    """pytorch3d.io.load_obj's verts / faces.verts_idx for what the commented-out target-mesh loader reads
+    (src/data/datasets.py:88-103): `v x y z [extra]` lines (per-vertex colours, as export_obj writes them, are ignored) and
+    `f` lines with `a`, `a/b`, `a//c` or `a/b/c` entries, 1-based or negative (relative to the vertices read so far);
+    polygons are fan-triangulated.  Returns (float32 (V,3), int32 (F,3)) CPU tensors."""
+    verts, faces = [], []
+    with open(path) as fh:
+        for line in fh:
+            tok = line.split()
+            if not tok:
+                continue
+            if tok[0] == "v":
+                verts.append([float(x) for x in tok[1:4]])
+            elif tok[0] == "f":
+                ids = []
+                for t in tok[1:]:
+                    i = int(t.split("/")[0])
+                    ids.append(i - 1 if i > 0 else len(verts) + i)
+                if len(ids) < 3:
+                    raise ValueError(f"{path}: face with fewer than 3 vertices: {line.strip()}")
+                faces.extend([ids[0], ids[k], ids[k + 1]] for k in range(1, len(ids) - 1))
+    v = torch.tensor(np.asarray(verts, dtype=np.float32).reshape(-1, 3))
+    f = torch.tensor(np.asarray(faces, dtype=np.int32).reshape(-1, 3))
+    return v, f
+
+
 def mesh_appearance(model, vertices, normals, args):
     """The appearance pass of export_marching_cubes (src/mesh_nerf.py:160-192): per-vertex colour, either the raw network
     colour at the vertex (no_view_dependence) or a short ray cast along -normal through model.query — one batched call
