@@ -289,12 +289,17 @@ int nm_debug_gemm(NmHandle h, const float* a_dev, const float* b_dev, int M, int
 int nm_debug_mlp_backward(NmHandle h, int which, const float* pts_dev, const float* dirs_dev, int64_t M, const float* dout_dev,
                           void* stream);
 
-/* ---- host-only debugging aid (no CUDA): the layer program + tensor-core weight stream nm_load_weights would
- * upload, for CPU tests of the schedule / swizzle logic.  program_out receives the internal NetProgram struct
+/* ---- host-only debugging aid (no CUDA): the layer program + tensor-core weight blocks (64x64, 128B-swizzled, schedule
+ * order), for CPU tests of the schedule / swizzle logic.  program_out receives the internal NetProgram struct
  * (nerfmeshes_b200/csrc/nm_program.h). */
 int nm_debug_pack(const NmNetDesc* desc, int n_tensors, const char* const* names, const float* const* tensors_host,
                   const int64_t* numel, int sigma_only, void* program_out, size_t program_cap, uint8_t* pack_out,
                   size_t pack_cap, size_t* pack_need);
+/* The same blocks regrouped into the wide stream nm_load_weights uploads and the wgmma kernel reads (layout:
+ * nm_program.h wide_offset). */
+int nm_debug_pack_wide(const NmNetDesc* desc, int n_tensors, const char* const* names, const float* const* tensors_host,
+                       const int64_t* numel, int sigma_only, void* program_out, size_t program_cap, uint8_t* pack_out,
+                       size_t pack_cap, size_t* pack_need);
 
 /* Host-only: how the fused compositor deals 64-point tiles to the kernel's workers (two consumer warpgroups per CTA) for
  * `samples_per_ray` samples (nm_mlp_tc.cu).  Returns the group size g = lcm(S,64)/64 (0: the fused compositor is not used

@@ -975,7 +975,19 @@ int nm_debug_pack(const NmNetDesc* desc, int n_tensors, const char* const* names
   NM_CHECK(program_cap >= sizeof(NetProgram), "program buffer too small (%zu needed)", sizeof(NetProgram));
   WeightSource src;
   src.n = n_tensors; src.names = names; src.ptrs = tensors_host; src.numel = numel;
-  return debug_pack(*desc, src, sigma_only != 0, reinterpret_cast<NetProgram*>(program_out), pack_out, pack_cap, pack_need);
+  return debug_pack(*desc, src, sigma_only != 0, false, reinterpret_cast<NetProgram*>(program_out), pack_out, pack_cap,
+                    pack_need);
+}
+
+int nm_debug_pack_wide(const NmNetDesc* desc, int n_tensors, const char* const* names, const float* const* tensors_host,
+                       const int64_t* numel, int sigma_only, void* program_out, size_t program_cap, uint8_t* pack_out,
+                       size_t pack_cap, size_t* pack_need) {
+  NM_CHECK(desc && program_out && pack_need, "null argument");
+  NM_CHECK(program_cap >= sizeof(NetProgram), "program buffer too small (%zu needed)", sizeof(NetProgram));
+  WeightSource src;
+  src.n = n_tensors; src.names = names; src.ptrs = tensors_host; src.numel = numel;
+  return debug_pack(*desc, src, sigma_only != 0, true, reinterpret_cast<NetProgram*>(program_out), pack_out, pack_cap,
+                    pack_need);
 }
 
 int nm_check_flags(NmHandle h, void* stream) {

@@ -38,7 +38,7 @@ struct NetDev {
   // device arrays
   NetProgram* d_full = nullptr;
   NetProgram* d_sigma = nullptr;
-  uint8_t* d_wpack_full = nullptr;   // tensor-core weight stages, issue order of `full`
+  uint8_t* d_wpack_full = nullptr;   // tensor-core weight stages of `full`: the wide stream (nm_program.h)
   uint8_t* d_wpack_sigma = nullptr;
   float* d_bias = nullptr;
   float* d_head = nullptr;
@@ -118,8 +118,8 @@ struct WeightSource {
 int pack_network(const NmNetDesc& d, const WeightSource& src, NetDev* net);
 int load_network_dev(const NmNetDesc& d, const WeightSource& src_device, NetDev* net, cudaStream_t st, int64_t* launches);
 void free_network(NetDev* net);
-int debug_pack(const NmNetDesc& d, const WeightSource& src, bool sigma_only, NetProgram* prog, uint8_t* out, size_t cap,
-               size_t* need);
+int debug_pack(const NmNetDesc& d, const WeightSource& src, bool sigma_only, bool wide, NetProgram* prog, uint8_t* out,
+               size_t cap, size_t* need);
 
 // kernel launchers (return 0 / <0; count launches via *launches)
 struct CompositeArgs;

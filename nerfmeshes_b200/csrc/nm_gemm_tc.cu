@@ -51,12 +51,12 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[2][64], uint32_t a, uint
     const uint32_t bs = stage + kPtileBytes * (uint32_t)(1 + j);
     const uint64_t b_hi = ptx::make_kmajor_sw128_desc(bs), b_lo = ptx::make_kmajor_sw128_desc(bs + kPtileHalf);
 #pragma unroll
-    for (int k = 0; k < 4; ++k) ptx::wgmma_m64n128<1, 0>(acc[j], a_hi + k * a_step, b_hi + k * b_step, 1u);
+    for (int k = 0; k < 4; ++k) ptx::wgmma<128, 1, 0, 1>(acc[j], a_hi + k * a_step, b_hi + k * b_step, 1u);
     if (n_passes == 3) {
 #pragma unroll
-      for (int k = 0; k < 4; ++k) ptx::wgmma_m64n128<1, 0>(acc[j], a_lo + k * a_step, b_hi + k * b_step, 1u);
+      for (int k = 0; k < 4; ++k) ptx::wgmma<128, 1, 0, 1>(acc[j], a_lo + k * a_step, b_hi + k * b_step, 1u);
 #pragma unroll
-      for (int k = 0; k < 4; ++k) ptx::wgmma_m64n128<1, 0>(acc[j], a_hi + k * a_step, b_lo + k * b_step, 1u);
+      for (int k = 0; k < 4; ++k) ptx::wgmma<128, 1, 0, 1>(acc[j], a_hi + k * a_step, b_lo + k * b_step, 1u);
     }
   }
 }

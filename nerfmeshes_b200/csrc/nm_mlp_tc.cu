@@ -2,8 +2,8 @@
 // -> sigma / rgb heads in ONE persistent kernel.  Activations never leave the SM: the fp32 accumulator of a layer lives
 // in the registers of a warpgroup, whose epilogue turns it (bias, ReLU, fp16 hi/lo split) into the next layer's A
 // operand in shared memory (128B-swizzled K-major tiles that wgmma reads through a descriptor), and the weights stream
-// through a shared-memory ring filled by the bulk-copy (TMA) engine from an L2-resident, pre-swizzled,
-// schedule-ordered image (nm_program.cu).
+// through a shared-memory ring filled by the bulk-copy (TMA) engine from an L2-resident, pre-swizzled image: the wide
+// stream of nm_program.h, whose stages hold 64-deep K-blocks of 128 (64) output rows.
 //
 // Reference semantics: src/nerf/models.py:60-80 (network), src/nerf/modules.py:26-34 (encoding).
 //
@@ -14,11 +14,10 @@
 // CTA = 12 warps:
 //   warps 0-3, 4-7  two consumer warpgroups.  Each owns a 64-point tile at a time (its own tile sequence), its own
 //                   activation buffer (4 K-blocks x hi/lo, 64 KB) and encoding buffer (one K-block x hi/lo, 16 KB), and
-//                   walks the layer program: encodings -> for each layer, m64n64k16 wgmmas of every 64x64 weight block
-//                   into register accumulator chunk nc (4 chunks = 128 fp32 registers per thread) -> epilogue straight
-//                   from the accumulator fragments back into the activation buffer.  While one warpgroup runs its
-//                   epilogue the other keeps the tensor cores busy.
-//   warps 8-11      producer: warp 8 issues cp.async.bulk weight stages (16 KB = one 64x64 block, hi|lo) into the ring.  Both
+//                   walks the layer program: encodings -> for each layer, m64nWk16 wgmmas at W = min(n_out, 128) columns
+//                   into the register accumulator (128 fp32 registers per thread) -> epilogue straight from the
+//                   accumulator fragments back into the activation buffer.
+//   warps 8-11      producer: warp 8 issues cp.async.bulk weight stages (16 KB, hi|lo) into the ring.  Both
 //                   warpgroups consume every stage in schedule order; a stage is free once both have released it
 //                   (empty barrier count 2), so one L2 read of the weights feeds 128 points.
 // The view-direction encoding reuses the encoding buffer: every layer that reads the xyz encoding precedes the one that
@@ -64,6 +63,7 @@ struct TcParams {
   int n_passes;
   float act_scale, act_inv_scale;
   int num_stages;
+  int n_stages;     // stages of the wide weight stream streamed per round at this precision (nm_program.h wide_stages)
   long long n_tiles;
   int* err;
   uint32_t off_wg, off_bias, off_head, off_bars, off_comp;
@@ -123,22 +123,26 @@ __device__ __forceinline__ void split_bf16x2(float a0, float a1, uint32_t* hi, u
   *lo = *reinterpret_cast<const uint32_t*>(&l2);
 }
 
-// One 64x64 weight block: ksteps K=16 steps of every pass (exact: a_hi*b_hi, a_lo*b_hi, a_hi*b_lo) into chunk d.
-template <int BF16>
-__device__ __forceinline__ void mma_block(float* d, uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo, int ksteps,
-                                          int n_passes) {
+// The MMAs of one K-block (four K = 16 steps) into a W-column accumulator d, in the canonical order of every column:
+// HH: a_hi*b_hi then (LH) a_lo*b_hi over the four steps; HL: a_hi*b_lo.  Straight-line: no guard between two wgmmas, so
+// ptxas issues the group back to back.  A and B steps are 32 B apart in their 128B-swizzled K-major tiles.
+template <int W, int HH, int LH, int HL, int BF16>
+__device__ __forceinline__ void mma_kblock(float* d, uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo) {
 #pragma unroll
   for (int k = 0; k < 4; ++k)
-    if (k < ksteps) ptx::wgmma_m64n64<0, 0, BF16>(d, a_hi + 2 * k, b_hi + 2 * k, 1u);
-  if (n_passes == 3) {
+    if (HH) ptx::wgmma<W, 0, 0, BF16>(d, a_hi + 2 * k, b_hi + 2 * k, 1u);
 #pragma unroll
-    for (int k = 0; k < 4; ++k)
-      if (k < ksteps) ptx::wgmma_m64n64<0, 0, BF16>(d, a_lo + 2 * k, b_hi + 2 * k, 1u);
+  for (int k = 0; k < 4; ++k)
+    if (LH) ptx::wgmma<W, 0, 0, BF16>(d, a_lo + 2 * k, b_hi + 2 * k, 1u);
 #pragma unroll
-    for (int k = 0; k < 4; ++k)
-      if (k < ksteps) ptx::wgmma_m64n64<0, 0, BF16>(d, a_hi + 2 * k, b_lo + 2 * k, 1u);
-  }
+  for (int k = 0; k < 4; ++k)
+    if (HL) ptx::wgmma<W, 0, 0, BF16>(d, a_hi + 2 * k, b_lo + 2 * k, 1u);
 }
+
+template <int V>
+struct IntC {
+  static constexpr int value = V;
+};
 
 // MODE 0: inference; 1: training forward (the epilogue also emits the backward's operands); 2: data-gradient chain
 template <int MODE>
@@ -150,7 +154,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
   const int NS = P.num_stages;
   float* s_bias = reinterpret_cast<float*>(smem + P.off_bias);
   float* s_head = reinterpret_cast<float*>(smem + P.off_head);
-  const int n_layers = P.net.n_layers, n_blocks = P.net.n_blocks;
+  const int n_layers = P.net.n_layers, n_stages = P.n_stages;
 
   // ---------------------------------------------------------------- one-time setup
   if (threadIdx.x == 0) {
@@ -180,13 +184,20 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
     if (warp == kProdWarp && lane == 0) {
       int slot = 0;
       uint32_t ph = 0;
-      const uint32_t bytes = (P.n_passes == 3) ? (uint32_t)kStageBytes : (uint32_t)kHalfStage;
+      const bool exact = P.n_passes == 3;
       for (uint32_t i = 0; tile_of(v0, i) >= 0; ++i) {
-        for (int b = 0; b < n_blocks; ++b) {
-          ptx::mbar_wait(bars + kBarWEmpty + 8 * slot, ph ^ 1, P.err, ERR_W_EMPTY);
-          ptx::mbar_expect_tx(bars + kBarWFull + 8 * slot, bytes);
-          ptx::bulk_g2s(sbase + (uint32_t)slot * kStageBytes, P.wpack + (size_t)b * kStageBytes, bytes, bars + kBarWFull + 8 * slot);
-          if (++slot == NS) { slot = 0; ph ^= 1; }
+        int b = 0;                       // image stage
+        for (int li = 0; li < n_layers; ++li) {
+          const LayerProg& L = P.net.layers[li];
+          const bool wide = wide_width(L) == 128;
+          // exact: every stage in full; fast: the hi stages of a 128-wide layer, the hi half of a 64-wide layer's blocks
+          const uint32_t bytes = (exact || wide) ? (uint32_t)kStageBytes : (uint32_t)kHalfStage;
+          for (int e = b + wide_stages(L); b < e; b += (wide && !exact) ? 2 : 1) {
+            ptx::mbar_wait(bars + kBarWEmpty + 8 * slot, ph ^ 1, P.err, ERR_W_EMPTY);
+            ptx::mbar_expect_tx(bars + kBarWFull + 8 * slot, bytes);
+            ptx::bulk_g2s(sbase + (uint32_t)slot * kStageBytes, P.wpack + (size_t)b * kStageBytes, bytes, bars + kBarWFull + 8 * slot);
+            if (++slot == NS) { slot = 0; ph ^= 1; }
+          }
         }
       }
     }
@@ -208,7 +219,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
   const int Lx = P.net.L_xyz, Ld = P.net.L_dir, ix = P.net.inc_xyz, idr = P.net.inc_dir;
   int slot = 0;
   uint32_t ph = 0;
-  float acc[4][32];
+  float acc[128];
   NM_ST(volatile long long* const st = reinterpret_cast<volatile long long*>(smem + P.off_bars + kBarStalls) + 4 * wg;
         if (t == 0) { st[0] = 0; st[1] = 0; st[2] = clock64(); })
 
@@ -353,7 +364,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
     if (tile < 0) {
       // ghost iteration: no tile of our own, but the other warpgroup consumes this round's stages — wait for each stage and
       // hand it straight back
-      for (int b = 0; b < n_blocks; ++b) {
+      for (int b = 0; b < n_stages; ++b) {
         if (t == 0) {
           NM_ST(const long long c0 = clock64();)
           ptx::mbar_wait(bars + kBarWFull + 8 * slot, ph, P.err, ERR_W_FULL);
@@ -370,42 +381,66 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
     for (int li = 0; li < n_layers; ++li) {
       const LayerProg& L = P.net.layers[li];
       if (MODE != 2 && L.pe_src == SRC_PE_DIR) encode(tile, true);
-      // ------------------------------------------------------------ main loop: this layer's weight blocks
-      if (L.kind != KIND_LOAD) {
+      // ------------------------------------------------------------ main loop: this layer's stages of the wide stream
+      // (per K-block — the encoding source's first, then the activation K-blocks in ascending order — and column half: the
+      // hi stage's a_hi*b_hi, a_lo*b_hi group, then the lo stage's a_hi*b_lo group; a 64-wide layer has both in one stage).
+      // Width and pass count are fixed per layer, so each instantiation's wgmma groups are straight-line.
+      auto main_loop = [&](auto width, auto exact) {
+        constexpr int N = decltype(width)::value, W = N > 128 ? 128 : N, EX = decltype(exact)::value;
 #pragma unroll
-        for (int c = 0; c < 4; ++c)
-#pragma unroll
-          for (int i = 0; i < 32; ++i) acc[c][i] = 0.f;
-        ptx::wgmma_fence();
+        for (int i = 0; i < 128; ++i) acc[i] = 0.f;
         NM_ST(if (t == 0) st[1] -= clock64() - st[0];)      // + (loop end - loop start) - (waits inside the loop)
         int prev = -1;
-        for (int b = L.blk_begin; b < L.blk_end; ++b) {
-          const BlockProg& B = P.net.blocks[b];
+        // one stage: wait for it, issue its group, release the previous stage once that group's MMAs are complete
+        auto stage = [&](auto issue) {
           NM_ST(const long long c0 = clock64();)
           ptx::mbar_wait_warp(bars + kBarWFull + 8 * slot, ph, P.err, ERR_W_FULL);
           NM_ST(if (t == 0) st[0] += clock64() - c0;)
-          const uint32_t wst = sbase + (uint32_t)slot * kStageBytes;
-          const uint64_t b_hi = ptx::make_kmajor_sw128_desc(wst), b_lo = ptx::make_kmajor_sw128_desc(wst + (uint32_t)kHalfStage);
-          const uint32_t a_t = (B.src == SRC_ACT) ? act_s + (uint32_t)B.kb * kKBlock : pe_s;
-          const uint64_t a_hi = ptx::make_kmajor_sw128_desc(a_t), a_lo = ptx::make_kmajor_sw128_desc(a_t + 8192u);
-          const int ks = (B.src == SRC_ACT) ? 4 : (int)B.ksteps;
-          switch (B.nc) {
-            case 0: mma_block<MODE == 2>(acc[0], a_hi, a_lo, b_hi, b_lo, ks, n_passes); break;
-            case 1: mma_block<MODE == 2>(acc[1], a_hi, a_lo, b_hi, b_lo, ks, n_passes); break;
-            case 2: mma_block<MODE == 2>(acc[2], a_hi, a_lo, b_hi, b_lo, ks, n_passes); break;
-            default: mma_block<MODE == 2>(acc[3], a_hi, a_lo, b_hi, b_lo, ks, n_passes); break;
-          }
+          ptx::wgmma_fence();                        // (what ptxas would otherwise inject before the group, C7519)
+          issue(sbase + (uint32_t)slot * kStageBytes);
           ptx::wgmma_commit();
-          ptx::wgmma_wait<1>();                      // the previous block's MMAs are complete: release its stage
+          ptx::wgmma_wait<1>();
           if (prev >= 0 && t == 0) ptx::mbar_arrive(bars + kBarWEmpty + 8 * prev);
           prev = slot;
           if (++slot == NS) { slot = 0; ph ^= 1; }
+        };
+        const int n_kb = wide_kblocks(L), has_pe = L.pe_src ? 1 : 0;
+        for (int kbi = 0; kbi < n_kb; ++kbi) {
+          const uint32_t a_t = (kbi < has_pe) ? pe_s : act_s + (uint32_t)(kbi - has_pe) * kKBlock;
+          const uint64_t a_hi = ptx::make_kmajor_sw128_desc(a_t), a_lo = ptx::make_kmajor_sw128_desc(a_t + 8192u);
+#pragma unroll
+          for (int h = 0; h < N / W; ++h) {
+            if (W == 64) {
+              stage([&](uint32_t w) {
+                mma_kblock<W, 1, EX, EX, MODE == 2>(acc, a_hi, a_lo, ptx::make_kmajor_sw128_desc(w),
+                                                    ptx::make_kmajor_sw128_desc(w + (uint32_t)kHalfStage));
+              });
+            } else {
+              stage([&](uint32_t w) {
+                const uint64_t b = ptx::make_kmajor_sw128_desc(w);
+                mma_kblock<W, 1, EX, 0, MODE == 2>(acc + 64 * h, a_hi, a_lo, b, b);
+              });
+              if (EX)
+                stage([&](uint32_t w) {
+                  const uint64_t b = ptx::make_kmajor_sw128_desc(w);
+                  mma_kblock<W, 0, 0, 1, MODE == 2>(acc + 64 * h, a_hi, a_lo, b, b);
+                });
+            }
+          }
         }
         ptx::wgmma_wait<0>();
         if (prev >= 0 && t == 0) ptx::mbar_arrive(bars + kBarWEmpty + 8 * prev);
         NM_ST(if (t == 0) st[1] += clock64() - st[0];)
-#pragma unroll
-        for (int c = 0; c < 4; ++c) ptx::fence_regs<32>(acc[c]);
+        ptx::fence_regs<128>(acc);
+      };
+      if (L.kind != KIND_LOAD) {
+        if (L.n_out == 256) {
+          if (n_passes == 3) main_loop(IntC<256>{}, IntC<1>{}); else main_loop(IntC<256>{}, IntC<0>{});
+        } else if (L.n_out == 128) {
+          if (n_passes == 3) main_loop(IntC<128>{}, IntC<1>{}); else main_loop(IntC<128>{}, IntC<0>{});
+        } else {
+          if (n_passes == 3) main_loop(IntC<64>{}, IntC<1>{}); else main_loop(IntC<64>{}, IntC<0>{});
+        }
       }
       // ------------------------------------------------------------ epilogue, straight from the accumulator fragments
       const int NC = L.n_out >> 6;
@@ -452,7 +487,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
               // gradient — are taken by the weight-gradient GEMM from the pack emitted below: nm_gemm_tc.cu a_rowsum.)
 #pragma unroll
               for (int u = 0; u < 2; ++u) {
-                float y = acc[nc][j8 * 4 + 2 * e + u] * so;
+                float y = acc[nc * 32 + j8 * 4 + 2 * e + u] * so;
                 if (L.aux2) y = fmaf(dsg[e], s_head[L.head_off + col + u], y);
                 const uint32_t w = valid ? mk_in[e][j8 >> 2] : 0u;
                 x[e][u] = ((w >> ((col + u) & 31)) & 1u) ? y : 0.f;
@@ -460,7 +495,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
             } else {
 #pragma unroll
               for (int u = 0; u < 2; ++u) {
-                float y = fmaf(acc[nc][j8 * 4 + 2 * e + u], so, s_bias[L.bias_off + col + u]);
+                float y = fmaf(acc[nc * 32 + j8 * 4 + 2 * e + u], so, s_bias[L.bias_off + col + u]);
                 if (L.relu) y = fmaxf(y, 0.f);
                 x[e][u] = y;
               }
@@ -604,6 +639,11 @@ static int launch_prepared(TcParams& P, int num_sms, cudaStream_t st, int64_t* l
   if (ns > kMaxStages) ns = kMaxStages;
   NM_CHECK(ns >= 2, "network too large for the shared-memory budget (%u B fixed, %d B available)", fixed, max_smem);
   P.num_stages = ns;
+  for (int i = 0; i < hp.n_layers; ++i)
+    NM_CHECK(hp.layers[i].kind == KIND_LOAD || hp.layers[i].n_out == 64 || hp.layers[i].n_out == 128 || hp.layers[i].n_out == 256,
+             "layer %d: output width %d not 64, 128 or 256", i, hp.layers[i].n_out);
+  P.n_stages = 0;
+  for (int i = 0; i < hp.n_layers; ++i) P.n_stages += wide_stages(hp.layers[i], P.n_passes == 3 ? 1 : 2);
   uint32_t off = (uint32_t)ns * kStageBytes;
   P.off_wg = off; off += 2 * kWgBytes;
   P.off_bias = off; off += align_up(hp.n_bias * 4, 16);

@@ -1,7 +1,8 @@
 // Host side of the fused MLP: turns the constructor arguments of FlexibleNeRFModel (src/nerf/models.py:5-58) into
 // a layer program + tensor-core block schedule, and packs the reference's (out,in) fp32 weights into
-//   (a) 16 KB tensor-core stages [hi | lo] fp16, K-major, 128B-swizzled, in schedule order (one linear stream the
-//       kernel's producer warp walks with cp.async.bulk), and
+//   (a) 16 KB tensor-core stages [hi | lo] fp16: the canonical 64x64 blocks (K-major, 128B-swizzled, in schedule order;
+//       the CPU checks read them), regrouped into the wide stream (nm_program.h) that the kernel's producer warp walks
+//       with cp.async.bulk, and
 //   (b) transposed fp32 Wt[k][n] for the CUDA-core kernel.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -71,8 +72,8 @@ static bool is_skip(const NmNetDesc& d, int i) {  // src/nerf/models.py:36-42,64
 static int schedule_blocks(NetProgram* p) {
   const int nl = p->n_layers;
   // tensor-core schedule: the block order within a layer (row part first, then the column part of each j) is the order of
-  // the weight stream.  The wgmma kernel (nm_mlp_tc.cu) reads only src / kb / nc / ksteps of each block, in this order, and
-  // blk_begin / blk_end of each layer.  The rest (group, first / last, the per-issuer flags / next / first_blk / none_d /
+  // the canonical block image, which regroup_wide turns into the wide stream the wgmma kernel (nm_mlp_tc.cu) reads; the
+  // kernel itself reads no block.  The rest (group, first / last, the per-issuer flags / next / first_blk / none_d /
   // none_k and accumulate_only) is bookkeeping the kernel does not use; the CPU schedule tests check it.
   const int policy = 1;   // a block's "issuer" owns its accumulator chunk
   p->accumulate_only = policy == 0 ? 1 : 0;
@@ -276,17 +277,39 @@ static int pack_stream(const NetProgram& p, const std::vector<LayerNames>& names
   return 0;
 }
 
-// Host-only view of the packer for CPU tests of the schedule / swizzle logic (no CUDA calls).
-int debug_pack(const NmNetDesc& d, const WeightSource& src, bool sigma_only, NetProgram* prog, uint8_t* out, size_t cap,
-               size_t* need) {
+// The canonical block image regrouped into the wide stream: every element of a block moves to wide_offset() of its layer.
+static void regroup_wide(const NetProgram& p, const std::vector<uint8_t>& canon, std::vector<uint8_t>* wide) {
+  wide->assign((size_t)wide_stage_begin(p, p.n_layers) * kStageBytes, 0);
+  for (int li = 0; li < p.n_layers; ++li) {
+    const LayerProg& L = p.layers[li];
+    uint8_t* base = wide->data() + (size_t)wide_stage_begin(p, li) * kStageBytes;
+    for (int b = L.blk_begin; b < L.blk_end; ++b) {
+      const BlockProg& B = p.blocks[b];
+      const int pe = B.src == SRC_ACT ? 0 : 1;
+      const uint8_t* st = canon.data() + (size_t)b * kStageBytes;
+      for (int r = 0; r < kChunk; ++r)
+        for (int c = 0; c < kChunk; ++c) {
+          const uint32_t o = wide_offset(L, pe, B.nc * kChunk + r, pe ? c : B.kb * kChunk + c);
+          memcpy(base + o, st + swz_off(r, c), 2);
+          memcpy(base + wide_lo_delta(L) + o, st + kHalfStage + swz_off(r, c), 2);
+        }
+    }
+  }
+}
+
+// Host-only views of the packer for CPU tests of the schedule / swizzle logic (no CUDA calls): the canonical block image
+// (wide = false) or the wide stream the kernel reads (wide = true).
+int debug_pack(const NmNetDesc& d, const WeightSource& src, bool sigma_only, bool wide, NetProgram* prog, uint8_t* out,
+               size_t cap, size_t* need) {
   std::vector<LayerNames> names;
   if (int e = build_one(d, sigma_only, prog, &names)) return e;
-  *need = (size_t)prog->n_blocks * kStageBytes;
+  *need = (size_t)(wide ? wide_stage_begin(*prog, prog->n_layers) : prog->n_blocks) * kStageBytes;
   if (!out) return 0;
   NM_CHECK(cap >= *need, "buffer too small");
-  std::vector<uint8_t> pk;
+  std::vector<uint8_t> pk, pw;
   if (int e = pack_stream(*prog, names, src, &pk)) return e;
-  memcpy(out, pk.data(), pk.size());
+  if (wide) regroup_wide(*prog, pk, &pw);
+  memcpy(out, wide ? pw.data() : pk.data(), *need);
   return 0;
 }
 
@@ -326,9 +349,11 @@ int pack_network(const NmNetDesc& d, const WeightSource& src, NetDev* net) {
       memcpy(&head[L.head_off + rows * L.n_out], HB, sizeof(float) * rows);
     }
   }
-  std::vector<uint8_t> pk_full, pk_sig;
-  if (int e = pack_stream(full, nf, src, &pk_full)) return e;
-  if (int e = pack_stream(sig, ns, src, &pk_sig)) return e;
+  std::vector<uint8_t> pk_full, pk_sig, canon;
+  if (int e = pack_stream(full, nf, src, &canon)) return e;
+  regroup_wide(full, canon, &pk_full);
+  if (int e = pack_stream(sig, ns, src, &canon)) return e;
+  regroup_wide(sig, canon, &pk_sig);
 
   free_network(net);
   net->desc = d; net->full = full; net->sigma = sig;
@@ -366,58 +391,61 @@ __global__ void transpose_in_kernel(const float* __restrict__ W, int N, int K, f
   Wt[i] = W[(size_t)n * K + k];
 }
 
-__device__ __forceinline__ uint32_t swz_off_dev(int r, int c) {
-  return (uint32_t)r * 128u + (uint32_t)((((c >> 3) ^ (r & 7)) << 4) + ((c & 7) << 1));
+// Element e (of 8192) of stage `blockIdx.x` of the wide stream: its layer *li, source *pe, (row *n, column *k) of that
+// source and copy *lo (0: hi, 1: lo); every element of the stage (padding included) is visited once, and wide_offset()
+// (+ wide_lo_delta() for a lo copy) of the result is where it goes.
+__device__ __forceinline__ void wide_element(const NetProgram& P, int e, int* li, int* pe, int* n, int* k, int* lo) {
+  int l = 0, s0 = 0;
+  while (l + 1 < P.n_layers && (int)blockIdx.x >= s0 + wide_stages(P.layers[l])) s0 += wide_stages(P.layers[l++]);
+  const LayerProg& L = P.layers[l];
+  const int s = (int)blockIdx.x - s0, W = wide_width(L);
+  int kbi;
+  if (W == 128) {                       // stage = (K-block * halves + half) * 2 + lo, 128 rows x 64 columns
+    kbi = (s >> 1) / (L.n_out / W);
+    *n = ((s >> 1) % (L.n_out / W)) * W + (e >> 6);
+    *lo = s & 1;
+  } else {                              // stage = K-block, [hi | lo] of 64 rows x 64 columns
+    kbi = s;
+    *n = (e & 4095) >> 6;
+    *lo = e >> 12;
+  }
+  *li = l;
+  *pe = (L.pe_src && kbi == 0) ? 1 : 0;
+  *k = (*pe ? 0 : (kbi - (L.pe_src ? 1 : 0)) * 64) + (e & 63);
 }
 
-// one CTA per 16 KB stage of the schedule (pack_stream above, on the device)
+__device__ __forceinline__ uint32_t wide_stage_base(const NetProgram& P, int li) { return (uint32_t)wide_stage_begin(P, li) * kStageBytes; }
+
+// one CTA per 16 KB stage of the wide stream (pack_stream + regroup_wide above, on the device)
 __global__ void __launch_bounds__(256) pack_stream_kernel(const NetProgram* __restrict__ prog, const float* __restrict__ w_rm,
                                                           uint8_t* __restrict__ out) {
   const NetProgram& P = *prog;
-  const int b = blockIdx.x;
-  int li = 0;
-  while (li + 1 < P.n_layers && b >= P.layers[li].blk_end) ++li;
-  const LayerProg& L = P.layers[li];
-  const BlockProg B = P.blocks[b];
-  const int K = L.k_act + L.k_pe;
-  const float* W = w_rm + L.wt_off;
-  uint8_t* st = out + (size_t)b * kStageBytes;
-  for (int e = threadIdx.x; e < kChunk * kChunk; e += blockDim.x) {
-    const int r = e >> 6, c = e & 63;
-    const int n = B.nc * kChunk + r;
-    int kcol;
-    if (B.src == SRC_ACT) kcol = B.kb * kChunk + c;
-    else kcol = (c < L.k_pe) ? L.k_act + c : -1;
-    const float w = (kcol >= 0) ? W[(size_t)n * K + kcol] : 0.f;
+  for (int e = threadIdx.x; e < kStageBytes / 2; e += blockDim.x) {
+    int li, pe, n, k, lo;
+    wide_element(P, e, &li, &pe, &n, &k, &lo);
+    const LayerProg& L = P.layers[li];
+    const int K = L.k_act + L.k_pe;
+    const float w = (!pe || k < L.k_pe) ? w_rm[L.wt_off + (size_t)n * K + (pe ? L.k_act + k : k)] : 0.f;
     const __half hi = __float2half_rn(w);
-    const __half lo = __float2half_rn(w - __half2float(hi));
-    *reinterpret_cast<__half*>(st + swz_off_dev(r, c)) = hi;
-    *reinterpret_cast<__half*>(st + kHalfStage + swz_off_dev(r, c)) = lo;
+    *reinterpret_cast<__half*>(out + wide_stage_base(P, li) + wide_offset(L, pe, n, k) + (lo ? wide_lo_delta(L) : 0u)) =
+        lo ? __float2half_rn(w - __half2float(hi)) : hi;
   }
 }
 
-// stages of the backward program: block (kb, nc) of layer L holds rows n' = nc*64.. (input feature of forward layer L.aux)
-// and columns k' = kb*64.. (its output feature) of W^T, i.e. Wt[n'][k'] with Wt = the transposed fp32 weights (ld = the
-// forward layer's n_out); bf16 hi/lo split (gradients span fp32's exponent range)
+// wide stream of the backward program: layer L's element (n', k') is W^T[n'][k'] — row n' an input feature of forward
+// layer L.aux, column k' one of its output features — read from the transposed fp32 weights (ld = the forward layer's
+// n_out); bf16 hi/lo split (gradients span fp32's exponent range)
 __global__ void __launch_bounds__(256) pack_bwd_stream_kernel(const NetProgram* __restrict__ prog, const float* __restrict__ wt,
                                                               uint8_t* __restrict__ out) {
   const NetProgram& P = *prog;
-  const int b = blockIdx.x;
-  int li = 0;
-  while (li + 1 < P.n_layers && b >= P.layers[li].blk_end) ++li;
-  const LayerProg& L = P.layers[li];
-  const BlockProg B = P.blocks[b];
-  const int ld = L.k_act;                          // forward n_out
-  const float* W = wt + L.wt_off;
-  uint8_t* st = out + (size_t)b * kStageBytes;
-  for (int e = threadIdx.x; e < kChunk * kChunk; e += blockDim.x) {
-    const int r = e >> 6, c = e & 63;
-    const int n = B.nc * kChunk + r, k = B.kb * kChunk + c;
-    const float w = (n < L.n_out && k < L.k_act) ? W[(size_t)n * ld + k] : 0.f;
+  for (int e = threadIdx.x; e < kStageBytes / 2; e += blockDim.x) {
+    int li, pe, n, k, lo;
+    wide_element(P, e, &li, &pe, &n, &k, &lo);
+    const LayerProg& L = P.layers[li];
+    const float w = wt[L.wt_off + (size_t)n * L.k_act + k];
     const __nv_bfloat16 hi = __float2bfloat16_rn(w);
-    const __nv_bfloat16 lo = __float2bfloat16_rn(w - __bfloat162float(hi));
-    *reinterpret_cast<__nv_bfloat16*>(st + swz_off_dev(r, c)) = hi;
-    *reinterpret_cast<__nv_bfloat16*>(st + kHalfStage + swz_off_dev(r, c)) = lo;
+    *reinterpret_cast<__nv_bfloat16*>(out + wide_stage_base(P, li) + wide_offset(L, pe, n, k) + (lo ? wide_lo_delta(L) : 0u)) =
+        lo ? __float2bfloat16_rn(w - __bfloat162float(hi)) : hi;
   }
 }
 
@@ -429,9 +457,9 @@ int build_backward_stream(NetDev* net, cudaStream_t st, int64_t* launches) {
     if (int e = build_backward_program(net->full, &net->bwd)) return e;
     NM_CUDA(cudaMalloc(&net->d_bwd, sizeof(NetProgram)));
     NM_CUDA(cudaMemcpyAsync(net->d_bwd, &net->bwd, sizeof(NetProgram), cudaMemcpyHostToDevice, st));
-    NM_CUDA(cudaMalloc(&net->d_wpack_bwd, (size_t)net->bwd.n_blocks * kStageBytes));
+    NM_CUDA(cudaMalloc(&net->d_wpack_bwd, (size_t)wide_stage_begin(net->bwd, net->bwd.n_layers) * kStageBytes));
   }
-  pack_bwd_stream_kernel<<<net->bwd.n_blocks, 256, 0, st>>>(net->d_bwd, net->d_wt, net->d_wpack_bwd);
+  pack_bwd_stream_kernel<<<wide_stage_begin(net->bwd, net->bwd.n_layers), 256, 0, st>>>(net->d_bwd, net->d_wt, net->d_wpack_bwd);
   NM_CUDA(cudaGetLastError());
   if (launches) ++*launches;
   net->bwd_valid = true;
@@ -452,8 +480,8 @@ int load_network_dev(const NmNetDesc& d, const WeightSource& src, NetDev* net, c
     for (const LayerNames& n : nf) { net->names.push_back(n.w); net->names.push_back(n.b); net->names.push_back(n.head_w); net->names.push_back(n.head_b); }
     NM_CUDA(cudaMalloc(&net->d_full, sizeof(NetProgram)));
     NM_CUDA(cudaMalloc(&net->d_sigma, sizeof(NetProgram)));
-    NM_CUDA(cudaMalloc(&net->d_wpack_full, (size_t)full.n_blocks * kStageBytes));
-    NM_CUDA(cudaMalloc(&net->d_wpack_sigma, (size_t)sig.n_blocks * kStageBytes));
+    NM_CUDA(cudaMalloc(&net->d_wpack_full, (size_t)wide_stage_begin(full, full.n_layers) * kStageBytes));
+    NM_CUDA(cudaMalloc(&net->d_wpack_sigma, (size_t)wide_stage_begin(sig, sig.n_layers) * kStageBytes));
     NM_CUDA(cudaMalloc(&net->d_bias, (size_t)full.n_bias * sizeof(float)));
     NM_CUDA(cudaMalloc(&net->d_head, (size_t)(full.n_head > 0 ? full.n_head : 1) * sizeof(float)));
     NM_CUDA(cudaMalloc(&net->d_wt, wt_total * sizeof(float)));
@@ -482,9 +510,9 @@ int load_network_dev(const NmNetDesc& d, const WeightSource& src, NetDev* net, c
       NM_CUDA(cudaMemcpyAsync(net->d_head + L.head_off + rows * N, HB, sizeof(float) * rows, cudaMemcpyDeviceToDevice, st));
     }
   }
-  pack_stream_kernel<<<full.n_blocks, 256, 0, st>>>(net->d_full, net->d_w, net->d_wpack_full);
+  pack_stream_kernel<<<wide_stage_begin(full, full.n_layers), 256, 0, st>>>(net->d_full, net->d_w, net->d_wpack_full);
   NM_CUDA(cudaGetLastError());
-  pack_stream_kernel<<<sig.n_blocks, 256, 0, st>>>(net->d_sigma, net->d_w, net->d_wpack_sigma);
+  pack_stream_kernel<<<wide_stage_begin(sig, sig.n_layers), 256, 0, st>>>(net->d_sigma, net->d_w, net->d_wpack_sigma);
   NM_CUDA(cudaGetLastError());
   if (launches) *launches += 2;
   net->bwd_valid = false;

@@ -14,7 +14,7 @@ constexpr int kMaxFreq = 16;
 constexpr int kIssuers = 4;           // schedule bookkeeping only (BlockProg.flags >> 4); the wgmma kernel does not read it
 constexpr int kTileM = 64;           // points per tile (= rows of one warpgroup MMA)
 constexpr int kChunk = 64;           // N-chunk / K-block width
-constexpr int kStageBytes = 16384;   // one weight stage: [hi 64x64 fp16 | lo 64x64 fp16], 128B-swizzled K-major
+constexpr int kStageBytes = 16384;   // one weight stage / canonical block: [hi 64x64 fp16 | lo 64x64 fp16]
 constexpr int kHalfStage = 8192;
 
 enum : int { SRC_ACT = 0, SRC_PE_XYZ = 1, SRC_PE_DIR = 2 };
@@ -76,5 +76,44 @@ struct NetProgram {
   LayerProg layers[kMaxLayers];
   BlockProg blocks[kMaxBlocks];
 };
+
+// ---- the wide weight stream: what the wgmma kernel's ring walks (packers: nm_program.cu, reader: nm_mlp_tc.cu)
+// The canonical 64x64 blocks above are the unit of scheduling and of the CPU checks; the device streams a layer at an MMA
+// width W = min(n_out, 128) (n_out / W column halves).  Inside a layer, for every K-block of 64 (the encoding source first
+// if the layer has one, then the activation K-blocks in ascending order) and every column half h:
+//   W = 128: two 16 KB stages, the hi then the lo fp16 (bf16) copy of the 128 x 64 tile (rows h*128.., 128B-swizzled
+//            K-major: 16-byte chunk c of row r at r * 128 + ((c ^ (r % 8)) << 4)), i.e. the hi (lo) halves of the two
+//            canonical blocks nc = 2h, 2h + 1 stacked.  Fast precision streams only the hi stages.
+//   W = 64:  one stage, the canonical block itself [hi 8 KB | lo 8 KB] (fast precision: its hi half).
+// Each K-block's MMAs thus keep the canonical order of every output column: a_hi*b_hi over its four K = 16 steps, then
+// a_lo*b_hi, then a_hi*b_lo, one m64nWk16 wgmma each.
+#if defined(__CUDACC__)
+#define NM_HD __host__ __device__ __forceinline__
+#else
+#define NM_HD inline
+#endif
+NM_HD int wide_width(const LayerProg& L) { return L.n_out > 128 ? 128 : L.n_out; }
+NM_HD int wide_kblocks(const LayerProg& L) { return L.kind == KIND_LOAD ? 0 : (L.pe_src ? 1 : 0) + L.k_act / 64; }
+// stages of the layer in the image (stream = 0) or streamed at the given precision (stream = 1: exact, 2: fast)
+NM_HD int wide_stages(const LayerProg& L, int stream = 0) {
+  const int W = wide_width(L), per = (W == 128 && stream != 2) ? 2 : 1;
+  return wide_kblocks(L) * (L.n_out / W) * per;
+}
+// first image stage of layer li (li = n_layers: the image's stage count)
+NM_HD int wide_stage_begin(const NetProgram& p, int li) {
+  int s = 0;
+  for (int i = 0; i < li; ++i) s += wide_stages(p.layers[i]);
+  return s;
+}
+// distance of an element's lo copy from its hi copy
+NM_HD uint32_t wide_lo_delta(const LayerProg& L) { return wide_width(L) == 128 ? (uint32_t)kStageBytes : (uint32_t)kHalfStage; }
+// byte offset, from the layer's first stage, of the hi copy of element (row n, column k) of source pe (1: the encoding,
+// k < 64; 0: the activations, k < k_act)
+NM_HD uint32_t wide_offset(const LayerProg& L, int pe, int n, int k) {
+  const int W = wide_width(L), kbi = pe ? 0 : (L.pe_src ? 1 : 0) + (k >> 6);
+  const int stage = (kbi * (L.n_out / W) + n / W) * (W == 128 ? 2 : 1), r = n % W, c = k & 63;
+  return (uint32_t)stage * (uint32_t)kStageBytes + (uint32_t)r * 128u + (uint32_t)((((c >> 3) ^ (r & 7)) << 4) + ((c & 7) << 1));
+}
+#undef NM_HD
 
 }  // namespace nm

@@ -116,13 +116,14 @@ def layer_runs(prog):
             if prog.layers[i].blk_end > prog.layers[i].blk_begin]
 
 
-def simulate(prog, tiles, NS, seeds=(0, 1, 2), release_count=2):
+def simulate(prog, tiles, NS, seeds=(0, 1, 2), release_count=2, runs=None):
     """The MLP kernel on one CTA processing `tiles` 64-point tiles: warpgroup 0 takes tiles 0, 2, 4, ..., warpgroup 1 tiles
-    1, 3, ...; rounds = ceil(tiles / 2), warpgroup 1 ghosts the last round when tiles is odd."""
+    1, 3, ...; rounds = ceil(tiles / 2), warpgroup 1 ghosts the last round when tiles is odd.  runs: stages per layer (as
+    run_ring takes them), by default the layer program's block runs (layer_runs)."""
     rounds = (tiles + 1) // 2
     own = lambda wg, r: 2 * r + wg < tiles
     for seed in seeds:
-        ok, info = run_ring(NS, rounds, layer_runs(prog), own, seed, release_count)
+        ok, info = run_ring(NS, rounds, layer_runs(prog) if runs is None else runs, own, seed, release_count)
         if not ok:
             return False, f"seed {seed}: {info}"
     return True, "ok"
