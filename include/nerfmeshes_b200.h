@@ -289,6 +289,15 @@ int nm_debug_gemm(NmHandle h, const float* a_dev, const float* b_dev, int M, int
 int nm_debug_mlp_backward(NmHandle h, int which, const float* pts_dev, const float* dirs_dev, int64_t M, const float* dout_dev,
                           void* stream);
 
+/* Test hook for the training compositor adjoint alone (composite_backward_kernel, nm_train.cu): from raw_dev (R,S,4) =
+ * (sigmoid rgb, raw sigma), t_dev (R,S), dirs_dev (R,3) and d_rgb_dev (R,3) = dL/d rgb_map it writes dout_dev (R,S,4) =
+ * [dL/d rgb logits (through the sigmoid), dL/d raw sigma], the per-point adjoint nm_debug_mlp_backward takes.  noise_std
+ * and seed are the sigma noise of the forward: seed is the compositor's stream, already salted (the training backward
+ * passes seed ^ salt of the pass).  1 <= S <= 512; raw_dev and dout_dev 16-byte aligned; R = 0 launches nothing. */
+int nm_debug_composite_backward(NmHandle h, const float* raw_dev, const float* t_dev, const float* dirs_dev,
+                                const float* d_rgb_dev, int64_t R, int S, float noise_std, uint64_t seed, int white_bg,
+                                float* dout_dev, void* stream);
+
 /* ---- host-only debugging aid (no CUDA): the layer program + tensor-core weight blocks (64x64, 128B-swizzled, schedule
  * order), for CPU tests of the schedule / swizzle logic.  program_out receives the internal NetProgram struct
  * (nerfmeshes_b200/csrc/nm_program.h). */

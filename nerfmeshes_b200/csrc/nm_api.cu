@@ -697,6 +697,22 @@ int nm_debug_mlp_backward(NmHandle h, int which, const float* pts_dev, const flo
   return mlp_backward(net, in, dout_dev, ws, &g, h->num_sms, mode, st, &h->launches, 0);
 }
 
+int nm_debug_composite_backward(NmHandle h, const float* raw_dev, const float* t_dev, const float* dirs_dev,
+                                const float* d_rgb_dev, int64_t R, int S, float noise_std, uint64_t seed, int white_bg,
+                                float* dout_dev, void* stream) {
+  if (int e = bind_checked(h)) return e;
+  NM_CHECK(raw_dev && t_dev && dirs_dev && d_rgb_dev && dout_dev, "null pointer argument");
+  NM_CHECK(R >= 0, "negative ray count %lld", (long long)R);
+  NM_CHECK(S >= 1 && S <= 512, "samples per ray %d outside [1, 512] (the compositor adjoint holds 16 per lane)", S);
+  NM_CHECK((reinterpret_cast<uintptr_t>(raw_dev) & 15) == 0 && (reinterpret_cast<uintptr_t>(dout_dev) & 15) == 0,
+           "raw and dout must be 16-byte aligned (R,S,4) arrays");
+  if (R == 0) return 0;
+  // the same call as train_chunk's, with the transmittance scratch it passes
+  if (int e = h->trans.ensure((size_t)R * S * 4)) return e;
+  return launch_composite_backward(raw_dev, t_dev, dirs_dev, d_rgb_dev, R, S, noise_std, seed, white_bg, h->trans.as<float>(),
+                                   dout_dev, (cudaStream_t)stream, &h->launches);
+}
+
 // ---------------------------------------------------------------------------------------------- BuFF tree maintenance
 int nm_ray_voxel_indices(NmHandle h, const float* origins_dev, int o_stride, const float* dirs_dev, int64_t R,
                          const float* near_far_host, float* z_out_dev, int32_t* idx_out_dev, void* stream) {

@@ -323,6 +323,19 @@ class Engine:
         assert g.shape == (M, 4) and (d is None or d.shape == (M, 3)), (p.shape, g.shape)
         L.check(self.lib.nm_debug_mlp_backward(self._h, which, _ptr(p), _ptr(d), M, _ptr(g), self._stream()))
 
+    def debug_composite_backward(self, raw, t, dirs, d_rgb, *, noise_std=0.0, seed=0, white_bg=False):
+        """Test hook (nm_debug_composite_backward): the training compositor adjoint alone.  raw (R,S,4) = (sigmoid rgb,
+        raw sigma), t (R,S), dirs (R,3), d_rgb (R,3) = dL/d rgb_map; `seed` is the pass's salted noise stream.  Returns
+        dout (R,S,4) = [dL/d rgb logits, dL/d raw sigma]."""
+        q, tt = _f32c(raw, self.device), _f32c(t, self.device)
+        d, g = _f32c(dirs, self.device), _f32c(d_rgb, self.device)
+        R, S = tt.shape
+        assert q.shape == (R, S, 4) and d.shape == (R, 3) and g.shape == (R, 3), (q.shape, tt.shape, d.shape, g.shape)
+        out = torch.empty((R, S, 4), dtype=torch.float32, device=self.device)
+        L.check(self.lib.nm_debug_composite_backward(self._h, _ptr(q), _ptr(tt), _ptr(d), _ptr(g), R, S, float(noise_std),
+                                                     int(seed) % 2 ** 64, int(white_bg), _ptr(out), self._stream()))
+        return out
+
     def render_image(self, pose, H, W, focal, near, far, *, ndc=False, rows=None, training=False, buff=False, seed=0,
                      want=None, to_host=False, host_out=None, out=None) -> Dict[str, torch.Tensor]:
         """Rays generated on the device from a 3x4 / 4x4 camera-to-world pose (get_ray_bundle [+ ndc_rays])."""

@@ -252,14 +252,15 @@ class Bundle:
 
 def volume_render(raw: torch.Tensor, t: torch.Tensor, ray_directions: torch.Tensor, *, noise_std=0.0,
                   white_background=False, training=False, attenuation_threshold=1e-5,
-                  generator: Optional[torch.Generator] = None) -> Bundle:
-    """src/nerf/modules.py:67-121 (threshold 1e-5 from src/models/model_base.py:28-33)."""
+                  generator: Optional[torch.Generator] = None, noise: Optional[torch.Tensor] = None) -> Bundle:
+    """src/nerf/modules.py:67-121 (threshold 1e-5 from src/models/model_base.py:28-33).  `noise` (shape of raw[..., 3]),
+    if given, is the sigma noise itself (already scaled), added instead of noise_std * randn: lets a test feed the
+    noise stream of another implementation."""
     big = torch.tensor([1e10]).expand(t[..., :1].shape)
     dists = torch.cat((t[..., 1:] - t[..., :-1], big), dim=-1) * ray_directions[..., None, :].norm(p=2, dim=-1)
     rgb = raw[..., :3]
-    noise = 0.0
-    if noise_std > 0.0:
-        noise = torch.randn(raw[..., 3].shape, generator=generator) * noise_std
+    if noise is None:
+        noise = torch.randn(raw[..., 3].shape, generator=generator) * noise_std if noise_std > 0.0 else 0.0
     sigma = torch.nn.functional.relu(raw[..., 3] + noise)
     alpha = 1.0 - torch.exp(-sigma * dists)
     trans = cumprod_exclusive(1.0 - alpha + 1e-10)
@@ -426,26 +427,29 @@ class RenderCfg:
 
 
 def nerf_forward(coarse_sd, fine_sd, net_c: NetCfg, net_f: Optional[NetCfg], rcfg: RenderCfg,
-                 ray_origins, ray_directions, near, far, training=False, u=None):
-    """src/models/model_nerf.py:37-78.  Returns (coarse Bundle, fine Bundle or None, t_coarse, t_fine)."""
+                 ray_origins, ray_directions, near, far, training=False, u=None, noise_c=None, noise_f=None):
+    """src/models/model_nerf.py:37-78.  Returns (coarse Bundle, fine Bundle or None, t_coarse, t_fine).  noise_c / noise_f:
+    explicit sigma noise of the coarse / fine compositor (volume_render's `noise`)."""
     R = ray_directions.shape[0]
     t_c = ray_sample_interval(rcfg.num_coarse, R, near, far, rcfg.lindisp, rcfg.perturb)
     p_c = intervals_to_ray_points(t_c, ray_directions, ray_origins)
     raw_c = flexible_nerf_forward(coarse_sd, net_c, p_c, ray_directions[..., None, :].expand_as(p_c))
     b_c = volume_render(raw_c, t_c, ray_directions, noise_std=rcfg.noise_std, white_background=rcfg.white_background,
-                        training=training, attenuation_threshold=rcfg.attenuation_threshold)
+                        training=training, attenuation_threshold=rcfg.attenuation_threshold, noise=noise_c)
     if fine_sd is None:
         return b_c, None, t_c, None
     t_f = sample_pdf_forward(t_c, b_c.weights, rcfg.num_fine, rcfg.perturb, u=u)
     p_f = intervals_to_ray_points(t_f, ray_directions, ray_origins)
     raw_f = flexible_nerf_forward(fine_sd, net_f, p_f, ray_directions[..., None, :].expand_as(p_f))
     b_f = volume_render(raw_f, t_f, ray_directions, noise_std=rcfg.noise_std, white_background=rcfg.white_background,
-                        training=training, attenuation_threshold=rcfg.attenuation_threshold)
+                        training=training, attenuation_threshold=rcfg.attenuation_threshold, noise=noise_f)
     return b_c, b_f, t_c, t_f
 
 
-def buff_forward(sd, net: NetCfg, rcfg: RenderCfg, voxels, ray_origins, ray_directions, near, far, training=False):
-    """src/models/model_buff.py:34-69 (inference part): uniform fallback samples, AABB samples, overwrite misses."""
+def buff_forward(sd, net: NetCfg, rcfg: RenderCfg, voxels, ray_origins, ray_directions, near, far, training=False,
+                 noise=None):
+    """src/models/model_buff.py:34-69 (inference part): uniform fallback samples, AABB samples, overwrite misses.
+    noise: explicit sigma noise (volume_render's `noise`)."""
     R = ray_directions.shape[0]
     t_u = ray_sample_interval(rcfg.num_coarse, R, near, far, rcfg.lindisp, rcfg.perturb)
     z, mask = batch_ray_voxel_intersect(voxels, ray_origins, ray_directions, near, far, rcfg.num_coarse)
@@ -453,7 +457,7 @@ def buff_forward(sd, net: NetCfg, rcfg: RenderCfg, voxels, ray_origins, ray_dire
     p = intervals_to_ray_points(t, ray_directions, ray_origins)
     raw = flexible_nerf_forward(sd, net, p, ray_directions[..., None, :].expand_as(p))
     b = volume_render(raw, t, ray_directions, noise_std=rcfg.noise_std, white_background=rcfg.white_background,
-                      training=training, attenuation_threshold=rcfg.attenuation_threshold)
+                      training=training, attenuation_threshold=rcfg.attenuation_threshold, noise=noise)
     return b, t, mask
 
 
