@@ -123,6 +123,14 @@ int nm_set_tree(NmHandle h, const float* voxels_host, int32_t V);
  * pts/dirs (M,3) fp32; out (M,4) = [sigmoid rgb, raw sigma], or (M,) raw sigma when sigma_only. */
 int nm_point_mlp(NmHandle h, int which, const float* pts_dev, const float* dirs_dev, int64_t M, float* out_dev,
                  int sigma_only, void* stream);
+/* d sigma / d p of network `which` at M points (no reference counterpart: analytic normals for the mesh path).  pts (M,3)
+ * fp32; grad (M,3); sigma (M,) raw density or NULL (then bit for bit nm_point_mlp's sigma_only output).  Handle precision
+ * selects tensor cores (exact / fast) or fp32.  Deterministic, independent of batch composition; leaves the gradient
+ * buffers and every other handle state untouched.  M = 0 launches nothing.  Points are walked in chunks of
+ * NM_SIGMA_GRAD_CHUNK_POINTS (default 256 Ki) in a workspace of the handle: it grows to one chunk's size (~22 KB per point
+ * for the 8x256 network, ~5.8 GB at the default) and is held until nm_destroy; a smaller chunk bounds it. */
+int nm_sigma_grad(NmHandle h, int which, const float* pts_dev, int64_t M, float* sigma_dev_or_null, float* grad_dev,
+                  void* stream);
 /* NeRFModel.forward / BuFFModel.forward (src/models/model_nerf.py:37-78, model_buff.py:34-69).
  * origins: o_stride = 0 -> one shared (3,) origin, 3 -> per-ray (R,3).  near/far: nf_stride = 0 -> 2 scalars in
  * near_far_host[0..1]; 1 -> per-ray near (R,) and far (R,) device arrays in near_dev / far_dev. */

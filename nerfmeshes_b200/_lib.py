@@ -47,6 +47,7 @@ _SIGNATURES = {
     "nm_set_tables": (C.c_int, [_P, _P, _P]),
     "nm_set_tree": (C.c_int, [_P, _P, C.c_int32]),
     "nm_point_mlp": (C.c_int, [_P, _I, _P, _P, _L, _P, _I, _P]),
+    "nm_sigma_grad": (C.c_int, [_P, _I, _P, _L, _P, _P, _P]),
     "nm_render_rays": (C.c_int, [_P, _P, _I, _P, _L, _P, _P, _P, _I, C.c_uint64, C.POINTER(NmRenderOut), _P]),
     "nm_render_image": (C.c_int, [_P, _P, _I, _I, _F, _I, _I, _I, _P, _I, C.c_uint64, C.POINTER(NmRenderOut), _P]),
     "nm_ray_bundle": (C.c_int, [_P, _P, _I, _I, _F, _I, _F, _I, _I, _P, _P, _P]),

@@ -67,6 +67,8 @@ struct NmHandle_t {
   int64_t mc_counts[2] = {0, 0};   // {vertices, triangles} of the last count step: sizes of the emit step
   Buf ss_tab, ss_ws;               // super-sampled emit: the six coordinate tables; chunk points (M,3) + sigma (M,)
   Buf ms_ws, nn_ws;                // chamfer evaluation: surface sampler (areas, cdf); grid nearest-neighbour search
+  Buf sg_ws;                       // density gradient (nm_sigma_grad): one chunk's forward / chain / tail workspace; grow-only,
+                                   // held until nm_destroy (~22 KB per chunk point for the 8x256 network, ~5.8 GB at the default)
   // training (nm_train.cu): gradient accumulators per network + scratch
   Buf g_wt[2], g_bias[2], g_head[2], train_ws, dout, trans, tr_rgb[2], tr_drgb[2];
   bool grads_ready = false;
@@ -80,6 +82,14 @@ long long ss_chunk_points() {
   const char* e = getenv("NM_SS_CHUNK_POINTS");
   const long long x = e ? atoll(e) : 0;
   return x > 0 ? x : (1ll << 22);
+}
+
+// points per chunk of the density gradient (~22 KB of workspace each for the 8x256 network: ~5.8 GB at 256 Ki);
+// NM_SIGMA_GRAD_CHUNK_POINTS overrides it, read per call (the tests cross chunk boundaries with small values)
+long long sigma_grad_chunk_points() {
+  const char* e = getenv("NM_SIGMA_GRAD_CHUNK_POINTS");
+  const long long x = e ? atoll(e) : 0;
+  return x > 0 ? x : (1ll << 18);
 }
 
 // rays per internal chunk (bounds the per-sample workspace: 20 B x 192 samples x 1 Mi rays = 4 GB); NM_CHUNK_RAYS overrides (tests)
@@ -489,7 +499,7 @@ int nm_destroy(NmHandle h) {
   for (Buf& b : h->stage_out) b.release();
   for (int i = 0; i < 2; ++i) { h->g_wt[i].release(); h->g_bias[i].release(); h->g_head[i].release(); h->tr_rgb[i].release(); h->tr_drgb[i].release(); }
   h->train_ws.release(); h->dout.release(); h->trans.release();
-  h->ss_tab.release(); h->ss_ws.release(); h->ms_ws.release(); h->nn_ws.release();
+  h->ss_tab.release(); h->ss_ws.release(); h->ms_ws.release(); h->nn_ws.release(); h->sg_ws.release();
   if (h->mc_ws_ptr) cudaFree(h->mc_ws_ptr);
   if (h->mc_ws2_ptr) cudaFree(h->mc_ws2_ptr);
   if (h->h_err) cudaFreeHost(h->h_err);
@@ -859,6 +869,39 @@ int nm_mc_emit_ss(NmHandle h, const float* vol_dev, int nb, int ny, int nz, floa
   }
   return mc_emit_ss(sh, h->mc_ws_ptr, h->mc_ws_bytes, &h->mc_ws2_ptr, &h->mc_ws2_bytes, v_base, nv, nt, ss, verts_dev,
                     normals_dev, faces_dev, st, &h->launches);
+}
+
+// ---------------------------------------------------------------------------------------------- density gradient
+// Argument checks come before the handle is touched, so a bad call is rejected without a device.  The gradient buffers and
+// the training workspace are not used: the chain runs in a workspace of its own, chunk by chunk.
+int nm_sigma_grad(NmHandle h, int which, const float* pts_dev, int64_t M, float* sigma_dev_or_null, float* grad_dev,
+                  void* stream) {
+  NM_CHECK(pts_dev && grad_dev, "density gradient: null point or gradient pointer");
+  NM_CHECK(M >= 0, "density gradient: negative point count %lld", (long long)M);
+  NM_CHECK(h != nullptr, "null handle");
+  NM_CHECK(which == NM_NET_COARSE || (which == NM_NET_FINE && h->has_fine), "network slot %d not present", which);
+  if (M == 0) return 0;
+  if (int e = bind_checked(h)) return e;
+  NetDev& net = h->nets[which];
+  NM_CHECK(net.loaded, "weights of network %d not loaded", which);
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool use_tc = h->cfg.precision != NM_PREC_FP32;
+  const TrainMode mode{use_tc ? 1 : 0, h->cfg.precision == NM_PREC_FAST ? 1 : 3, h->d_err};
+  const long long chunk = sigma_grad_chunk_points();
+  const long long P = M < chunk ? M : chunk;
+  // the chunk workspace is held by the handle like the training workspace: allocating and freeing it per call (stream-ordered)
+  // took the 512^3 normal pass from 82 ms to 169 ms on an H100 (DESIGN 4.8)
+  if (int e = h->sg_ws.ensure(sigma_grad_ws_bytes(net.full, P, use_tc) + 1024)) return e;
+  float* ws = reinterpret_cast<float*>(((uintptr_t)h->sg_ws.p + 1023) & ~(uintptr_t)1023);
+  for (long long m0 = 0; m0 < M; m0 += chunk) {
+    const long long n = M - m0 < chunk ? M - m0 : chunk;
+    if (int e = sigma_grad(net, pts_dev + 3 * m0, n, ws, grad_dev + 3 * m0, h->num_sms, mode, st, &h->launches)) return e;
+  }
+  if (!sigma_dev_or_null) return 0;
+  // sigma: the sigma-only forward of nm_point_mlp, so that it is that call's value bit for bit
+  MlpInput in{};
+  in.mode = IN_POINTS; in.pts = pts_dev; in.dirs = nullptr; in.M = M;
+  return run_mlp(h, which, true, in, sigma_dev_or_null, st);
 }
 
 // ---------------------------------------------------------------------------------------------- chamfer evaluation

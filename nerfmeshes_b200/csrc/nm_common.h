@@ -183,6 +183,33 @@ int launch_composite_backward(const float* raw, const float* t, const float* dir
                               cudaStream_t st, int64_t* launches);
 int launch_mse_grad(const float* rgb, const float* target, long long n, long long count, float* d_rgb, float* loss,
                     cudaStream_t st, int64_t* launches);
+// density gradient g = d raw sigma / d p (nm_sigma_grad.cu, orchestrated by sigma_grad in nm_train.cu; DESIGN 4.8)
+struct PeDesc { int L, inc; float freq[kMaxFreq]; };     // the xyz encoding
+constexpr int kSgMaxKb = 64;                             // 64-feature K-blocks of the xyz-reading layers
+struct SigmaGradWeights {
+  const float* wt[kSgMaxKb];    // per K-block: &Wt[k_act][64 kb'] of its layer; element (column j, feature kk) at wt[j * ld + kk]
+  int ld[kSgMaxKb];             // the layer's n_out
+  int k_pe;
+  uint8_t* out;                 // n_kb x 16 KB of packed B tiles
+};
+struct SigmaGradTail {
+  const uint8_t* a[kSgMaxKb];   // per K-block: the 64-feature group of its layer's dZ pack at point block 0 (point block b: + b ptiles)
+  const uint8_t* b;             // SigmaGradWeights.out
+  int n_kb, n_passes;
+  long long M;
+  const float* pts;             // (M,3)
+  PeDesc pe;
+  float* grad;                  // (M,3)
+  int* err;
+};
+int launch_sigma_grad_tail(const SigmaGradWeights& W, const SigmaGradTail& T, int num_sms, cudaStream_t st, int64_t* launches);
+int launch_pe_vjp(const float* pts, long long M, const float* dpe, int ld, const PeDesc& pe, float* grad, cudaStream_t st,
+                  int64_t* launches);
+// g of network `net` at M points (one chunk); ws: sigma_grad_ws_bytes(full, M, use_tc) bytes, 1 KB aligned.  Writes nothing
+// but ws and grad.
+size_t sigma_grad_ws_bytes(const NetProgram& full, long long points, bool use_tc);
+int sigma_grad(NetDev& net, const float* pts, long long M, float* ws, float* grad, int num_sms, const TrainMode& mode,
+               cudaStream_t st, int64_t* launches);
 // marching cubes (nm_mc.cu): one shard of a global grid — buffer planes [0,nb) are global planes [g_x0, g_x0+nb) of g_nx;
 // the call owns the points (vertices, cells) of buffer planes [p_lo,p_hi)
 struct McShard {

@@ -59,4 +59,23 @@ __device__ __forceinline__ void positional_encoding(const float x[3], int L, int
   }
 }
 
+// The encoding's vector-Jacobian product: g_c = sum_j adj(j) d enc_j / d x_c in positional_encoding's column order, at the
+// same fp32 argument x_c*f_k and with the same accurate sincosf:  d sin(f x)/dx = f cos(f x),  d cos(f x)/dx = -f sin(f x),
+// the identity block when include_input.  adj(column) returns the adjoint of that encoding column.
+template <class Adj>
+__device__ __forceinline__ void positional_encoding_vjp(const float x[3], int L, int include_input, const float* freq,
+                                                        Adj adj, float g[3]) {
+  const int base = include_input ? 3 : 0;
+  for (int c = 0; c < 3; ++c) {
+    float acc = include_input ? adj(c) : 0.f;
+    for (int k = 0; k < L; ++k) {
+      float s, co;
+      sincosf(__fmul_rn(x[c], freq[k]), &s, &co);
+      const float t = fmaf(adj(base + c * L + k), co, -adj(base + 3 * L + c * L + k) * s);
+      acc = fmaf(freq[k], t, acc);
+    }
+    g[c] = acc;
+  }
+}
+
 }  // namespace nm

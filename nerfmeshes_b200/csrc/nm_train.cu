@@ -576,6 +576,20 @@ __global__ void mse_grad_kernel(const float* __restrict__ rgb, const float* __re
   if (threadIdx.x == 0 && loss) atomicAdd(loss, red[0]);
 }
 
+// Seed of the density-gradient chain (nm_sigma_grad): dout = (0, 0, 0, 1) per point (d raw sigma = 1) and dZ (P,N) of the
+// last layer = relu'(act) * w_sigma when that layer's head carries sigma (fc_out row 3, w_sigma != nullptr), else 0 (the
+// colour head: d rgb = 0; sigma enters the chain at the fc_alpha layer through dout).
+__global__ void sigma_seed_kernel(long long P, int N, const float* __restrict__ act, const float* __restrict__ w_sigma,
+                                  int relu, float* __restrict__ dout, float* __restrict__ dZ) {
+  const long long n = P * N;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const long long p = i / N;
+    const int k = (int)(i - p * N);
+    if (k == 0) reinterpret_cast<float4*>(dout)[p] = make_float4(0.f, 0.f, 0.f, 1.f);
+    dZ[i] = (w_sigma && !(relu && !(act[i] > 0.f))) ? w_sigma[k] : 0.f;
+  }
+}
+
 }  // namespace
 
 
@@ -740,18 +754,15 @@ int backward_tc(NetDev& net, const MlpInput& in, const float* dout, float* ws_ba
   return 0;
 }
 
-// NM_PREC_FP32: forward recompute act[l] = act_l([act[l-1] | PE] W^T + b) and the backward layer by layer, every GEMM in
-// fp32 FMAs on the CUDA cores.
-int backward_fp32(NetDev& net, const MlpInput& in, const float* dout, float* ws_base, NetGrads* g, int num_sms,
-                  cudaStream_t st, int64_t* launches) {
+// NM_PREC_FP32 forward recompute: the encodings, then act[l] = act_l([act[l-1] | PE] W^T + b) layer by layer in fp32 FMAs
+// on the CUDA cores.
+int forward_fp32(NetDev& net, const MlpInput& in, const TrainWs& W, cudaStream_t st, int64_t* launches) {
   const NetProgram& G = net.full;
   const int P = (int)in.M;
-  const TrainWs W = carve(G, P, false, reinterpret_cast<uint8_t*>(ws_base));
   encode_kernel<<<(P + 127) / 128, 128, 0, st>>>(in, net.d_full, W.pe_x, W.pe_d);
   NM_CUDA(cudaGetLastError());
   if (launches) ++*launches;
   auto pe_of = [&](const LayerProg& L) { return L.pe_src == SRC_PE_XYZ ? W.pe_x : W.pe_d; };
-
   for (int l = 0; l < G.n_layers; ++l) {
     const LayerProg& L = G.layers[l];
     const int N = L.n_out;
@@ -767,6 +778,17 @@ int backward_fp32(NetDev& net, const MlpInput& in, const float* dout, float* ws_
       if (int rc = sgemm<false>(pe_of(L), kPeLd, Wt + (size_t)L.k_act * N, N, W.act[l], N, P, N, L.k_pe, fin, st, launches)) return rc;
     }
   }
+  return 0;
+}
+
+// NM_PREC_FP32: forward recompute and the backward layer by layer, every GEMM in fp32 FMAs on the CUDA cores.
+int backward_fp32(NetDev& net, const MlpInput& in, const float* dout, float* ws_base, NetGrads* g, int num_sms,
+                  cudaStream_t st, int64_t* launches) {
+  const NetProgram& G = net.full;
+  const int P = (int)in.M;
+  const TrainWs W = carve(G, P, false, reinterpret_cast<uint8_t*>(ws_base));
+  auto pe_of = [&](const LayerProg& L) { return L.pe_src == SRC_PE_XYZ ? W.pe_x : W.pe_d; };
+  if (int rc = forward_fp32(net, in, W, st, launches)) return rc;
 
   size_t gw_off[kMaxLayers];
   int gw_ld[kMaxLayers];
@@ -835,6 +857,143 @@ int mlp_backward(NetDev& net, const MlpInput& in, const float* dout, float* ws_b
   if (in.M <= 0) return 0;
   if (mode.use_tc) return backward_tc(net, in, dout, ws_base, g, num_sms, mode, st, launches, have_acts);
   return backward_fp32(net, in, dout, ws_base, g, num_sms, st, launches);
+}
+
+// ------------------------------------------------------------------------------------------------ density gradient
+// g = d raw sigma / d p (DESIGN 4.8): the training backward's data-gradient chain seeded with d raw sigma = 1 and no
+// weight- or head-gradient work, then the input tail dPE = sum dZ_l W_l[:, PE] over the xyz-reading layers and the encoding
+// Jacobian.  Workspace: the backward's carving for P points, dout (P,4), then the packed B tiles (tensor cores) or the
+// fp32 dPE (P, kPeLd).
+namespace {
+
+int sigma_xyz_kblocks(const NetProgram& G) {
+  int n = 0;
+  for (int l = 0; l < G.n_layers; ++l)
+    if (G.layers[l].pe_src == SRC_PE_XYZ) n += G.layers[l].n_out / 64;
+  return n;
+}
+
+int launch_sigma_seed(const NetDev& net, const TrainWs& W, long long P, float* dout, cudaStream_t st, int64_t* launches) {
+  const NetProgram& G = net.full;
+  const int last = G.n_layers - 1;
+  const LayerProg& Ltop = G.layers[last];
+  NM_CHECK(Ltop.kind == KIND_RGB || Ltop.kind == KIND_OUT4, "the last layer must carry the colour head");
+  const float* w_sigma = Ltop.kind == KIND_OUT4 ? net.d_head + Ltop.head_off + 3 * Ltop.n_out : nullptr;
+  const long long n = P * Ltop.n_out;
+  const long long blocks = (n + 255) / 256 < 4096 ? (n + 255) / 256 : 4096;
+  sigma_seed_kernel<<<(unsigned)blocks, 256, 0, st>>>(P, Ltop.n_out, W.act[last], w_sigma, Ltop.relu, dout, W.dbuf[0]);
+  NM_CUDA(cudaGetLastError());
+  if (launches) ++*launches;
+  return 0;
+}
+
+PeDesc pe_desc(const NetProgram& G) {
+  PeDesc d{};
+  d.L = G.L_xyz; d.inc = G.inc_xyz;
+  for (int k = 0; k < kMaxFreq; ++k) d.freq[k] = G.freq_xyz[k];
+  return d;
+}
+
+// Tensor cores: mode-1 forward (relu masks, activation packs), the mode-2 chain (dZ packs of every layer), the wgmma tail.
+int sigma_grad_tc(NetDev& net, const MlpInput& in, uint8_t* ws, float* grad, int num_sms, const TrainMode& mode,
+                  cudaStream_t st, int64_t* launches) {
+  const NetProgram& G = net.full;
+  const int P = (int)in.M;
+  const TrainWs W = carve(G, P, true, ws);
+  float* dout = reinterpret_cast<float*>(ws + W.bytes);
+  uint8_t* bpack = ws + W.bytes + up((size_t)P * 16);
+  const int kbtP = 2 * ((P + 127) / 128);
+  MlpEmit E{};
+  train_emit_setup(G, P, reinterpret_cast<float*>(ws), &E);
+  if (int e = launch_mlp_tc(net, false, mode.n_passes, 0, in, nullptr, num_sms, mode.d_err, st, launches, &E)) return e;
+  if (!net.bwd_valid)
+    if (int e = build_backward_stream(&net, st, launches)) return e;
+  if (int e = launch_sigma_seed(net, W, P, dout, st, launches)) return e;
+  const int last = G.n_layers - 1;
+  MlpEmit io{};
+  io.kbt = kbtP;
+  io.packT[0] = W.pkt_dz[last];
+  for (int li = 1; li < net.bwd.n_layers; ++li) {
+    const int l = net.bwd.layers[li].aux;
+    io.packT[li] = W.pkt_dz[l - 1];
+    if (G.layers[l - 1].relu) io.bits[li] = reinterpret_cast<uint32_t*>(W.bits[l - 1]);
+  }
+  if (int e = launch_mlp_tc_bwd(net, P, W.dbuf[0], G.layers[last].n_out, dout, io, mode.n_passes, num_sms, mode.d_err, st, launches))
+    return e;
+  // the tail's K-blocks: every 64-feature group of every xyz-reading layer, layers in forward order
+  SigmaGradWeights Wb{};
+  SigmaGradTail T{};
+  int kb = 0;
+  for (int l = 0; l < G.n_layers; ++l) {
+    const LayerProg& L = G.layers[l];
+    if (L.pe_src != SRC_PE_XYZ) continue;
+    NM_CHECK(L.k_pe == G.dim_xyz && L.n_out % 64 == 0, "layer %d: unexpected xyz encoding block", l);
+    for (int fg = 0; fg < L.n_out / 64; ++fg, ++kb) {
+      NM_CHECK(kb < kSgMaxKb, "density gradient: more than %d K-blocks", kSgMaxKb);
+      T.a[kb] = W.pkt_dz[l] + (size_t)(fg >> 1) * kbtP * kPtileBytes + (size_t)(fg & 1) * 8192u;
+      Wb.wt[kb] = net.d_wt + L.wt_off + (size_t)L.k_act * L.n_out + fg * 64;
+      Wb.ld[kb] = L.n_out;
+    }
+  }
+  Wb.k_pe = G.dim_xyz; Wb.out = bpack;
+  T.b = bpack; T.n_kb = kb; T.n_passes = mode.n_passes; T.M = P; T.pts = in.pts; T.pe = pe_desc(G); T.grad = grad;
+  T.err = mode.d_err;
+  return launch_sigma_grad_tail(Wb, T, num_sms, st, launches);
+}
+
+// NM_PREC_FP32: the SIMT recompute, the data-gradient half of backward_fp32's layer loop with dPE taken (sgemm) from the dZ of
+// every xyz-reading layer as the walk passes it, then the same Jacobian contraction.
+int sigma_grad_fp32(NetDev& net, const MlpInput& in, uint8_t* ws, float* grad, cudaStream_t st, int64_t* launches) {
+  const NetProgram& G = net.full;
+  const int P = (int)in.M;
+  const TrainWs W = carve(G, P, false, ws);
+  float* dout = reinterpret_cast<float*>(ws + W.bytes);
+  float* dpe = reinterpret_cast<float*>(ws + W.bytes + up((size_t)P * 16));
+  if (int rc = forward_fp32(net, in, W, st, launches)) return rc;
+  if (int rc = launch_sigma_seed(net, W, P, dout, st, launches)) return rc;
+  int cur = 0;
+  bool first = true;
+  for (int l = G.n_layers - 1; l >= 0; --l) {
+    const LayerProg& L = G.layers[l];
+    const int N = L.n_out;
+    float* dZ = W.dbuf[cur];
+    if (L.pe_src == SRC_PE_XYZ) {       // dPE (+)= dZ_l W_l[:, k_act, k_act + k_pe)
+      GemmEpi e{};
+      e.accumulate = first ? 0 : 1;
+      if (int rc = sgemm<true>(dZ, N, net.d_wt + L.wt_off + (size_t)L.k_act * N, N, dpe, kPeLd, P, L.k_pe, N, e, st, launches)) return rc;
+      first = false;
+    }
+    if (l > 0) {                        // dZ of layer l-1, as backward_fp32
+      const LayerProg& Lp = G.layers[l - 1];
+      NM_CHECK(L.k_act == Lp.n_out, "layer chain mismatch");
+      GemmEpi e{};
+      if (Lp.kind == KIND_SIGMA) { e.r1_vec = dout + 3; e.r1_stride = 4; e.r1_w = net.d_head + Lp.head_off; }
+      if (Lp.relu) { e.mask = W.act[l - 1]; e.ldmask = Lp.n_out; }
+      if (int rc = sgemm<true>(dZ, N, net.d_wt + L.wt_off, N, W.dbuf[cur ^ 1], L.k_act, P, L.k_act, N, e, st, launches)) return rc;
+      cur ^= 1;
+    }
+  }
+  NM_CHECK(!first, "no layer reads the xyz encoding");
+  return launch_pe_vjp(in.pts, P, dpe, kPeLd, pe_desc(G), grad, st, launches);
+}
+
+}  // namespace
+
+size_t sigma_grad_ws_bytes(const NetProgram& G, long long points, bool use_tc) {
+  const size_t tail = use_tc ? (size_t)sigma_xyz_kblocks(G) * 16384 : (size_t)points * kPeLd * 4;
+  return carve(G, points, use_tc, nullptr).bytes + up((size_t)points * 16) + up(tail);
+}
+
+int sigma_grad(NetDev& net, const float* pts, long long M, float* ws, float* grad, int num_sms, const TrainMode& mode,
+               cudaStream_t st, int64_t* launches) {
+  if (M <= 0) return 0;
+  NM_CHECK(M <= INT32_MAX, "density gradient: chunk of %lld points", M);
+  NM_CHECK(net.full.dim_xyz <= kPeLd, "encoding wider than %d", kPeLd);
+  MlpInput in{};
+  in.mode = IN_POINTS; in.pts = pts; in.dirs = nullptr; in.M = M;     // directions = positions, as in the grid sweep
+  uint8_t* base = reinterpret_cast<uint8_t*>(ws);
+  if (mode.use_tc) return sigma_grad_tc(net, in, base, grad, num_sms, mode, st, launches);
+  return sigma_grad_fp32(net, in, base, grad, st, launches);
 }
 
 }  // namespace nm

@@ -151,6 +151,18 @@ class Engine:
             L.check(self.lib.nm_point_mlp(self._h, which, _ptr(p), _ptr(d), M, _ptr(out), int(sigma_only), self._stream()))
         return out.reshape(*lead, *(() if sigma_only else (4,)))
 
+    def sigma_grad(self, which: int, pts: torch.Tensor, want_sigma=True):
+        """d raw sigma / d p of network `which` at pts (...,3) (nm_sigma_grad): (sigma (...) or None, grad (...,3)) device
+        tensors.  The network's analytic density gradient in the handle's precision, independent of batch composition."""
+        lead = pts.shape[:-1]
+        p = _f32c(pts, self.device).reshape(-1, 3)
+        M = p.shape[0]
+        grad = torch.empty((M, 3), dtype=torch.float32, device=self.device)
+        sigma = torch.empty((M,), dtype=torch.float32, device=self.device) if want_sigma else None
+        if M:
+            L.check(self.lib.nm_sigma_grad(self._h, which, _ptr(p), M, _ptr(sigma), _ptr(grad), self._stream()))
+        return (None if sigma is None else sigma.reshape(lead)), grad.reshape(*lead, 3)
+
     def num_samples(self, buff=False):
         s = self.settings
         return s.num_coarse + (s.num_fine if (self.has_fine and not buff) else 0)

@@ -57,10 +57,51 @@ def super_sampling_tables(limit, nums, s):
     return lins, fines
 
 
+def sweep_coordinates(verts, lins):
+    """Marching-cubes vertices in index coordinates (V,3) -> the sweep's coordinates: per axis the torch.linspace table
+    `lins[a]` interpolated at the index coordinate, so that an integer index gives the table's value bit for bit (the grid
+    point the sweep sampled).  Not the exported coordinates, whose limit*(v/(res/2) - 1) scale drifts from linspace."""
+    out = []
+    for a in range(3):
+        lin = lins[a].to(verts.device, torch.float32)
+        v = verts[:, a]
+        n = lin.shape[0]
+        i0 = torch.floor(v).clamp(0, n - 1)
+        frac = v - i0
+        i0 = i0.long()
+        i1 = (i0 + 1).clamp(max=n - 1)
+        x0 = lin[i0]
+        out.append(torch.where(frac == 0, x0, x0 + frac * (lin[i1] - x0)))
+    return torch.stack(out, 1).contiguous()
+
+
+def network_normals(eng, which, verts, lins, grid_normals):
+    """n = -g / |g| with g the network's density gradient (nm_sigma_grad) at each vertex's sweep coordinates — the grid
+    normals' convention, pointing towards decreasing sigma.  Where |g| is 0 or not finite the grid normal is kept.
+    Returns (normals (V,3), number of vertices that kept their grid normal)."""
+    if verts.shape[0] == 0:
+        return grid_normals, 0
+    _, g = eng.sigma_grad(which, sweep_coordinates(verts, lins), want_sigma=False)
+    gn = grid_normals.to(g.device)
+    norm = torch.sqrt(g[:, 0] * g[:, 0] + g[:, 1] * g[:, 1] + g[:, 2] * g[:, 2])
+    ok = torch.isfinite(norm) & (norm > 0)
+    n = torch.where(ok[:, None], -g / torch.where(ok, norm, torch.ones_like(norm))[:, None], gn)
+    return n, int((~ok).sum())
+
+
+def _report_fallback(n_fallback, n_vertices):
+    if n_fallback:
+        print(f"network normals: {n_fallback} of {n_vertices} vertices have a zero or non-finite density gradient "
+              "and keep their grid normal")
+
+
 def extract_geometry(model, device, args):
     """src/mesh_nerf.py:68-92: sigma sweep -> adaptive iso -> marching cubes -> rescale to (-limit, limit).
     With args.super_sampling = s >= 1 (mesh_nerf.py:95-128) the coarse grid's mesh keeps its topology, faces and normals,
-    and each edge vertex is placed from s extra network samples along its edge (nm_mc_emit_ss, DESIGN 4.3)."""
+    and each edge vertex is placed from s extra network samples along its edge (nm_mc_emit_ss, DESIGN 4.3).
+    With args.network_normals the normals are the network's analytic density gradient at the vertices (network_normals,
+    DESIGN 4.8) instead of central differences of the sigma grid; vertices and faces are unchanged.  Measured on lego, they
+    are better than grid normals with super_sampling >= 1 (vertices on the network's surface) but not at s = 0."""
     eng = model._engine()
     density = extract_radiance(model, args, device, args.res, sigma_only=True)
     iso_value = extract_iso_level(density, args, eng)
@@ -72,6 +113,10 @@ def extract_geometry(model, device, args):
         lins, fines = super_sampling_tables(args.limit, tuple(density.shape), s)
         nv, nt = eng.mc_count(density, float(iso_value), 0, n0, 0, n0)
         verts, faces, normals = eng.mc_emit_ss(density, float(iso_value), 0, n0, 0, n0, nv, nt, 0, s, lins, fines)
+    if getattr(args, "network_normals", False):
+        lins = [torch.linspace(-args.limit, args.limit, n) for n in density.shape]
+        normals, fb = network_normals(eng, model.get_model()._owner[1], verts, lins, normals)
+        _report_fallback(fb, verts.shape[0])
     # the reference rescales CPU tensors (:82-90); do the same on the host so the rounding is identical (torch's CUDA
     # division by a python scalar multiplies by the reciprocal, which differs in the last bit)
     vertices = args.limit * (verts.cpu() / (args.res / 2.0) - 1.0)    # keeps the reference's res/2 scale (:90)

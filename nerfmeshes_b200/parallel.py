@@ -250,7 +250,8 @@ def extract_geometry_sharded(model, args, group=None, to_host=True, timings=None
     A vertex belongs to the rank that owns its grid point, and the last owned cell layer addresses the next rank's
     vertices by the ids that rank assigns (nm_mc_count / nm_mc_emit), so the concatenation IS the single-GPU mesh — same
     arrays, bit for bit; there are no duplicates to remove.  args.super_sampling = s >= 1 emits through nm_mc_emit_ss
-    (super-sampled edge vertices, the same arrays as single-GPU extract_geometry with that s).  Returns (vertices, triangles, normals, iso) like the single-GPU
+    (super-sampled edge vertices, the same arrays as single-GPU extract_geometry with that s); args.network_normals
+    replaces each rank's own normals by the network's density gradient before the gather (mesh.network_normals).  Returns (vertices, triangles, normals, iso) like the single-GPU
     function (vertices rescaled to (-limit, limit) when to_host).  Works without a process group (one slab)."""
     import numpy as np
     rank, world = _rank_world(group)
@@ -294,6 +295,9 @@ def extract_geometry_sharded(model, args, group=None, to_host=True, timings=None
     shard = (iso, buf0, res, own0 - buf0, own1 - buf0)
     nv, nt = eng.mc_count(buf, *shard)
     s = int(getattr(args, "super_sampling", 0) or 0)
+    net_normals = bool(getattr(args, "network_normals", False))
+    if net_normals:
+        from .mesh import network_normals, _report_fallback
     if s:          # super-sampled vertices: the network is evaluated at the edge samples directly, no extra halo planes
         from .mesh import super_sampling_tables
         lins, fines = super_sampling_tables(args.limit, res, s)
@@ -304,6 +308,9 @@ def extract_geometry_sharded(model, args, group=None, to_host=True, timings=None
         outs = (_scratch("v", 3 * nv, torch.float32, dev).view(nv, 3), _scratch("n", 3 * nv, torch.float32, dev).view(nv, 3),
                 _scratch("f", 3 * nt, torch.int32, dev).view(nt, 3))
         v, f, n = emit(buf, *shard, nv, nt, 0, out=outs)
+        if net_normals:
+            n, fb = network_normals(eng, model.get_model()._owner[1], v, tiles, n)
+            _report_fallback(fb, nv)
         tm.mark("mc")
         tm.mark("gather")
     else:
@@ -321,6 +328,10 @@ def extract_geometry_sharded(model, args, group=None, to_host=True, timings=None
         full = _scratch("full", world * seg, torch.float32, dev)
         views = (local[:3 * vmax].view(vmax, 3), local[3 * vmax:6 * vmax].view(vmax, 3), local[6 * vmax:].view(torch.int32).view(tmax, 3))
         emit(buf, *shard, nv, nt, v_base, out=views)
+        if net_normals and nv:     # this rank's own vertices, before the gather: a vertex's normal depends on it alone
+            nn, fb = network_normals(eng, model.get_model()._owner[1], views[0][:nv], tiles, views[1][:nv])
+            views[1][:nv].copy_(nn)
+            _report_fallback(fb, nv)
         tm.mark("mc")
         dist.all_gather_into_tensor(full, local, group=group)
         full = full.view(world, seg)
