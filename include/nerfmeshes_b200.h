@@ -225,6 +225,18 @@ int nm_chamfer(NmHandle h, const float* x_dev, int64_t N, const float* y_dev, in
 int nm_debug_nearest_brute(NmHandle h, const float* q_dev, int64_t N, const float* p_dev, int64_t M, float* dist2_dev,
                            int32_t* idx_dev_or_null, void* stream);
 
+/* Small-component removal on an indexed mesh (no reference counterpart; DESIGN §4.9).  Components are the connected
+ * components of the vertex graph spanned by the faces; a component's id is its smallest vertex index; its size is its
+ * number of faces.  Keeps the vertices and faces of components with >= min_faces faces, in their original order, faces
+ * re-indexed.  Outputs are caller-allocated with room for V vertices / F faces; labels_out (V,) int32 (the component id of
+ * every INPUT vertex) may be NULL.  counts_host = {kept vertices, kept faces, components with >= 1 face, kept components};
+ * synchronises.  Deterministic: the same bits on every run.  Argument errors (null pointers, negative sizes or min_faces,
+ * sizes >= 2^31) are rejected before anything is launched; V = F = 0 launches nothing.  A face index outside [0,V) is
+ * reported through the device-side error word (nm_check_flags raises it, once) and that face is dropped. */
+int nm_mesh_components(NmHandle h, const float* verts_dev, const float* normals_dev, int64_t V, const int32_t* faces_dev,
+                       int64_t F, int64_t min_faces, float* verts_out_dev, float* normals_out_dev, int32_t* faces_out_dev,
+                       int32_t* labels_out_dev_or_null, int64_t* counts_host, void* stream);
+
 /* Replaces export_obj (src/nerf/nerf_helpers.py:86-111): `v x y z [r g b]`, `vn x y z`, `f i//i j//j k//k` (1-based) with
  * byte-identical number formatting (python repr of the float32 widened to double).  Host arrays, no GPU involved;
  * diffuse may be NULL or shorter than the vertex list (vertices beyond it get no colour, like the reference's

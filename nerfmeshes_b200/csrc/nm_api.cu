@@ -48,8 +48,9 @@ struct NmHandle_t {
   // workspace
   Buf t_c, raw_c, w_c, t_f, raw_f, t_u, dirs, origins, lin[3], small, stage_in[3], stage_out[12];
   int lin_n[3] = {0, 0, 0};
-  int* d_err = nullptr;       // [0] tensor-core pipeline watchdog code, [1] aabb hit-list overflow, [2] mesh sampler input
-                              // error (1: face index out of range, 2: total area not positive; cleared when reported)
+  int* d_err = nullptr;       // [0] tensor-core pipeline watchdog code, [1] aabb hit-list overflow, [2] mesh input error
+                              // (mesh sampler 1: face index out of range, 2: total area not positive; component filter
+                              // 3: face index out of range; cleared when reported)
                               // (device alias of h_err)
   int* h_err = nullptr;       // mapped pinned host memory: still readable after a device-side trap
   double* d_stats = nullptr;
@@ -67,6 +68,7 @@ struct NmHandle_t {
   int64_t mc_counts[2] = {0, 0};   // {vertices, triangles} of the last count step: sizes of the emit step
   Buf ss_tab, ss_ws;               // super-sampled emit: the six coordinate tables; chunk points (M,3) + sigma (M,)
   Buf ms_ws, nn_ws;                // chamfer evaluation: surface sampler (areas, cdf); grid nearest-neighbour search
+  Buf cc_ws;                       // small-component removal: labels, sizes, masks and scans (~28 B per vertex + 8 B per face)
   Buf sg_ws;                       // density gradient (nm_sigma_grad): one chunk's forward / chain / tail workspace; grow-only,
                                    // held until nm_destroy (~22 KB per chunk point for the 8x256 network, ~5.8 GB at the default)
   // training (nm_train.cu): gradient accumulators per network + scratch
@@ -133,7 +135,9 @@ int check_kernel_flags(NmHandle h) {
   NM_CHECK(flags[1] == 0, "AABB sampler: more than 512 voxel hits on one ray (samples / voxel indices of that ray are truncated)");
   if (const int c = flags[2]) {     // a bad input mesh, not a broken device: reported once
     h->h_err[2] = 0;
-    NM_CHECK(false, c == 1 ? "mesh sampler: a face index lies outside [0, V)" : "mesh sampler: the total face area is not positive and finite");
+    NM_CHECK(false, c == 1   ? "mesh sampler: a face index lies outside [0, V)"
+                    : c == 2 ? "mesh sampler: the total face area is not positive and finite"
+                             : "mesh components: a face index lies outside [0, V) (the face was dropped)");
   }
   return 0;
 }
@@ -500,6 +504,7 @@ int nm_destroy(NmHandle h) {
   for (int i = 0; i < 2; ++i) { h->g_wt[i].release(); h->g_bias[i].release(); h->g_head[i].release(); h->tr_rgb[i].release(); h->tr_drgb[i].release(); }
   h->train_ws.release(); h->dout.release(); h->trans.release();
   h->ss_tab.release(); h->ss_ws.release(); h->ms_ws.release(); h->nn_ws.release(); h->sg_ws.release();
+  h->cc_ws.release();
   if (h->mc_ws_ptr) cudaFree(h->mc_ws_ptr);
   if (h->mc_ws2_ptr) cudaFree(h->mc_ws2_ptr);
   if (h->h_err) cudaFreeHost(h->h_err);
@@ -955,6 +960,26 @@ int nm_chamfer(NmHandle h, const float* x_dev, int64_t N, const float* y_dev, in
   NM_CHECK(h != nullptr, "null handle");
   if (int e = bind_checked(h)) return e;
   return chamfer(x_dev, N, y_dev, M, means_dev, &h->nn_ws.p, &h->nn_ws.cap, (cudaStream_t)stream, &h->launches);
+}
+
+// ---------------------------------------------------------------------------------------------- small-component removal
+// Argument checks come before the handle is touched, so a bad call is rejected without a device.
+int nm_mesh_components(NmHandle h, const float* verts_dev, const float* normals_dev, int64_t V, const int32_t* faces_dev,
+                       int64_t F, int64_t min_faces, float* verts_out_dev, float* normals_out_dev, int32_t* faces_out_dev,
+                       int32_t* labels_out_dev_or_null, int64_t* counts_host, void* stream) {
+  NM_CHECK(V >= 0 && F >= 0, "mesh components: negative size (V = %lld, F = %lld)", (long long)V, (long long)F);
+  NM_CHECK(min_faces >= 0, "mesh components: negative min_faces %lld", (long long)min_faces);
+  NM_CHECK(V < (1ll << 31) && F < (1ll << 31), "mesh components: sizes must be below 2^31");
+  NM_CHECK(counts_host, "mesh components: null counts pointer");
+  NM_CHECK(V == 0 || (verts_dev && normals_dev && verts_out_dev && normals_out_dev), "mesh components: null vertex pointer");
+  NM_CHECK(F == 0 || (faces_dev && faces_out_dev), "mesh components: null face pointer");
+  NM_CHECK(h != nullptr, "null handle");
+  for (int i = 0; i < 4; ++i) counts_host[i] = 0;
+  if (V == 0 && F == 0) return 0;
+  if (int e = bind_checked(h)) return e;
+  if (int e = h->cc_ws.ensure(components_ws_bytes(V, F))) return e;
+  return mesh_components(verts_dev, normals_dev, V, faces_dev, F, min_faces, verts_out_dev, normals_out_dev, faces_out_dev,
+                         labels_out_dev_or_null, counts_host, h->cc_ws.p, h->d_err + 2, (cudaStream_t)stream, &h->launches);
 }
 
 int nm_marching_cubes_count(NmHandle h, const float* vol_dev, int nx, int ny, int nz, float iso, int64_t* counts_host,

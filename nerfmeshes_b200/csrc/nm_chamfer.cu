@@ -19,7 +19,7 @@ namespace {
 
 constexpr int kBlock = 256;
 constexpr int kRange = 256;          // faces per range of the area scan
-constexpr int kScanBlock = 1024;     // entries per block of the cell-count scan
+constexpr int kScanBlock = kScanBlockEntries;   // entries per block of the cell-count scan (shared: exclusive_scan)
 constexpr int kSumBlocks = 256;      // blocks per array of the chamfer reduction
 
 int grow(void** ptr, size_t* bytes, size_t need) {
@@ -444,14 +444,7 @@ int carve(void** ws, size_t* bytes, long long cap, long long maxM, long long max
   return 0;
 }
 
-int scan_cells(const NnWs& w, const int* cnt, int* start, cudaStream_t st) {
-  const long long nblk = (w.cells + kScanBlock - 1) / kScanBlock;
-  nn_scan_sums<<<(unsigned)nblk, kScanBlock, 0, st>>>(cnt, w.cells, w.blk);
-  nn_scan_blocks<<<1, kScanBlock, 0, st>>>(w.blk, (int)nblk);
-  nn_scan_apply<<<(unsigned)nblk, kScanBlock, 0, st>>>(cnt, w.cells, w.blk, start);
-  NM_CUDA(cudaGetLastError());
-  return 0;
-}
+int scan_cells(const NnWs& w, const int* cnt, int* start, cudaStream_t st) { return exclusive_scan(cnt, w.cells, w.blk, start, st); }
 
 // bounding box of (a, b): the grid every search of one call uses
 int box_of(const NnWs& w, const float* a, long long na, const float* b, long long nb, cudaStream_t st, int64_t* launches) {
@@ -486,6 +479,15 @@ int search(const NnWs& w, const float* q, long long N, const float* p, long long
 }
 
 }  // namespace
+
+int exclusive_scan(const int* cnt, long long n, int* blk, int* start, cudaStream_t st) {
+  const long long nblk = (n + kScanBlock - 1) / kScanBlock;
+  nn_scan_sums<<<(unsigned)nblk, kScanBlock, 0, st>>>(cnt, n, blk);
+  nn_scan_blocks<<<1, kScanBlock, 0, st>>>(blk, (int)nblk);
+  nn_scan_apply<<<(unsigned)nblk, kScanBlock, 0, st>>>(cnt, n, blk, start);
+  NM_CUDA(cudaGetLastError());
+  return 0;
+}
 
 int mesh_sample(const float* verts, long long V, const int32_t* faces, long long F, long long n, uint64_t seed, float* pts,
                 int32_t* face_idx, int* d_err, void** ws, size_t* ws_bytes, cudaStream_t st, int64_t* launches) {

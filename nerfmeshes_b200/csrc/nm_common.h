@@ -240,6 +240,12 @@ int mc_emit_ss(const McShard& s, void* ws, size_t ws_bytes, void** ws2, size_t* 
                int64_t nt, const McSuperSampling& ss, float* verts, float* normals, int32_t* faces, cudaStream_t st,
                int64_t* launches);
 
+// exclusive scan of n >= 1 ints (nm_chamfer.cu: the grid search's cell-count scan, also used by the component filter):
+// start[i] = cnt[0] + ... + cnt[i-1], exact (integers).  blk: (n + kScanBlockEntries - 1) / kScanBlockEntries ints of scratch.
+// Three launches.
+constexpr int kScanBlockEntries = 1024;
+int exclusive_scan(const int* cnt, long long n, int* blk, int* start, cudaStream_t st);
+
 // chamfer evaluation (nm_chamfer.cu).  ws / ws_bytes: a grow-only workspace of the handle.
 // mesh_sample: n area-weighted surface points (face index per point if face_idx != nullptr); a face index outside [0,V)
 // sets *d_err = 1, a total area that is not positive and finite *d_err = 2 (device-side, mapped memory)
@@ -253,5 +259,13 @@ int nearest_brute(const float* q, long long N, const float* p, long long M, floa
 // means[0] = mean_i d2(x_i, Y), means[1] = mean_j d2(y_j, X) (double, fixed summation order)
 int chamfer(const float* x, long long N, const float* y, long long M, double* means, void** ws, size_t* ws_bytes, cudaStream_t st,
             int64_t* launches);
+
+// small-component removal (nm_components.cu, DESIGN §4.9).  ws: components_ws_bytes(V, F) bytes of the handle's grow-only
+// workspace.  A face index outside [0,V) sets *d_err = 3 (device-side, mapped memory); such a face joins nothing and is
+// dropped.  counts_host = {kept vertices, kept faces, components with >= 1 face, kept components}; synchronises.
+size_t components_ws_bytes(long long V, long long F);
+int mesh_components(const float* verts, const float* normals, long long V, const int32_t* faces, long long F, long long min_faces,
+                    float* verts_out, float* normals_out, int32_t* faces_out, int32_t* labels_out, int64_t* counts_host, void* ws,
+                    int* d_err, cudaStream_t st, int64_t* launches);
 
 }  // namespace nm

@@ -533,6 +533,30 @@ class Engine:
         L.check(self.lib.nm_chamfer(self._h, _ptr(x), x.shape[0], _ptr(y), y.shape[0], _ptr(means), self._stream()))
         return means
 
+    # ------------------------------------------------------------------ small-component removal (DESIGN 4.9)
+    def mesh_components(self, verts, normals, faces, min_faces: int, want_labels=False):
+        """Keep the components of the mesh with >= min_faces faces (nm_mesh_components): (verts (v,3), normals (v,3),
+        faces (f,3) int32, counts, labels) with v / f the kept sizes, rows in their original order, faces re-indexed;
+        counts = (kept vertices, kept faces, components with >= 1 face, kept components); labels (V,) int32 = the component
+        id (smallest vertex index) of every input vertex when want_labels, else None.  Synchronises, and raises if a face
+        index lies outside [0, V)."""
+        v = _f32c(verts, self.device).reshape(-1, 3)
+        n = _f32c(normals, self.device).reshape(-1, 3)
+        f = torch.as_tensor(faces).to(self.device, torch.int32).contiguous().reshape(-1, 3)
+        V, F = v.shape[0], f.shape[0]
+        if n.shape[0] != V:
+            raise L.NmError(f"mesh components: {n.shape[0]} normals for {V} vertices")
+        vo, no = torch.empty_like(v), torch.empty_like(n)
+        fo = torch.empty_like(f)
+        labels = torch.empty((V,), dtype=torch.int32, device=self.device) if want_labels else None
+        counts = (C.c_int64 * 4)()
+        p = lambda t: _ptr(t) if t is not None and t.numel() else None
+        L.check(self.lib.nm_mesh_components(self._h, p(v), p(n), V, p(f), F, int(min_faces), p(vo), p(no), p(fo), p(labels),
+                                            counts, self._stream()))
+        self.check_flags()
+        kv, kf = int(counts[0]), int(counts[1])
+        return vo[:kv], no[:kv], fo[:kf], (kv, kf, int(counts[2]), int(counts[3])), labels
+
     # ------------------------------------------------------------------ introspection
     def kernel_flags(self):
         out = (C.c_int32 * 2)()

@@ -95,13 +95,28 @@ def _report_fallback(n_fallback, n_vertices):
               "and keep their grid normal")
 
 
+def remove_small_components(eng, verts, normals, faces, m):
+    """Drop the connected components of the mesh with fewer than m faces (nm_mesh_components, DESIGN 4.9): the floaters of
+    a NeRF mesh.  Kept vertices and faces stay in their original order, faces re-indexed; rows are copied unchanged.  m <= 0
+    returns the inputs as they are.  Prints one line when something was dropped."""
+    if m <= 0:
+        return verts, normals, faces
+    v, n, f, (kv, kf, comps, kept), _ = eng.mesh_components(verts, normals, faces, m)
+    if kv < verts.shape[0] or kf < faces.shape[0]:
+        print(f"small components: kept {kept} of {comps} components, {kf} of {faces.shape[0]} faces "
+              f"(min_component_faces = {m})")
+    return v, n, f
+
+
 def extract_geometry(model, device, args):
     """src/mesh_nerf.py:68-92: sigma sweep -> adaptive iso -> marching cubes -> rescale to (-limit, limit).
     With args.super_sampling = s >= 1 (mesh_nerf.py:95-128) the coarse grid's mesh keeps its topology, faces and normals,
     and each edge vertex is placed from s extra network samples along its edge (nm_mc_emit_ss, DESIGN 4.3).
     With args.network_normals the normals are the network's analytic density gradient at the vertices (network_normals,
     DESIGN 4.8) instead of central differences of the sigma grid; vertices and faces are unchanged.  Measured on lego, they
-    are better than grid normals with super_sampling >= 1 (vertices on the network's surface) but not at s = 0."""
+    are better than grid normals with super_sampling >= 1 (vertices on the network's surface) but not at s = 0.
+    With args.min_component_faces = m >= 1 the components with fewer than m faces (floaters) are removed as the last step
+    on the device (remove_small_components, DESIGN 4.9); 0 or unset keeps every output as it is."""
     eng = model._engine()
     density = extract_radiance(model, args, device, args.res, sigma_only=True)
     iso_value = extract_iso_level(density, args, eng)
@@ -117,6 +132,9 @@ def extract_geometry(model, device, args):
         lins = [torch.linspace(-args.limit, args.limit, n) for n in density.shape]
         normals, fb = network_normals(eng, model.get_model()._owner[1], verts, lins, normals)
         _report_fallback(fb, verts.shape[0])
+    # the last step on the device arrays: everything downstream (rescale, cache, appearance, OBJ) sees the filtered mesh
+    m = int(getattr(args, "min_component_faces", 0) or 0)
+    verts, normals, faces = remove_small_components(eng, verts, normals, faces, m)
     # the reference rescales CPU tensors (:82-90); do the same on the host so the rounding is identical (torch's CUDA
     # division by a python scalar multiplies by the reciprocal, which differs in the last bit)
     vertices = args.limit * (verts.cpu() / (args.res / 2.0) - 1.0)    # keeps the reference's res/2 scale (:90)

@@ -251,8 +251,11 @@ def extract_geometry_sharded(model, args, group=None, to_host=True, timings=None
     vertices by the ids that rank assigns (nm_mc_count / nm_mc_emit), so the concatenation IS the single-GPU mesh — same
     arrays, bit for bit; there are no duplicates to remove.  args.super_sampling = s >= 1 emits through nm_mc_emit_ss
     (super-sampled edge vertices, the same arrays as single-GPU extract_geometry with that s); args.network_normals
-    replaces each rank's own normals by the network's density gradient before the gather (mesh.network_normals).  Returns (vertices, triangles, normals, iso) like the single-GPU
-    function (vertices rescaled to (-limit, limit) when to_host).  Works without a process group (one slab)."""
+    replaces each rank's own normals by the network's density gradient before the gather (mesh.network_normals).
+    args.min_component_faces = m >= 1 removes the components with fewer than m faces AFTER the gather (components cross
+    slab boundaries): every rank filters the identical gathered mesh, so every rank returns the single-GPU arrays.  Returns
+    (vertices, triangles, normals, iso) like the single-GPU function (vertices rescaled to (-limit, limit) when to_host).
+    Works without a process group (one slab)."""
     import numpy as np
     rank, world = _rank_world(group)
     eng = model._engine()
@@ -339,6 +342,11 @@ def extract_geometry_sharded(model, args, group=None, to_host=True, timings=None
         n = torch.cat([full[r, 3 * vmax:3 * vmax + 3 * nvs[r]] for r in range(world)]).view(-1, 3)
         f = torch.cat([full[r, 6 * vmax:6 * vmax + 3 * nts[r]] for r in range(world)]).view(torch.int32).view(-1, 3)
         tm.mark("gather")
+    m = int(getattr(args, "min_component_faces", 0) or 0)
+    if m > 0:
+        from .mesh import remove_small_components
+        v, n, f = remove_small_components(eng, v, n, f, m)
+        tm.mark("components")
     tm.finish()
     if to_host:
         v = args.limit * (v.cpu() / (res / 2.0) - 1.0)
