@@ -61,10 +61,8 @@ struct NmHandle_t {
   std::vector<cudaEvent_t> ev;
   size_t ev_used = 0;
   int64_t mlp_points = 0, mlp_launches = 0;
-  size_t mc_ws_bytes = 0;
-  void* mc_ws_ptr = nullptr;
-  size_t mc_ws2_bytes = 0;
-  void* mc_ws2_ptr = nullptr;
+  Buf mc_ws, mc_ws2;               // marching cubes: the count step's bit masks and scans, read by the emit step; the emit
+                                   // step's vertex / triangle records
   int64_t mc_counts[2] = {0, 0};   // {vertices, triangles} of the last count step: sizes of the emit step
   Buf ss_tab, ss_ws;               // super-sampled emit: the six coordinate tables; chunk points (M,3) + sigma (M,)
   Buf ms_ws, nn_ws;                // chamfer evaluation: surface sampler (areas, cdf); grid nearest-neighbour search
@@ -504,9 +502,7 @@ int nm_destroy(NmHandle h) {
   for (int i = 0; i < 2; ++i) { h->g_wt[i].release(); h->g_bias[i].release(); h->g_head[i].release(); h->tr_rgb[i].release(); h->tr_drgb[i].release(); }
   h->train_ws.release(); h->dout.release(); h->trans.release();
   h->ss_tab.release(); h->ss_ws.release(); h->ms_ws.release(); h->nn_ws.release(); h->sg_ws.release();
-  h->cc_ws.release();
-  if (h->mc_ws_ptr) cudaFree(h->mc_ws_ptr);
-  if (h->mc_ws2_ptr) cudaFree(h->mc_ws2_ptr);
+  h->cc_ws.release(); h->mc_ws.release(); h->mc_ws2.release();
   if (h->h_err) cudaFreeHost(h->h_err);
   cudaFree(h->d_stats);
   for (cudaEvent_t e : h->ev) cudaEventDestroy(e);
@@ -813,7 +809,8 @@ int nm_mc_count(NmHandle h, const float* vol_dev, int nb, int ny, int nz, float 
   if (int e = bind_device(h)) return e;
   NM_CHECK(vol_dev && counts_host, "null argument");
   const McShard s{vol_dev, nb, ny, nz, iso, g_x0, g_nx, p_lo, p_hi, 0};
-  if (int e = mc_count(s, &h->mc_ws_ptr, &h->mc_ws_bytes, counts_host, (cudaStream_t)stream, &h->launches)) return e;
+  if (int e = h->mc_ws.ensure(mc_ws_bytes(s))) return e;
+  if (int e = mc_count(s, h->mc_ws.p, h->mc_ws.cap, counts_host, h->num_sms, (cudaStream_t)stream, &h->launches)) return e;
   h->mc_counts[0] = counts_host[0]; h->mc_counts[1] = counts_host[1];
   return 0;
 }
@@ -821,10 +818,11 @@ int nm_mc_count(NmHandle h, const float* vol_dev, int nb, int ny, int nz, float 
 int nm_mc_emit(NmHandle h, const float* vol_dev, int nb, int ny, int nz, float iso, int g_x0, int g_nx, int p_lo, int p_hi,
                int64_t v_base, float* verts_dev, float* normals_dev, int32_t* faces_dev, void* stream) {
   if (int e = bind_device(h)) return e;
-  NM_CHECK(vol_dev && verts_dev && faces_dev && h->mc_ws_ptr, "bad arguments (call nm_mc_count first)");
+  NM_CHECK(vol_dev && verts_dev && faces_dev && h->mc_ws.p, "bad arguments (call nm_mc_count first)");
   const McShard s{vol_dev, nb, ny, nz, iso, g_x0, g_nx, p_lo, p_hi, 0};
-  return mc_emit(s, h->mc_ws_ptr, h->mc_ws_bytes, &h->mc_ws2_ptr, &h->mc_ws2_bytes, v_base, h->mc_counts[0], h->mc_counts[1],
-                 verts_dev, normals_dev, faces_dev, (cudaStream_t)stream, &h->launches);
+  if (int e = h->mc_ws2.ensure(mc_emit_ws_bytes(h->mc_counts[0], h->mc_counts[1]))) return e;
+  return mc_emit(s, h->mc_ws.p, h->mc_ws.cap, h->mc_ws2.p, v_base, h->mc_counts[0], h->mc_counts[1], verts_dev, normals_dev,
+                 faces_dev, (cudaStream_t)stream, &h->launches);
 }
 
 int nm_mc_emit_ss(NmHandle h, const float* vol_dev, int nb, int ny, int nz, float iso, int g_x0, int g_nx, int p_lo, int p_hi,
@@ -834,7 +832,7 @@ int nm_mc_emit_ss(NmHandle h, const float* vol_dev, int nb, int ny, int nz, floa
   if (int e = bind_checked(h)) return e;
   NM_CHECK(s >= 0 && s <= kMcMaxSuperSampling, "super-sampling factor %d outside [0, %d]", s, kMcMaxSuperSampling);
   NM_CHECK(lin0_host && lin1_host && lin2_host && fine0_host && fine1_host && fine2_host, "null coordinate table");
-  NM_CHECK(vol_dev && verts_dev && faces_dev && h->mc_ws_ptr, "bad arguments (call nm_mc_count first)");
+  NM_CHECK(vol_dev && verts_dev && faces_dev && h->mc_ws.p, "bad arguments (call nm_mc_count first)");
   NM_CHECK(ny >= 2 && nz >= 2 && g_nx >= 2, "marching cubes: bad volume shape");
   const int64_t nv = h->mc_counts[0], nt = h->mc_counts[1];
   const McShard sh{vol_dev, nb, ny, nz, iso, g_x0, g_nx, p_lo, p_hi, 0};
@@ -872,8 +870,9 @@ int nm_mc_emit_ss(NmHandle h, const float* vol_dev, int nb, int ny, int nz, floa
       };
     }
   }
-  return mc_emit_ss(sh, h->mc_ws_ptr, h->mc_ws_bytes, &h->mc_ws2_ptr, &h->mc_ws2_bytes, v_base, nv, nt, ss, verts_dev,
-                    normals_dev, faces_dev, st, &h->launches);
+  if (int e = h->mc_ws2.ensure(mc_emit_ws_bytes(nv, nt))) return e;
+  return mc_emit_ss(sh, h->mc_ws.p, h->mc_ws.cap, h->mc_ws2.p, v_base, nv, nt, ss, verts_dev, normals_dev, faces_dev, st,
+                    &h->launches);
 }
 
 // ---------------------------------------------------------------------------------------------- density gradient
@@ -921,7 +920,8 @@ int nm_mesh_sample(NmHandle h, const float* verts_dev, int64_t V, const int32_t*
   NM_CHECK(h != nullptr, "null handle");
   if (n == 0) return 0;
   if (int e = bind_checked(h)) return e;
-  return mesh_sample(verts_dev, V, faces_dev, F, n, seed, points_dev, face_idx_dev, h->d_err + 2, &h->ms_ws.p, &h->ms_ws.cap,
+  if (int e = h->ms_ws.ensure(mesh_sample_ws_bytes(F))) return e;
+  return mesh_sample(verts_dev, V, faces_dev, F, n, seed, points_dev, face_idx_dev, h->d_err + 2, h->ms_ws.p, h->ms_ws.cap,
                      (cudaStream_t)stream, &h->launches);
 }
 
@@ -942,7 +942,9 @@ int nm_nearest(NmHandle h, const float* q_dev, int64_t N, const float* p_dev, in
   if (int e = check_nn_args(h, q_dev, N, p_dev, M, dist2_dev)) return e;
   if (N == 0) return 0;
   if (int e = bind_checked(h)) return e;
-  return nearest(q_dev, N, p_dev, M, dist2_dev, idx_dev, &h->nn_ws.p, &h->nn_ws.cap, (cudaStream_t)stream, &h->launches);
+  if (int e = h->nn_ws.ensure(nearest_ws_bytes(N, M, false))) return e;
+  return nearest(q_dev, N, p_dev, M, dist2_dev, idx_dev, h->nn_ws.p, h->nn_ws.cap, h->num_sms, (cudaStream_t)stream,
+                 &h->launches);
 }
 
 int nm_debug_nearest_brute(NmHandle h, const float* q_dev, int64_t N, const float* p_dev, int64_t M, float* dist2_dev,
@@ -959,7 +961,8 @@ int nm_chamfer(NmHandle h, const float* x_dev, int64_t N, const float* y_dev, in
   NM_CHECK(N < (1ll << 31) && M < (1ll << 31), "chamfer: sizes must be below 2^31");
   NM_CHECK(h != nullptr, "null handle");
   if (int e = bind_checked(h)) return e;
-  return chamfer(x_dev, N, y_dev, M, means_dev, &h->nn_ws.p, &h->nn_ws.cap, (cudaStream_t)stream, &h->launches);
+  if (int e = h->nn_ws.ensure(nearest_ws_bytes(N, M, true))) return e;
+  return chamfer(x_dev, N, y_dev, M, means_dev, h->nn_ws.p, h->nn_ws.cap, h->num_sms, (cudaStream_t)stream, &h->launches);
 }
 
 // ---------------------------------------------------------------------------------------------- small-component removal
@@ -992,10 +995,11 @@ int nm_marching_cubes_emit(NmHandle h, const float* vol_dev, int nx, int ny, int
   NM_CHECK(x_off >= 0.f && x_off == (float)(int)x_off, "x_off must be a non-negative integer number of planes");
   // a stand-alone volume whose axis-0 vertex coordinates start at x_off (a pure coordinate shift)
   if (int e = bind_device(h)) return e;
-  NM_CHECK(vol_dev && verts_dev && faces_dev && h->mc_ws_ptr, "bad arguments (call nm_marching_cubes_count first)");
+  NM_CHECK(vol_dev && verts_dev && faces_dev && h->mc_ws.p, "bad arguments (call nm_marching_cubes_count first)");
   const McShard s{vol_dev, nx, ny, nz, iso, 0, nx, 0, nx, (int)x_off};
-  return mc_emit(s, h->mc_ws_ptr, h->mc_ws_bytes, &h->mc_ws2_ptr, &h->mc_ws2_bytes, 0, h->mc_counts[0], h->mc_counts[1], verts_dev,
-                 normals_dev, faces_dev, (cudaStream_t)stream, &h->launches);
+  if (int e = h->mc_ws2.ensure(mc_emit_ws_bytes(h->mc_counts[0], h->mc_counts[1]))) return e;
+  return mc_emit(s, h->mc_ws.p, h->mc_ws.cap, h->mc_ws2.p, 0, h->mc_counts[0], h->mc_counts[1], verts_dev, normals_dev,
+                 faces_dev, (cudaStream_t)stream, &h->launches);
 }
 
 int nm_query_host(NmHandle h, const float* origins_host, int o_stride, const float* dirs_host, int64_t R,

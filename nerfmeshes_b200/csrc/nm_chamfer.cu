@@ -22,15 +22,6 @@ constexpr int kRange = 256;          // faces per range of the area scan
 constexpr int kScanBlock = kScanBlockEntries;   // entries per block of the cell-count scan (shared: exclusive_scan)
 constexpr int kSumBlocks = 256;      // blocks per array of the chamfer reduction
 
-int grow(void** ptr, size_t* bytes, size_t need) {
-  if (*bytes >= need) return 0;
-  if (*ptr) NM_CUDA(cudaFree(*ptr));
-  *ptr = nullptr; *bytes = 0;
-  const size_t want = need + need / 8;
-  NM_CUDA(cudaMalloc(ptr, want));
-  *bytes = want;
-  return 0;
-}
 size_t align_up(size_t x) { return (x + 255) & ~(size_t)255; }
 
 // ------------------------------------------------------------------------------------------------ 1. surface sampler
@@ -409,9 +400,8 @@ __global__ void __launch_bounds__(kSumBlocks) nn_mean_kernel(const double* __res
 }
 
 unsigned blocks_for(long long n, int per) { return (unsigned)((n + per - 1) / per); }
-unsigned stride_blocks(long long n) {
-  static int sms = [] { int dev = 0, s = 132; cudaGetDevice(&dev); cudaDeviceGetAttribute(&s, cudaDevAttrMultiProcessorCount, dev); return s; }();
-  const long long b = (n + kBlock - 1) / kBlock, cap = (long long)sms * 8;
+unsigned stride_blocks(long long n, int num_sms) {
+  const long long b = (n + kBlock - 1) / kBlock, cap = (long long)num_sms * 8;
   return (unsigned)(b < 1 ? 1 : (b > cap ? cap : b));
 }
 
@@ -425,15 +415,18 @@ long long cell_cap(long long M) {
   const long long T = M / 2 < 1 ? 1 : (M / 2 > (1ll << 20) ? (1ll << 20) : M / 2);
   return 2 * T + 64;
 }
-int carve(void** ws, size_t* bytes, long long cap, long long maxM, long long maxN, long long nd0, long long nd1, NnWs* w) {
-  const long long cells = cap + 1, nblk = (cells + kScanBlock - 1) / kScanBlock;
+// Lays out the workspace of one search of N queries among M points, or (both) of chamfer's two searches with their distance
+// arrays, and returns its size; with ws == nullptr only the size is computed.
+size_t carve(void* ws, long long N, long long M, bool both, NnWs* w) {
+  const long long big = N > M ? N : M, maxM = both ? big : M, maxN = both ? big : N, nd0 = both ? N : 0, nd1 = both ? M : 0;
+  const long long cells = cell_cap(maxM) + 1, nblk = (cells + kScanBlock - 1) / kScanBlock;
   const size_t sz[12] = {64, sizeof(NnGrid), (size_t)nblk * 4, (size_t)cells * 4, (size_t)cells * 4, (size_t)cells * 4,
                          (size_t)cells * 4, (size_t)maxM * 16, (size_t)maxN * 4, (size_t)nd0 * 4, (size_t)nd1 * 4,
                          2 * kSumBlocks * sizeof(double)};
   size_t off[12], tot = 0;
   for (int i = 0; i < 12; ++i) { off[i] = tot; tot += align_up(sz[i]); }
-  if (int e = grow(ws, bytes, tot)) return e;
-  char* b = reinterpret_cast<char*>(*ws);
+  if (!ws) return tot;
+  char* b = reinterpret_cast<char*>(ws);
   w->box = reinterpret_cast<int*>(b + off[0]); w->grid = reinterpret_cast<NnGrid*>(b + off[1]);
   w->blk = reinterpret_cast<int*>(b + off[2]); w->cntP = reinterpret_cast<int*>(b + off[3]);
   w->startP = reinterpret_cast<int*>(b + off[4]); w->cntQ = reinterpret_cast<int*>(b + off[5]);
@@ -441,37 +434,38 @@ int carve(void** ws, size_t* bytes, long long cap, long long maxM, long long max
   w->qorder = reinterpret_cast<int*>(b + off[8]); w->d[0] = reinterpret_cast<float*>(b + off[9]);
   w->d[1] = reinterpret_cast<float*>(b + off[10]); w->partial = reinterpret_cast<double*>(b + off[11]);
   w->cells = cells;
-  return 0;
+  return tot;
 }
 
 int scan_cells(const NnWs& w, const int* cnt, int* start, cudaStream_t st) { return exclusive_scan(cnt, w.cells, w.blk, start, st); }
 
 // bounding box of (a, b): the grid every search of one call uses
-int box_of(const NnWs& w, const float* a, long long na, const float* b, long long nb, cudaStream_t st, int64_t* launches) {
+int box_of(const NnWs& w, const float* a, long long na, const float* b, long long nb, int num_sms, cudaStream_t st,
+           int64_t* launches) {
   NM_CUDA(cudaMemsetAsync(w.box, 0x7f, 12, st));
   NM_CUDA(cudaMemsetAsync(w.box + 3, 0x80, 12, st));
-  nn_box_kernel<<<stride_blocks(na + nb), kBlock, 0, st>>>(a, na, b, nb, w.box);
+  nn_box_kernel<<<stride_blocks(na + nb, num_sms), kBlock, 0, st>>>(a, na, b, nb, w.box);
   NM_CUDA(cudaGetLastError());
   if (launches) *launches += 1;
   return 0;
 }
 
 // one search: grid over p (M points, cell size from M), queries q (N), results at the queries' original indices
-int search(const NnWs& w, const float* q, long long N, const float* p, long long M, float* dist2, int* idx, cudaStream_t st,
-           int64_t* launches) {
+int search(const NnWs& w, const float* q, long long N, const float* p, long long M, float* dist2, int* idx, int num_sms,
+           cudaStream_t st, int64_t* launches) {
   nn_params_kernel<<<1, 1, 0, st>>>(w.box, (double)(M / 2 < 1 ? 1 : M / 2), w.cells - 1, w.grid);
   NM_CUDA(cudaGetLastError());
   NM_CUDA(cudaMemsetAsync(w.cntP, 0, (size_t)w.cells * 4, st));
   NM_CUDA(cudaMemsetAsync(w.cntQ, 0, (size_t)w.cells * 4, st));
-  nn_count_kernel<<<stride_blocks(M), kBlock, 0, st>>>(p, M, w.grid, w.cntP, 1);
-  nn_count_kernel<<<stride_blocks(N), kBlock, 0, st>>>(q, N, w.grid, w.cntQ, 0);
+  nn_count_kernel<<<stride_blocks(M, num_sms), kBlock, 0, st>>>(p, M, w.grid, w.cntP, 1);
+  nn_count_kernel<<<stride_blocks(N, num_sms), kBlock, 0, st>>>(q, N, w.grid, w.cntQ, 0);
   NM_CUDA(cudaGetLastError());
   if (int e = scan_cells(w, w.cntP, w.startP, st)) return e;
   if (int e = scan_cells(w, w.cntQ, w.startQ, st)) return e;
   NM_CUDA(cudaMemsetAsync(w.cntP, 0, (size_t)w.cells * 4, st));
   NM_CUDA(cudaMemsetAsync(w.cntQ, 0, (size_t)w.cells * 4, st));
-  nn_scatter_kernel<<<stride_blocks(M), kBlock, 0, st>>>(p, M, w.grid, w.startP, w.cntP, w.sp, nullptr);
-  nn_scatter_kernel<<<stride_blocks(N), kBlock, 0, st>>>(q, N, w.grid, w.startQ, w.cntQ, nullptr, w.qorder);
+  nn_scatter_kernel<<<stride_blocks(M, num_sms), kBlock, 0, st>>>(p, M, w.grid, w.startP, w.cntP, w.sp, nullptr);
+  nn_scatter_kernel<<<stride_blocks(N, num_sms), kBlock, 0, st>>>(q, N, w.grid, w.startQ, w.cntQ, nullptr, w.qorder);
   nn_search_kernel<<<blocks_for(N, kBlock), kBlock, 0, st>>>(q, w.qorder, N, w.grid, w.sp, w.startP, dist2, idx);
   NM_CUDA(cudaGetLastError());
   if (launches) *launches += 12;
@@ -489,15 +483,24 @@ int exclusive_scan(const int* cnt, long long n, int* blk, int* start, cudaStream
   return 0;
 }
 
-int mesh_sample(const float* verts, long long V, const int32_t* faces, long long F, long long n, uint64_t seed, float* pts,
-                int32_t* face_idx, int* d_err, void** ws, size_t* ws_bytes, cudaStream_t st, int64_t* launches) {
-  const long long T = (F + kRange - 1) / kRange;
+// the surface sampler's workspace: area (F floats) | cdf (F doubles) | base (T+1 doubles), T ranges of kRange faces
+struct MsLayout { size_t o_cdf, o_base, bytes; };
+static MsLayout ms_layout(long long F) {
   const size_t o_cdf = align_up((size_t)F * 4), o_base = o_cdf + align_up((size_t)F * 8);
-  if (int e = grow(ws, ws_bytes, o_base + (size_t)(T + 1) * 8)) return e;
-  char* b = reinterpret_cast<char*>(*ws);
+  return {o_cdf, o_base, o_base + (size_t)((F + kRange - 1) / kRange + 1) * 8};
+}
+size_t mesh_sample_ws_bytes(long long F) { return ms_layout(F).bytes; }
+size_t nearest_ws_bytes(long long N, long long M, bool chamfer) { return carve(nullptr, N, M, chamfer, nullptr); }
+
+int mesh_sample(const float* verts, long long V, const int32_t* faces, long long F, long long n, uint64_t seed, float* pts,
+                int32_t* face_idx, int* d_err, void* ws, size_t ws_bytes, cudaStream_t st, int64_t* launches) {
+  const long long T = (F + kRange - 1) / kRange;
+  const MsLayout l = ms_layout(F);
+  NM_CHECK(ws && ws_bytes >= l.bytes, "mesh sampler: workspace smaller than mesh_sample_ws_bytes");
+  char* b = reinterpret_cast<char*>(ws);
   float* area = reinterpret_cast<float*>(b);
-  double* cdf = reinterpret_cast<double*>(b + o_cdf);
-  double* base = reinterpret_cast<double*>(b + o_base);
+  double* cdf = reinterpret_cast<double*>(b + l.o_cdf);
+  double* base = reinterpret_cast<double*>(b + l.o_base);
   ms_area_kernel<<<blocks_for(F, kBlock), kBlock, 0, st>>>(verts, V, faces, F, area, d_err);
   ms_range_kernel<<<blocks_for(T, kBlock), kBlock, 0, st>>>(area, F, base, cdf, 0);
   ms_chain_kernel<<<1, 1, 0, st>>>(base, T, d_err);
@@ -508,12 +511,13 @@ int mesh_sample(const float* verts, long long V, const int32_t* faces, long long
   return 0;
 }
 
-int nearest(const float* q, long long N, const float* p, long long M, float* dist2, int32_t* idx, void** ws, size_t* ws_bytes,
-            cudaStream_t st, int64_t* launches) {
+int nearest(const float* q, long long N, const float* p, long long M, float* dist2, int32_t* idx, void* ws, size_t ws_bytes,
+            int num_sms, cudaStream_t st, int64_t* launches) {
   NnWs w{};
-  if (int e = carve(ws, ws_bytes, cell_cap(M), M, N, 0, 0, &w)) return e;
-  if (int e = box_of(w, q, N, p, M, st, launches)) return e;
-  return search(w, q, N, p, M, dist2, idx, st, launches);
+  NM_CHECK(ws && ws_bytes >= nearest_ws_bytes(N, M, false), "nearest neighbour: workspace smaller than nearest_ws_bytes");
+  carve(ws, N, M, false, &w);
+  if (int e = box_of(w, q, N, p, M, num_sms, st, launches)) return e;
+  return search(w, q, N, p, M, dist2, idx, num_sms, st, launches);
 }
 
 int nearest_brute(const float* q, long long N, const float* p, long long M, float* dist2, int32_t* idx, cudaStream_t st,
@@ -524,14 +528,14 @@ int nearest_brute(const float* q, long long N, const float* p, long long M, floa
   return 0;
 }
 
-int chamfer(const float* x, long long N, const float* y, long long M, double* means, void** ws, size_t* ws_bytes, cudaStream_t st,
-            int64_t* launches) {
-  const long long big = N > M ? N : M;
+int chamfer(const float* x, long long N, const float* y, long long M, double* means, void* ws, size_t ws_bytes, int num_sms,
+            cudaStream_t st, int64_t* launches) {
   NnWs w{};
-  if (int e = carve(ws, ws_bytes, cell_cap(big), big, big, N, M, &w)) return e;
-  if (int e = box_of(w, x, N, y, M, st, launches)) return e;
-  if (int e = search(w, x, N, y, M, w.d[0], nullptr, st, launches)) return e;     // d(x_i, Y)
-  if (int e = search(w, y, M, x, N, w.d[1], nullptr, st, launches)) return e;     // d(y_j, X)
+  NM_CHECK(ws && ws_bytes >= nearest_ws_bytes(N, M, true), "chamfer: workspace smaller than nearest_ws_bytes");
+  carve(ws, N, M, true, &w);
+  if (int e = box_of(w, x, N, y, M, num_sms, st, launches)) return e;
+  if (int e = search(w, x, N, y, M, w.d[0], nullptr, num_sms, st, launches)) return e;     // d(x_i, Y)
+  if (int e = search(w, y, M, x, N, w.d[1], nullptr, num_sms, st, launches)) return e;     // d(y_j, X)
   nn_sum_kernel<<<dim3(kSumBlocks, 2), kBlock, 0, st>>>(w.d[0], N, w.d[1], M, w.partial);
   nn_mean_kernel<<<1, kSumBlocks, 0, st>>>(w.partial, N, M, means);
   NM_CUDA(cudaGetLastError());

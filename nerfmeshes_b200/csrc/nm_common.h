@@ -219,10 +219,13 @@ struct McShard {
   int g_x0, g_nx, p_lo, p_hi;
   int x_shift;       // added to the axis-0 vertex coordinates only (stand-alone volumes that are a window of a larger one)
 };
-// counts_host[2]: {vertices owned, triangles}; ws2 is a second grow-only workspace (8 bytes per output vertex / triangle)
-int mc_count(const McShard& s, void** ws, size_t* ws_bytes, int64_t* counts_host, cudaStream_t st, int64_t* launches);
-int mc_emit(const McShard& s, void* ws, size_t ws_bytes, void** ws2, size_t* ws2_bytes, long long v_base, int64_t nv, int64_t nt,
-            float* verts, float* normals, int32_t* faces, cudaStream_t st, int64_t* launches);
+// counts_host[2]: {vertices owned, triangles}.  ws: mc_ws_bytes(s) bytes (0 for a shard mc_count rejects) that the count step
+// writes and the emit step of the same shard reads; ws2: mc_emit_ws_bytes(nv, nt) bytes (8 per output vertex / triangle)
+size_t mc_ws_bytes(const McShard& s);
+size_t mc_emit_ws_bytes(int64_t nv, int64_t nt);
+int mc_count(const McShard& s, void* ws, size_t ws_bytes, int64_t* counts_host, int num_sms, cudaStream_t st, int64_t* launches);
+int mc_emit(const McShard& s, void* ws, size_t ws_bytes, void* ws2, long long v_base, int64_t nv, int64_t nt, float* verts,
+            float* normals, int32_t* faces, cudaStream_t st, int64_t* launches);
 // super-sampled emit (nm_mc_emit_ss): mc_emit, then every edge vertex is re-placed from s network samples along its edge.
 // The vertices are walked in chunks of chunk_vertices; each chunk's chunk_vertices*s points go to `pts` (M,3), are
 // evaluated by `eval` (sigma only, at most chunk_points per call) into `sig` (M,), and the chunk's vertices are refined.
@@ -236,9 +239,8 @@ struct McSuperSampling {
   long long chunk_vertices = 0, chunk_points = 0;
   std::function<int(const float* pts, long long M, float* sigma)> eval;
 };
-int mc_emit_ss(const McShard& s, void* ws, size_t ws_bytes, void** ws2, size_t* ws2_bytes, long long v_base, int64_t nv,
-               int64_t nt, const McSuperSampling& ss, float* verts, float* normals, int32_t* faces, cudaStream_t st,
-               int64_t* launches);
+int mc_emit_ss(const McShard& s, void* ws, size_t ws_bytes, void* ws2, long long v_base, int64_t nv, int64_t nt,
+               const McSuperSampling& ss, float* verts, float* normals, int32_t* faces, cudaStream_t st, int64_t* launches);
 
 // exclusive scan of n >= 1 ints (nm_chamfer.cu: the grid search's cell-count scan, also used by the component filter):
 // start[i] = cnt[0] + ... + cnt[i-1], exact (integers).  blk: (n + kScanBlockEntries - 1) / kScanBlockEntries ints of scratch.
@@ -246,19 +248,21 @@ int mc_emit_ss(const McShard& s, void* ws, size_t ws_bytes, void** ws2, size_t* 
 constexpr int kScanBlockEntries = 1024;
 int exclusive_scan(const int* cnt, long long n, int* blk, int* start, cudaStream_t st);
 
-// chamfer evaluation (nm_chamfer.cu).  ws / ws_bytes: a grow-only workspace of the handle.
+// chamfer evaluation (nm_chamfer.cu).  ws / ws_bytes: the handle's grow-only workspace, at least *_ws_bytes of the same counts.
+size_t mesh_sample_ws_bytes(long long F);
+size_t nearest_ws_bytes(long long N, long long M, bool chamfer);      // one search, or chamfer's two with their distances
 // mesh_sample: n area-weighted surface points (face index per point if face_idx != nullptr); a face index outside [0,V)
 // sets *d_err = 1, a total area that is not positive and finite *d_err = 2 (device-side, mapped memory)
 int mesh_sample(const float* verts, long long V, const int32_t* faces, long long F, long long n, uint64_t seed, float* pts,
-                int32_t* face_idx, int* d_err, void** ws, size_t* ws_bytes, cudaStream_t st, int64_t* launches);
+                int32_t* face_idx, int* d_err, void* ws, size_t ws_bytes, cudaStream_t st, int64_t* launches);
 // exact nearest neighbour of each of N queries among M >= 1 points: squared distance (+ index, lowest on ties)
-int nearest(const float* q, long long N, const float* p, long long M, float* dist2, int32_t* idx, void** ws, size_t* ws_bytes,
-            cudaStream_t st, int64_t* launches);
+int nearest(const float* q, long long N, const float* p, long long M, float* dist2, int32_t* idx, void* ws, size_t ws_bytes,
+            int num_sms, cudaStream_t st, int64_t* launches);
 int nearest_brute(const float* q, long long N, const float* p, long long M, float* dist2, int32_t* idx, cudaStream_t st,
                   int64_t* launches);
 // means[0] = mean_i d2(x_i, Y), means[1] = mean_j d2(y_j, X) (double, fixed summation order)
-int chamfer(const float* x, long long N, const float* y, long long M, double* means, void** ws, size_t* ws_bytes, cudaStream_t st,
-            int64_t* launches);
+int chamfer(const float* x, long long N, const float* y, long long M, double* means, void* ws, size_t ws_bytes, int num_sms,
+            cudaStream_t st, int64_t* launches);
 
 // small-component removal (nm_components.cu, DESIGN §4.9).  ws: components_ws_bytes(V, F) bytes of the handle's grow-only
 // workspace.  A face index outside [0,V) sets *d_err = 3 (device-side, mapped memory); such a face joins nothing and is

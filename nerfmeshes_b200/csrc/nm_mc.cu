@@ -585,23 +585,27 @@ int make_grid(const McShard& s, McGrid* g) {
 
 }  // namespace
 
-int mc_count(const McShard& s, void** ws_ptr, size_t* ws_bytes, int64_t* counts_host, cudaStream_t st, int64_t* launches) {
+size_t mc_ws_bytes(const McShard& s) {
+  McGrid g{};
+  size_t need = 0;
+  if (make_grid(s, &g)) return 0;            // a bad shard: mc_count reports it
+  carve(nullptr, 0, &g, &need);
+  return need;
+}
+
+size_t mc_emit_ws_bytes(int64_t nv, int64_t nt) { return align_up((size_t)nv * 8 + 8) + (size_t)nt * 8 + 8; }
+
+int mc_count(const McShard& s, void* ws, size_t ws_bytes, int64_t* counts_host, int num_sms, cudaStream_t st,
+             int64_t* launches) {
   McGrid g{};
   if (int e = make_grid(s, &g)) return e;
   size_t need = 0;
-  if (carve(*ws_ptr, *ws_bytes, &g, &need)) {
-    if (*ws_ptr) NM_CUDA(cudaFree(*ws_ptr));
-    *ws_ptr = nullptr; *ws_bytes = 0;
-    NM_CUDA(cudaMalloc(ws_ptr, need));
-    *ws_bytes = need;
-    NM_CHECK(carve(*ws_ptr, *ws_bytes, &g, &need) == 0, "workspace carve failed");
-  }
+  NM_CHECK(carve(ws, ws_bytes, &g, &need) == 0, "marching cubes: workspace smaller than mc_ws_bytes");
   counts_host[0] = counts_host[1] = 0;
   if (g.nwords == 0) return 0;
   const long long nlines = (long long)g.nb * g.ny;
-  static int sms = [] { int dev = 0, n = 148; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); return n; }();
   long long sign_blocks = (nlines * g.W + (kBlock / 32) * 8 - 1) / ((kBlock / 32) * 8);
-  if (sign_blocks > (long long)sms * 4) sign_blocks = (long long)sms * 4;       // one resident wave, grid-stride
+  if (sign_blocks > (long long)num_sms * 4) sign_blocks = (long long)num_sms * 4;       // one resident wave, grid-stride
   NM_CUDA(cudaMemsetAsync(g.totals, 0, 64, st));
   mc_sign_kernel<<<(unsigned)sign_blocks, kBlock, 0, st>>>(g.vol, nlines, g.nz, g.W, g.iso, g.sign);
   NM_CUDA(cudaGetLastError());
@@ -624,23 +628,16 @@ int mc_count(const McShard& s, void** ws_ptr, size_t* ws_bytes, int64_t* counts_
   return 0;
 }
 
-int mc_emit(const McShard& s, void* ws_ptr, size_t ws_bytes, void** ws2_ptr, size_t* ws2_bytes, long long v_base, int64_t nv,
-            int64_t nt, float* verts, float* normals, int32_t* faces, cudaStream_t st, int64_t* launches) {
+int mc_emit(const McShard& s, void* ws, size_t ws_bytes, void* ws2, long long v_base, int64_t nv, int64_t nt, float* verts,
+            float* normals, int32_t* faces, cudaStream_t st, int64_t* launches) {
   McGrid g{};
   if (int e = make_grid(s, &g)) return e;
   size_t need = 0;
-  NM_CHECK(carve(ws_ptr, ws_bytes, &g, &need) == 0, "workspace missing (call the count step first, same arguments)");
+  NM_CHECK(carve(ws, ws_bytes, &g, &need) == 0, "workspace missing (call the count step first, same arguments)");
   if (g.nwords_own == 0 || (nv == 0 && nt == 0)) return 0;
   NM_CHECK(g.nwords_own < (1ll << 32) && nv >= 0 && nt >= 0, "bad counts");
-  const size_t need2 = align_up((size_t)nv * 8 + 8) + (size_t)nt * 8 + 8;
-  if (*ws2_bytes < need2) {
-    if (*ws2_ptr) NM_CUDA(cudaFree(*ws2_ptr));
-    *ws2_ptr = nullptr; *ws2_bytes = 0;
-    NM_CUDA(cudaMalloc(ws2_ptr, need2 + need2 / 4));
-    *ws2_bytes = need2 + need2 / 4;
-  }
-  g.vmap = reinterpret_cast<unsigned long long*>(*ws2_ptr);
-  g.tmap = reinterpret_cast<unsigned long long*>(reinterpret_cast<char*>(*ws2_ptr) + align_up((size_t)nv * 8 + 8));
+  g.vmap = reinterpret_cast<unsigned long long*>(ws2);
+  g.tmap = reinterpret_cast<unsigned long long*>(reinterpret_cast<char*>(ws2) + align_up((size_t)nv * 8 + 8));
   const long long nblk = (g.nwords_own + kBlock - 1) / kBlock;
   mc_expand_kernel<<<(unsigned)nblk, kBlock, 0, st>>>(g);
   NM_CUDA(cudaGetLastError());
@@ -656,12 +653,11 @@ int mc_emit(const McShard& s, void* ws_ptr, size_t ws_bytes, void** ws2_ptr, siz
   return 0;
 }
 
-int mc_emit_ss(const McShard& s, void* ws_ptr, size_t ws_bytes, void** ws2_ptr, size_t* ws2_bytes, long long v_base, int64_t nv,
-               int64_t nt, const McSuperSampling& ss, float* verts, float* normals, int32_t* faces, cudaStream_t st,
-               int64_t* launches) {
+int mc_emit_ss(const McShard& s, void* ws, size_t ws_bytes, void* ws2, long long v_base, int64_t nv, int64_t nt,
+               const McSuperSampling& ss, float* verts, float* normals, int32_t* faces, cudaStream_t st, int64_t* launches) {
   NM_CHECK(ss.s >= 0 && ss.s <= kMcMaxSuperSampling, "super-sampling factor %d outside [0, %d]", ss.s, kMcMaxSuperSampling);
   // the s = 0 mesh (vertices, normals, faces, and the vertex records in the second workspace) ...
-  if (int e = mc_emit(s, ws_ptr, ws_bytes, ws2_ptr, ws2_bytes, v_base, nv, nt, verts, normals, faces, st, launches)) return e;
+  if (int e = mc_emit(s, ws, ws_bytes, ws2, v_base, nv, nt, verts, normals, faces, st, launches)) return e;
   if (nv == 0) return 0;
   NM_CHECK(ss.lin[0] && ss.lin[1] && ss.lin[2] && ss.fine[0] && ss.fine[1] && ss.fine[2], "super-sampling tables missing");
   NM_CHECK(ss.s == 0 || (ss.pts && ss.sig && ss.chunk_vertices > 0 && ss.chunk_points > 0 && ss.eval),
@@ -669,7 +665,7 @@ int mc_emit_ss(const McShard& s, void* ws_ptr, size_t ws_bytes, void** ws2_ptr, 
   // ... then the edge vertices are moved, chunk by chunk
   McGrid g{};
   if (int e = make_grid(s, &g)) return e;
-  g.vmap = reinterpret_cast<unsigned long long*>(*ws2_ptr);
+  g.vmap = reinterpret_cast<unsigned long long*>(ws2);
   SsTables t{};
   for (int a = 0; a < 3; ++a) { t.lin[a] = ss.lin[a]; t.fine[a] = ss.fine[a]; }
   t.s = ss.s;

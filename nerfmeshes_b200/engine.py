@@ -431,6 +431,18 @@ class Engine:
         assert mean is None or (mean.dtype == torch.float64 and mean.is_cuda)
         L.check(self.lib.nm_volume_stats_dev(self._h, _ptr(vol), vol.numel(), int(pass_no), _ptr(mean), _ptr(out), self._stream()))
 
+    def _mesh_out(self, nv, nt, out):
+        """(verts (nv,3), normals (nv,3), faces (nt,3) int32) of an emit step: fresh tensors, or the caller's `out` triple
+        checked for layout and capacity."""
+        if out is None:
+            return (torch.empty((nv, 3), dtype=torch.float32, device=self.device),
+                    torch.empty((nv, 3), dtype=torch.float32, device=self.device),
+                    torch.empty((nt, 3), dtype=torch.int32, device=self.device))
+        verts, normals, faces = out
+        assert verts.is_contiguous() and normals.is_contiguous() and faces.is_contiguous() and faces.dtype == torch.int32
+        assert verts.shape[0] >= nv and faces.shape[0] >= nt
+        return verts, normals, faces
+
     def marching_cubes(self, vol: torch.Tensor, iso: float, x_off: int = 0):
         """skimage.measure.marching_cubes(vol, iso) on the device: (verts (V,3), faces (F,3) int32, normals (V,3)); x_off is
         added to the axis-0 coordinates of the vertices."""
@@ -438,10 +450,8 @@ class Engine:
         nx, ny, nz = v.shape
         counts = (C.c_int64 * 2)()
         L.check(self.lib.nm_marching_cubes_count(self._h, _ptr(v), nx, ny, nz, float(iso), counts, self._stream()))
-        nv, nt = int(counts[0]), int(counts[1])
-        verts = torch.empty((nv, 3), dtype=torch.float32, device=self.device)
-        normals = torch.empty((nv, 3), dtype=torch.float32, device=self.device)
-        faces = torch.empty((nt, 3), dtype=torch.int32, device=self.device)
+        nv = int(counts[0])
+        verts, normals, faces = self._mesh_out(nv, int(counts[1]), None)
         if nv > 0:
             L.check(self.lib.nm_marching_cubes_emit(self._h, _ptr(v), nx, ny, nz, float(iso), float(int(x_off)), _ptr(verts),
                                                     _ptr(normals), _ptr(faces), self._stream()))
@@ -459,14 +469,7 @@ class Engine:
         """Emit step: vertices / normals / faces of the shard, faces offset by v_base.  `out`: optional (verts, normals,
         faces) device tensors to write into (e.g. slices of a gather buffer)."""
         nb, ny, nz = vol.shape
-        if out is None:
-            verts = torch.empty((nv, 3), dtype=torch.float32, device=self.device)
-            normals = torch.empty((nv, 3), dtype=torch.float32, device=self.device)
-            faces = torch.empty((nt, 3), dtype=torch.int32, device=self.device)
-        else:
-            verts, normals, faces = out
-            assert verts.is_contiguous() and normals.is_contiguous() and faces.is_contiguous() and faces.dtype == torch.int32
-            assert verts.shape[0] >= nv and faces.shape[0] >= nt
+        verts, normals, faces = self._mesh_out(nv, nt, out)
         if nv > 0:
             L.check(self.lib.nm_mc_emit(self._h, _ptr(vol), nb, ny, nz, float(iso), int(g_x0), int(g_nx), int(p_lo), int(p_hi),
                                         int(v_base), _ptr(verts), _ptr(normals), _ptr(faces), self._stream()))
@@ -477,14 +480,7 @@ class Engine:
         samples along its edge.  lins: the coarse tables (g_nx, ny, nz entries), fines: the fine tables
         ((n-1)(s+1)+1 entries; mesh.super_sampling_tables)."""
         nb, ny, nz = vol.shape
-        if out is None:
-            verts = torch.empty((nv, 3), dtype=torch.float32, device=self.device)
-            normals = torch.empty((nv, 3), dtype=torch.float32, device=self.device)
-            faces = torch.empty((nt, 3), dtype=torch.int32, device=self.device)
-        else:
-            verts, normals, faces = out
-            assert verts.is_contiguous() and normals.is_contiguous() and faces.is_contiguous() and faces.dtype == torch.int32
-            assert verts.shape[0] >= nv and faces.shape[0] >= nt
+        verts, normals, faces = self._mesh_out(nv, nt, out)
         want = (g_nx, ny, nz)
         tabs = [np.ascontiguousarray(torch.as_tensor(t).detach().cpu().numpy(), dtype=np.float32) for t in (*lins, *fines)]
         for a in range(3):                   # the library cannot see the host tables' lengths

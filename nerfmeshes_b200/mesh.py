@@ -25,6 +25,11 @@ def extract_radiance(model, args, device, nums, sigma_only=False, slab=None):
     return torch.cat((rgb, sigma[..., None]), -1).cpu().numpy()
 
 
+def clamp_iso_level(iso_level, mn, mx, sd):
+    """src/mesh_nerf.py:65, in the arithmetic of the statistics it is given (np.float32 for a float32 grid)."""
+    return min(max(iso_level, mn + sd), mx - sd)
+
+
 def extract_iso_level(density, args, engine=None):
     """src/mesh_nerf.py:56-65: clamp(iso_level, min+std, max-std)."""
     if isinstance(density, torch.Tensor) and density.is_cuda:
@@ -33,7 +38,7 @@ def extract_iso_level(density, args, engine=None):
     else:
         density = np.asarray(density)
         mn, mx, sd = density.min(), density.max(), density.std()
-    return min(max(args.iso_level, mn + sd), mx - sd)
+    return clamp_iso_level(args.iso_level, mn, mx, sd)
 
 
 def marching_cubes(volume, level, engine=None):
@@ -108,37 +113,23 @@ def remove_small_components(eng, verts, normals, faces, m):
     return v, n, f
 
 
+def rescale_vertices(verts, limit, res):
+    """Index coordinates -> (-limit, limit) with the reference's res/2 scale (src/mesh_nerf.py:82-90), on the host like the
+    reference's CPU tensors so the rounding is identical (torch's CUDA division by a python scalar multiplies by the
+    reciprocal, which differs in the last bit)."""
+    return limit * (verts.cpu() / (res / 2.0) - 1.0)
+
+
 def extract_geometry(model, device, args):
-    """src/mesh_nerf.py:68-92: sigma sweep -> adaptive iso -> marching cubes -> rescale to (-limit, limit).
-    With args.super_sampling = s >= 1 (mesh_nerf.py:95-128) the coarse grid's mesh keeps its topology, faces and normals,
-    and each edge vertex is placed from s extra network samples along its edge (nm_mc_emit_ss, DESIGN 4.3).
-    With args.network_normals the normals are the network's analytic density gradient at the vertices (network_normals,
-    DESIGN 4.8) instead of central differences of the sigma grid; vertices and faces are unchanged.  Measured on lego, they
-    are better than grid normals with super_sampling >= 1 (vertices on the network's surface) but not at s = 0.
-    With args.min_component_faces = m >= 1 the components with fewer than m faces (floaters) are removed as the last step
-    on the device (remove_small_components, DESIGN 4.9); 0 or unset keeps every output as it is."""
-    eng = model._engine()
-    density = extract_radiance(model, args, device, args.res, sigma_only=True)
-    iso_value = extract_iso_level(density, args, eng)
-    s = int(getattr(args, "super_sampling", 0) or 0)
-    if s == 0:
-        verts, faces, normals = eng.marching_cubes(density, float(iso_value))
-    else:
-        n0 = density.shape[0]
-        lins, fines = super_sampling_tables(args.limit, tuple(density.shape), s)
-        nv, nt = eng.mc_count(density, float(iso_value), 0, n0, 0, n0)
-        verts, faces, normals = eng.mc_emit_ss(density, float(iso_value), 0, n0, 0, n0, nv, nt, 0, s, lins, fines)
-    if getattr(args, "network_normals", False):
-        lins = [torch.linspace(-args.limit, args.limit, n) for n in density.shape]
-        normals, fb = network_normals(eng, model.get_model()._owner[1], verts, lins, normals)
-        _report_fallback(fb, verts.shape[0])
-    # the last step on the device arrays: everything downstream (rescale, cache, appearance, OBJ) sees the filtered mesh
-    m = int(getattr(args, "min_component_faces", 0) or 0)
-    verts, normals, faces = remove_small_components(eng, verts, normals, faces, m)
-    # the reference rescales CPU tensors (:82-90); do the same on the host so the rounding is identical (torch's CUDA
-    # division by a python scalar multiplies by the reciprocal, which differs in the last bit)
-    vertices = args.limit * (verts.cpu() / (args.res / 2.0) - 1.0)    # keeps the reference's res/2 scale (:90)
-    return vertices, faces.cpu(), normals.cpu(), density.cpu().numpy()
+    """src/mesh_nerf.py:68-92: sigma sweep -> adaptive iso -> marching cubes -> rescale to (-limit, limit).  This is the
+    one-slab case of the mesh pipeline (parallel._extract_mesh, which lists the stages and what args.super_sampling,
+    args.network_normals and args.min_component_faces do), in buffers that die with the call.  Everything downstream
+    (cache, appearance, OBJ) sees the filtered mesh.  `device` is the reference's argument and unused: the model's engine
+    device is.  Returns CPU (vertices, triangles, normals) and the (res, res, res) numpy density grid."""
+    from .parallel import _extract_mesh      # parallel imports this module for the stage helpers above
+    fresh = lambda key, numel, dtype, dev: torch.empty(numel, dtype=dtype, device=dev)
+    verts, faces, normals, _, density = _extract_mesh(model, args, 0, 1, None, fresh)
+    return rescale_vertices(verts, args.limit, args.res), faces.cpu(), normals.cpu(), density.cpu().numpy()
 
 
 def extract_geometry_with_super_sampling(model, device, args):

@@ -2,11 +2,12 @@
 
 Render: contiguous image-row shards, every rank generates its own rays from the 12-float pose; results are bit-identical
 to the single-GPU image (no cross-shard arithmetic), the exchange is one all_gather of the finished rows.
-Mesh: x-slabs of the density grid; every grid point (vertex, cell) is owned by exactly one rank; halo planes by send/recv;
-per-slab marching cubes in global index coordinates with globally consistent vertex ids; the exchange is an all_gather
-of the vertex / triangle counts and ONE all_gather of the per-slab indexed meshes (padded to the largest slab), plus
-scalar all_reduces for the iso-level statistics (extract_iso_level, src/mesh_nerf.py:56-65).  The gathered arrays equal
-the single-GPU arrays bit for bit.
+Mesh: ONE pipeline (_extract_mesh) over x-slabs of the density grid, which single-GPU mesh.extract_geometry runs as its
+one-slab case; every grid point (vertex, cell) is owned by exactly one rank; halo planes by send/recv; per-slab marching
+cubes in global index coordinates with globally consistent vertex ids; the exchange is an all_gather of the vertex /
+triangle counts and ONE all_gather of the per-slab indexed meshes (padded to the largest slab), plus two tiny all_gathers
+for the iso-level statistics (extract_iso_level, src/mesh_nerf.py:56-65).  The gathered arrays equal the one-slab arrays
+bit for bit.
 Training: data parallel over rays — every rank runs forward + backward on its own ray batch (no collective inside), then
 ONE all_reduce of the flattened gradients of both networks (595 k - 1.19 M floats, 4.8 MB) before the optimiser step.
 The collectives go through torch.distributed (NCCL on GPUs, gloo in the CPU tests); there is no data-path collective
@@ -17,8 +18,11 @@ from __future__ import annotations
 import math
 from typing import Dict, Optional, Tuple
 
+import numpy as np
 import torch
 import torch.distributed as dist
+
+from . import mesh
 
 
 def row_shard(H: int, rank: int, world: int) -> Tuple[int, int]:
@@ -170,9 +174,10 @@ _MESH_BUFFERS = {}
 
 
 def _scratch(key, numel, dtype, device):
-    """Grow-only scratch tensors of the mesh path (slab buffer, exchange segments, single-GPU outputs): steady-state calls
+    """Grow-only scratch tensors of the mesh path (slab buffer, exchange segment, gathered segments): steady-state calls
     make no allocator traffic.  Tensors returned by extract_geometry_sharded(to_host=False) are views of these buffers
-    and stay valid until the next call."""
+    and stay valid until the next call with as many slabs: the segments are keyed by the slab count, so a one-slab result
+    survives the N-slab call it is compared with."""
     t = _MESH_BUFFERS.get((key, str(device)))
     if t is None or t.numel() < numel or t.dtype != dtype:
         t = torch.empty(int(numel * 1.25) + 16, dtype=dtype, device=device)
@@ -239,116 +244,115 @@ def exchange_halo_planes(buf: torch.Tensor, n0: int, rank: int, world: int, grou
             r.wait()
 
 
-def extract_geometry_sharded(model, args, group=None, to_host=True, timings=None, halo="exchange"):
-    """mesh_nerf.extract_geometry (src/mesh_nerf.py:68-92) on N GPUs, x-slabs of the grid (SURVEY 8e):
-      1. every rank sweeps sigma over ITS planes (fused MLP, grid front-end) into its slab buffer;
+def _gathered_stats(eng, own, world, group):
+    """Two-pass statistics like the single-GPU nm_volume_stats, shards combined on the device: two tiny all_gathers, and one
+    host read at the end (every plane is owned exactly once, so sums are exact partitions)."""
+    acc = torch.empty(5, dtype=torch.float64, device=own.device)
+    acc[4] = float(own.numel())
+    eng.volume_stats_pass(own, 1, acc)
+    allacc = torch.empty((world, 5), dtype=torch.float64, device=own.device)
+    dist.all_gather_into_tensor(allacc, acc, group=group)
+    mean = (allacc[:, 2].sum() / allacc[:, 4].sum()).reshape(1)
+    eng.volume_stats_pass(own, 2, acc, mean)
+    allsq = torch.empty(world, dtype=torch.float64, device=own.device)
+    dist.all_gather_into_tensor(allsq, acc[3:4].contiguous(), group=group)
+    st3 = torch.stack([allacc[:, 0].min(), allacc[:, 1].max(), (allsq.sum() / allacc[:, 4].sum()).sqrt()]).cpu()
+    return tuple(float(x) for x in st3)
+
+
+def _extract_mesh(model, args, rank, world, group, alloc, timings=None, halo="exchange"):
+    """The mesh pipeline, written once: slab `rank` of `world` x-slabs of the grid (SURVEY 8e), one slab being the whole grid.
+      1. sweep: this rank's planes of sigma (fused MLP, grid front-end) into its slab buffer;
       2. halo planes: 3 planes per interior rank by send/recv from the neighbours (`halo="exchange"`), or recomputed;
-      3. extract_iso_level: min / max / std over the whole grid — scalar all_reduces (every plane is owned exactly once);
-      4. marching cubes, count step; all_gather of the (n_vertices, n_triangles) pairs -> every rank's index offset;
-      5. marching cubes, emit step, straight into this rank's segment of the exchange buffer; ONE all_gather of
-         [vertices | normals | faces] (padded to the largest slab) leaves the whole mesh on every rank.
-    A vertex belongs to the rank that owns its grid point, and the last owned cell layer addresses the next rank's
-    vertices by the ids that rank assigns (nm_mc_count / nm_mc_emit), so the concatenation IS the single-GPU mesh — same
-    arrays, bit for bit; there are no duplicates to remove.  args.super_sampling = s >= 1 emits through nm_mc_emit_ss
-    (super-sampled edge vertices, the same arrays as single-GPU extract_geometry with that s); args.network_normals
-    replaces each rank's own normals by the network's density gradient before the gather (mesh.network_normals).
-    args.min_component_faces = m >= 1 removes the components with fewer than m faces AFTER the gather (components cross
-    slab boundaries): every rank filters the identical gathered mesh, so every rank returns the single-GPU arrays.  Returns
-    (vertices, triangles, normals, iso) like the single-GPU function (vertices rescaled to (-limit, limit) when to_host).
-    Works without a process group (one slab)."""
-    import numpy as np
-    rank, world = _rank_world(group)
+      3. iso level: min / max / std over the whole grid (every plane is owned exactly once), clamped by mesh.clamp_iso_level;
+      4. marching cubes, count step; the (n_vertices, n_triangles) pairs of all ranks give every rank's index offset;
+      5. marching cubes, emit step, straight into this rank's segment [vertices | normals | faces] of the exchange buffer
+         (padded to the largest slab); with args.super_sampling = s >= 1 (mesh_nerf.py:95-128) through nm_mc_emit_ss: same
+         topology, faces and normals, each edge vertex placed from s extra network samples along its edge (DESIGN 4.3);
+      6. args.network_normals: this rank's own normals become the network's density gradient (mesh.network_normals, DESIGN
+         4.8) — before the gather, a vertex's normal depends on that vertex alone.  Measured on lego, they are better than
+         grid normals with super_sampling >= 1 (vertices on the network's surface) but not at s = 0;
+      7. gather: ONE all_gather of the segments leaves the whole mesh on every rank;
+      8. args.min_component_faces = m >= 1: components with fewer than m faces (floaters) are removed AFTER the gather
+         (components cross slab boundaries; DESIGN 4.9); every rank filters the identical gathered mesh.
+    `world > 1` guards nothing but the collectives (halo exchange, statistics, counts, mesh): with one slab the segment is
+    the mesh, the index offset is 0 and the gather is the identity.  A vertex belongs to the rank that owns its grid point,
+    and the last owned cell layer addresses the next rank's vertices by the ids that rank assigns (nm_mc_count /
+    nm_mc_emit), so the concatenation IS the one-slab mesh — same arrays, bit for bit; there are no duplicates to remove.
+    `alloc(key, numel, dtype, device)` supplies the flat device buffers; the results are views of them: device (vertices
+    in index coordinates, triangles, normals), the iso level and the slab buffer (the whole grid for one slab)."""
     eng = model._engine()
     res, dev = args.res, eng.device
     tm = _StageTimer(timings)
     tiles = [torch.linspace(-args.limit, args.limit, res) for _ in range(3)]
     own0, own1, buf0, buf1 = slab_layout(res, rank, world)
     tm.mark()
-    buf = _scratch("slab", (buf1 - buf0) * res * res, torch.float32, dev).view(buf1 - buf0, res, res)
-    can_exchange = world > 1 and halo == "exchange" and all(
+    buf = alloc("slab", (buf1 - buf0) * res * res, torch.float32, dev).view(buf1 - buf0, res, res)
+    exchange = world > 1 and halo == "exchange" and all(
         (lambda a: a[1] - a[0] >= 2)(slab_layout(res, r, world)) for r in range(world))
-    if world == 1 or can_exchange:
-        eng.grid_sigma(tiles, own0, own1, out=buf[own0 - buf0:own1 - buf0])
-        tm.mark("sweep")
-        if world > 1:
-            exchange_halo_planes(buf, res, rank, world, group)
-    else:
-        eng.grid_sigma(tiles, buf0, buf1, out=buf)            # halo planes recomputed (bit-identical to the owner's)
-        tm.mark("sweep")
+    # without an exchange the halo planes are recomputed (bit-identical to the owner's); one slab has none
+    p0, p1 = (own0, own1) if exchange else (buf0, buf1)
+    eng.grid_sigma(tiles, p0, p1, out=buf[p0 - buf0:p1 - buf0])
+    tm.mark("sweep")
+    if exchange:
+        exchange_halo_planes(buf, res, rank, world, group)
     own = buf[own0 - buf0:own1 - buf0]
     tm.mark("halo")
-    if world > 1:
-        # two-pass statistics like the single-GPU nm_volume_stats, shards combined on the device: two tiny all_gathers, and one
-        # host read at the end (every plane is owned exactly once, so sums are exact partitions)
-        acc = torch.empty(5, dtype=torch.float64, device=dev)
-        acc[4] = float(own.numel())
-        eng.volume_stats_pass(own, 1, acc)
-        allacc = torch.empty((world, 5), dtype=torch.float64, device=dev)
-        dist.all_gather_into_tensor(allacc, acc, group=group)
-        mean = (allacc[:, 2].sum() / allacc[:, 4].sum()).reshape(1)
-        eng.volume_stats_pass(own, 2, acc, mean)
-        allsq = torch.empty(world, dtype=torch.float64, device=dev)
-        dist.all_gather_into_tensor(allsq, acc[3:4].contiguous(), group=group)
-        st3 = torch.stack([allacc[:, 0].min(), allacc[:, 1].max(), (allsq.sum() / allacc[:, 4].sum()).sqrt()]).cpu()
-        smin, smax, sstd = (float(np.float32(float(x))) for x in st3)
-    else:
-        smin, smax, sstd = eng.volume_stats(own)
-    iso = float(min(max(args.iso_level, np.float32(smin) + np.float32(sstd)), np.float32(smax) - np.float32(sstd)))
+    smin, smax, sstd = _gathered_stats(eng, own, world, group) if world > 1 else eng.volume_stats(own)
+    iso = float(mesh.clamp_iso_level(args.iso_level, np.float32(smin), np.float32(smax), np.float32(sstd)))
     tm.mark("stats")
     shard = (iso, buf0, res, own0 - buf0, own1 - buf0)
     nv, nt = eng.mc_count(buf, *shard)
-    s = int(getattr(args, "super_sampling", 0) or 0)
-    net_normals = bool(getattr(args, "network_normals", False))
-    if net_normals:
-        from .mesh import network_normals, _report_fallback
-    if s:          # super-sampled vertices: the network is evaluated at the edge samples directly, no extra halo planes
-        from .mesh import super_sampling_tables
-        lins, fines = super_sampling_tables(args.limit, res, s)
-        emit = lambda *a, out: eng.mc_emit_ss(*a, s, lins, fines, out=out)
-    else:
-        emit = lambda *a, out: eng.mc_emit(*a, out=out)
-    if world == 1:
-        outs = (_scratch("v", 3 * nv, torch.float32, dev).view(nv, 3), _scratch("n", 3 * nv, torch.float32, dev).view(nv, 3),
-                _scratch("f", 3 * nt, torch.int32, dev).view(nt, 3))
-        v, f, n = emit(buf, *shard, nv, nt, 0, out=outs)
-        if net_normals:
-            n, fb = network_normals(eng, model.get_model()._owner[1], v, tiles, n)
-            _report_fallback(fb, nv)
-        tm.mark("mc")
-        tm.mark("gather")
-    else:
+    nvs, nts = [nv], [nt]
+    if world > 1:
         counts = torch.tensor([nv, nt], dtype=torch.int64, device=dev)
         allc = torch.empty((world, 2), dtype=torch.int64, device=dev)
         dist.all_gather_into_tensor(allc, counts, group=group)
         allc = allc.cpu()
         nvs, nts = [int(x) for x in allc[:, 0]], [int(x) for x in allc[:, 1]]
-        v_base = sum(nvs[:rank])
         if sum(nvs) >= 2 ** 31:
             raise OverflowError("mesh too large for int32 indices")
-        vmax, tmax = max(max(nvs), 1), max(max(nts), 1)
-        seg = 3 * (2 * vmax + tmax)                               # floats per rank: vertices | normals | faces (int32 bits)
-        local = _scratch("local", seg, torch.float32, dev)
-        full = _scratch("full", world * seg, torch.float32, dev)
-        views = (local[:3 * vmax].view(vmax, 3), local[3 * vmax:6 * vmax].view(vmax, 3), local[6 * vmax:].view(torch.int32).view(tmax, 3))
-        emit(buf, *shard, nv, nt, v_base, out=views)
-        if net_normals and nv:     # this rank's own vertices, before the gather: a vertex's normal depends on it alone
-            nn, fb = network_normals(eng, model.get_model()._owner[1], views[0][:nv], tiles, views[1][:nv])
-            views[1][:nv].copy_(nn)
-            _report_fallback(fb, nv)
-        tm.mark("mc")
+    v_base = sum(nvs[:rank])
+    vmax, tmax = max(max(nvs), 1), max(max(nts), 1)
+    seg = 3 * (2 * vmax + tmax)                               # floats per rank: vertices | normals | faces (int32 bits)
+    local = alloc(("local", world), seg, torch.float32, dev)
+    views = (local[:3 * vmax].view(vmax, 3), local[3 * vmax:6 * vmax].view(vmax, 3), local[6 * vmax:].view(torch.int32).view(tmax, 3))
+    s = int(getattr(args, "super_sampling", 0) or 0)
+    if s:          # super-sampled vertices: the network is evaluated at the edge samples directly, no extra halo planes
+        lins, fines = mesh.super_sampling_tables(args.limit, res, s)
+        eng.mc_emit_ss(buf, *shard, nv, nt, v_base, s, lins, fines, out=views)
+    else:
+        eng.mc_emit(buf, *shard, nv, nt, v_base, out=views)
+    if getattr(args, "network_normals", False) and nv:
+        nn, fb = mesh.network_normals(eng, model.get_model()._owner[1], views[0][:nv], tiles, views[1][:nv])
+        views[1][:nv].copy_(nn)
+        mesh._report_fallback(fb, nv)
+    tm.mark("mc")
+    v, n, f = views[0][:nv], views[1][:nv], views[2][:nt]
+    if world > 1:
+        full = alloc(("full", world), world * seg, torch.float32, dev)
         dist.all_gather_into_tensor(full, local, group=group)
         full = full.view(world, seg)
         v = torch.cat([full[r, :3 * nvs[r]] for r in range(world)]).view(-1, 3)
         n = torch.cat([full[r, 3 * vmax:3 * vmax + 3 * nvs[r]] for r in range(world)]).view(-1, 3)
         f = torch.cat([full[r, 6 * vmax:6 * vmax + 3 * nts[r]] for r in range(world)]).view(torch.int32).view(-1, 3)
-        tm.mark("gather")
+    tm.mark("gather")
     m = int(getattr(args, "min_component_faces", 0) or 0)
     if m > 0:
-        from .mesh import remove_small_components
-        v, n, f = remove_small_components(eng, v, n, f, m)
+        v, n, f = mesh.remove_small_components(eng, v, n, f, m)
         tm.mark("components")
     tm.finish()
+    return v, f, n, iso, buf
+
+
+def extract_geometry_sharded(model, args, group=None, to_host=True, timings=None, halo="exchange"):
+    """mesh_nerf.extract_geometry (src/mesh_nerf.py:68-92) on N GPUs: the mesh pipeline (_extract_mesh) on this rank's
+    x-slab of the grid, its buffers the grow-only scratch tensors of this module.  Every rank returns the whole mesh, the
+    same arrays as single-GPU mesh.extract_geometry bit for bit: (vertices, triangles, normals, iso), on the host with the
+    vertices rescaled to (-limit, limit) when to_host, otherwise device views that stay valid until the next call (vertices
+    in index coordinates).  Works without a process group (one slab)."""
+    rank, world = _rank_world(group)
+    v, f, n, iso, _ = _extract_mesh(model, args, rank, world, group, _scratch, timings, halo)
     if to_host:
-        v = args.limit * (v.cpu() / (res / 2.0) - 1.0)
-        return v, f.cpu(), n.cpu(), iso
+        return mesh.rescale_vertices(v, args.limit, args.res), f.cpu(), n.cpu(), iso
     return v, f, n, iso

@@ -286,6 +286,37 @@ def test_extract_geometry_on_lego_grid():
 
 
 @pytest.mark.gpu
+def test_extract_geometry_keeps_no_buffers_and_launches_what_one_slab_does():
+    """extract_geometry is the one-slab case of the sharded pipeline, but in buffers that die with the call (it runs inside
+    training processes), and with the kernel launches of the stand-alone stage calls: sweep, statistics, marching cubes."""
+    import nerfmeshes_b200 as nm
+    from conftest import load_npz
+    from test_gpu_parity import LEGO_CFG
+    from nerfmeshes_b200 import parallel as par
+    model = nm.NeRFModel.from_npz(LEGO_CFG, load_npz("weights_lego_nerf.npz")).eval()
+    eng = model._engine()
+
+    class A:
+        limit, res, iso_level = 1.2, 40, 32.0
+
+    def launches(fn):
+        before = eng.launch_count()
+        fn()
+        return eng.launch_count() - before
+
+    par._MESH_BUFFERS.clear()
+    n_single = launches(lambda: nm.extract_geometry(model, "cuda", A))
+    assert not par._MESH_BUFFERS
+    n_slab = launches(lambda: par.extract_geometry_sharded(model, A, group=par.SINGLE, to_host=False))
+    assert par._MESH_BUFFERS and n_single == n_slab > 0
+
+    def stages():
+        density = nm.extract_radiance(model, A, "cuda", A.res, sigma_only=True)
+        eng.marching_cubes(density, float(nm.extract_iso_level(density, A, eng)))
+    assert launches(stages) == n_single
+
+
+@pytest.mark.gpu
 def test_export_marching_cubes_writes_coloured_obj(tmp_path):
     """mesh_nerf.export_marching_cubes (geometry -> view-dependent appearance by ray casting along -normal -> OBJ)."""
     import nerfmeshes_b200 as nm
