@@ -237,6 +237,33 @@ int nm_mesh_components(NmHandle h, const float* verts_dev, const float* normals_
                        int64_t F, int64_t min_faces, float* verts_out_dev, float* normals_out_dev, int32_t* faces_out_dev,
                        int32_t* labels_out_dev_or_null, int64_t* counts_host, void* stream);
 
+/* Sparse density sweep for mesh extraction (no reference counterpart: the reference sweeps the whole grid; these two calls
+ * stand in for the extract_radiance interface, src/mesh_nerf.py:27-53, where resolution should cost in proportion to the
+ * surface; DESIGN §4.10).  Grid and tables as nm_grid_sigma's (host tables of n0 / n1 / n2 entries), the finest network at
+ * the handle's precision, directions = positions; every sigma written equals nm_grid_sigma's at that point bit for bit.
+ * block = B in {4, 8, 16}: block b of an axis covers cells [b*B, min((b+1)*B, n-1)); the lattice is every B-th grid point
+ * of an axis and its last.  Two calls, because the iso level is clamped between them on the host (mesh_nerf.py:56-65):
+ *   nm_sparse_sweep_lattice  writes sigma at the lattice points into vol_dev (n0,n1,n2); stats_host[0..2] = {min, max, std}
+ *                            over the LATTICE points (numpy's, like nm_volume_stats); synchronises.
+ *   nm_sparse_sweep_run      on the same grid, block and volume: blocks whose 8 lattice corners do not agree in
+ *                            sigma > iso are active; every point of an active block's closed point set, dilated by one
+ *                            point and clipped to the grid, is evaluated once; an inactive block with an evaluated point
+ *                            on the other side of iso than its corners becomes active; repeated until no block does.
+ *                            Every point never evaluated is set to +inf (its block's corners are > iso) or -inf.
+ *                            counts_host[0..4] = {lattice points, active blocks, blocks, evaluated points, rounds};
+ *                            synchronises once per round.
+ * Deterministic: the same volume on every run and for every NM_SPARSE_CHUNK_POINTS (points per network launch, default
+ * 4 Mi, read per call).  Argument errors (null pointers, block not in {4, 8, 16}, fewer than 2 points on an axis, 2^31
+ * grid points or more, missing weights, run without its lattice call) are rejected before anything is launched. */
+int nm_sparse_sweep_lattice(NmHandle h, const float* lin0_host, const float* lin1_host, const float* lin2_host, int n0, int n1,
+                            int n2, int block, float* vol_dev, float* stats_host, void* stream);
+int nm_sparse_sweep_run(NmHandle h, const float* lin0_host, const float* lin1_host, const float* lin2_host, int n0, int n1, int n2,
+                        int block, float iso, float* vol_dev, int64_t* counts_host, void* stream);
+/* Test hook: device copies of the last nm_sparse_sweep_run's evaluated mask (n0*n1*ceil(n2/32) words, bit k%32 of word k/32
+ * of grid line (i,j): the marching-cubes sign bit-volume's layout) and block states ((b0,b1,b2) row-major int32, bit 0: the
+ * corners are > iso, bit 1: active); either may be NULL. */
+int nm_debug_sparse_sweep_state(NmHandle h, uint32_t* mask_out_dev_or_null, int32_t* blocks_out_dev_or_null, void* stream);
+
 /* Replaces export_obj (src/nerf/nerf_helpers.py:86-111): `v x y z [r g b]`, `vn x y z`, `f i//i j//j k//k` (1-based) with
  * byte-identical number formatting (python repr of the float32 widened to double).  Host arrays, no GPU involved;
  * diffuse may be NULL or shorter than the vertex list (vertices beyond it get no colour, like the reference's

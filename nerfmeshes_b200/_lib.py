@@ -64,6 +64,9 @@ _SIGNATURES = {
     "nm_chamfer": (C.c_int, [_P, _P, _L, _P, _L, _P, _P]),
     "nm_debug_nearest_brute": (C.c_int, [_P, _P, _L, _P, _L, _P, _P, _P]),
     "nm_mesh_components": (C.c_int, [_P, _P, _P, _L, _P, _L, _L, _P, _P, _P, _P, C.POINTER(C.c_int64), _P]),
+    "nm_sparse_sweep_lattice": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P]),
+    "nm_sparse_sweep_run": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _F, _P, C.POINTER(C.c_int64), _P]),
+    "nm_debug_sparse_sweep_state": (C.c_int, [_P, _P, _P, _P]),
     "nm_export_obj": (C.c_int, [C.c_char_p, _P, _L, _P, _L, _P, _L, _P, _L]),
     "nm_query_host": (C.c_int, [_P, _P, _I, _P, _L, _P, _I, C.c_uint64, C.POINTER(NmRenderOut)]),
     "nm_render_image_host": (C.c_int, [_P, _P, _I, _I, _F, _I, _I, _I, _P, _I, C.c_uint64, C.POINTER(NmRenderOut)]),

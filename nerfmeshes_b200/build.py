@@ -26,6 +26,7 @@ SOURCES = {
     "nm_mc.cu": ["-fmad=false"],
     "nm_chamfer.cu": ["-fmad=false"],
     "nm_components.cu": [],
+    "nm_sparse_sweep.cu": [],
     "nm_train.cu": [],
     "nm_sigma_grad.cu": [],
     "nm_gemm_tc.cu": [],

@@ -67,6 +67,9 @@ struct NmHandle_t {
   Buf ss_tab, ss_ws;               // super-sampled emit: the six coordinate tables; chunk points (M,3) + sigma (M,)
   Buf ms_ws, nn_ws;                // chamfer evaluation: surface sampler (areas, cdf); grid nearest-neighbour search
   Buf cc_ws;                       // small-component removal: labels, sizes, masks and scans (~28 B per vertex + 8 B per face)
+  Buf sp_ws;                       // sparse sweep (nm_sparse_sweep.cu): block flags, two bit-volumes, scans, one chunk of points
+  int sp_grid[4] = {0, 0, 0, 0};   // {n0, n1, n2, block} of the last nm_sparse_sweep_lattice, and the volume it wrote:
+  const float* sp_vol = nullptr;   // what nm_sparse_sweep_run must be called with
   Buf sg_ws;                       // density gradient (nm_sigma_grad): one chunk's forward / chain / tail workspace; grow-only,
                                    // held until nm_destroy (~22 KB per chunk point for the 8x256 network, ~5.8 GB at the default)
   // training (nm_train.cu): gradient accumulators per network + scratch
@@ -80,6 +83,14 @@ namespace {
 // overrides it, read per call (the tests cross chunk boundaries with small values)
 long long ss_chunk_points() {
   const char* e = getenv("NM_SS_CHUNK_POINTS");
+  const long long x = e ? atoll(e) : 0;
+  return x > 0 ? x : (1ll << 22);
+}
+
+// points per network launch of the sparse sweep (20 B of workspace each: 80 MB at 4 Mi); NM_SPARSE_CHUNK_POINTS overrides
+// it, read per call (the tests use values below one round's point list)
+long long sparse_chunk_points() {
+  const char* e = getenv("NM_SPARSE_CHUNK_POINTS");
   const long long x = e ? atoll(e) : 0;
   return x > 0 ? x : (1ll << 22);
 }
@@ -502,7 +513,7 @@ int nm_destroy(NmHandle h) {
   for (int i = 0; i < 2; ++i) { h->g_wt[i].release(); h->g_bias[i].release(); h->g_head[i].release(); h->tr_rgb[i].release(); h->tr_drgb[i].release(); }
   h->train_ws.release(); h->dout.release(); h->trans.release();
   h->ss_tab.release(); h->ss_ws.release(); h->ms_ws.release(); h->nn_ws.release(); h->sg_ws.release();
-  h->cc_ws.release(); h->mc_ws.release(); h->mc_ws2.release();
+  h->cc_ws.release(); h->sp_ws.release(); h->mc_ws.release(); h->mc_ws2.release();
   if (h->h_err) cudaFreeHost(h->h_err);
   cudaFree(h->d_stats);
   for (cudaEvent_t e : h->ev) cudaEventDestroy(e);
@@ -983,6 +994,66 @@ int nm_mesh_components(NmHandle h, const float* verts_dev, const float* normals_
   if (int e = h->cc_ws.ensure(components_ws_bytes(V, F))) return e;
   return mesh_components(verts_dev, normals_dev, V, faces_dev, F, min_faces, verts_out_dev, normals_out_dev, faces_out_dev,
                          labels_out_dev_or_null, counts_host, h->cc_ws.p, h->d_err + 2, (cudaStream_t)stream, &h->launches);
+}
+
+// ---------------------------------------------------------------------------------------------- sparse density sweep
+namespace {
+// Argument checks come before the handle is touched, so a bad call is rejected without a device.
+int sparse_sweep_setup(NmHandle h, const float* lin0, const float* lin1, const float* lin2, int n0, int n1, int n2, int block,
+                       float* vol_dev, const void* out_host, cudaStream_t st, SparseSweep* s) {
+  NM_CHECK(lin0 && lin1 && lin2 && vol_dev && out_host, "sparse sweep: null pointer");
+  NM_CHECK(block == 4 || block == 8 || block == 16, "sparse sweep: block edge %d is not one of 4, 8, 16", block);
+  NM_CHECK(n0 >= 2 && n1 >= 2 && n2 >= 2, "sparse sweep: grid %d x %d x %d has fewer than 2 points on an axis", n0, n1, n2);
+  NM_CHECK((long long)n0 * n1 * n2 < (1ll << 31), "sparse sweep: grid %d x %d x %d has 2^31 points or more", n0, n1, n2);
+  NM_CHECK(h != nullptr, "null handle");
+  if (int e = bind_checked(h)) return e;
+  const int which = h->has_fine ? NM_NET_FINE : NM_NET_COARSE;     // the net nm_grid_sigma sweeps
+  NM_CHECK(h->nets[which].loaded, "sparse sweep: weights of network %d not loaded", which);
+  const float* hs[3] = {lin0, lin1, lin2};
+  const int ns[3] = {n0, n1, n2};
+  for (int i = 0; i < 3; ++i) { if (int e = upload(&h->lin[i], hs[i], sizeof(float) * ns[i])) return e; h->lin_n[i] = ns[i]; }
+  s->n0 = n0; s->n1 = n1; s->n2 = n2; s->block = block;
+  for (int i = 0; i < 3; ++i) s->lin[i] = h->lin[i].as<float>();
+  s->vol = vol_dev;
+  s->chunk_points = sparse_chunk_points();
+  s->eval = [h, which, st](const float* pts, long long M, float* sigma) -> int {
+    MlpInput in{};
+    in.mode = IN_POINTS; in.pts = pts; in.dirs = nullptr; in.M = M;     // directions = positions, as in the grid sweep
+    return run_mlp(h, which, true, in, sigma, st);
+  };
+  return h->sp_ws.ensure(sparse_sweep_ws_bytes(*s));
+}
+}  // namespace
+
+int nm_sparse_sweep_lattice(NmHandle h, const float* lin0_host, const float* lin1_host, const float* lin2_host, int n0, int n1,
+                            int n2, int block, float* vol_dev, float* stats_host, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  SparseSweep s;
+  if (h) h->sp_vol = nullptr;
+  if (int e = sparse_sweep_setup(h, lin0_host, lin1_host, lin2_host, n0, n1, n2, block, vol_dev, stats_host, st, &s)) return e;
+  if (int e = sparse_sweep_lattice(s, h->sp_ws.p, h->d_stats, stats_host, st, &h->launches)) return e;
+  h->sp_grid[0] = n0; h->sp_grid[1] = n1; h->sp_grid[2] = n2; h->sp_grid[3] = block;
+  h->sp_vol = vol_dev;
+  return 0;
+}
+
+int nm_sparse_sweep_run(NmHandle h, const float* lin0_host, const float* lin1_host, const float* lin2_host, int n0, int n1, int n2,
+                        int block, float iso, float* vol_dev, int64_t* counts_host, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  SparseSweep s;
+  if (int e = sparse_sweep_setup(h, lin0_host, lin1_host, lin2_host, n0, n1, n2, block, vol_dev, counts_host, st, &s)) return e;
+  NM_CHECK(h->sp_vol == vol_dev && h->sp_grid[0] == n0 && h->sp_grid[1] == n1 && h->sp_grid[2] == n2 && h->sp_grid[3] == block,
+           "sparse sweep: call nm_sparse_sweep_lattice with the same grid, block and volume first");
+  return sparse_sweep_run(s, iso, h->sp_ws.p, counts_host, h->num_sms, st, &h->launches);
+}
+
+int nm_debug_sparse_sweep_state(NmHandle h, uint32_t* mask_out_dev_or_null, int32_t* blocks_out_dev_or_null, void* stream) {
+  if (int e = bind_device(h)) return e;
+  NM_CHECK(h->sp_vol && h->sp_ws.p, "sparse sweep: no sweep has run on this handle");
+  SparseSweep s;
+  s.n0 = h->sp_grid[0]; s.n1 = h->sp_grid[1]; s.n2 = h->sp_grid[2]; s.block = h->sp_grid[3];
+  s.chunk_points = sparse_chunk_points();
+  return sparse_sweep_state(s, h->sp_ws.p, mask_out_dev_or_null, blocks_out_dev_or_null, (cudaStream_t)stream);
 }
 
 int nm_marching_cubes_count(NmHandle h, const float* vol_dev, int nx, int ny, int nz, float iso, int64_t* counts_host,

@@ -272,4 +272,23 @@ int mesh_components(const float* verts, const float* normals, long long V, const
                     float* verts_out, float* normals_out, int32_t* faces_out, int32_t* labels_out, int64_t* counts_host, void* ws,
                     int* d_err, cudaStream_t st, int64_t* launches);
 
+// sparse density sweep (nm_sparse_sweep.cu, DESIGN §4.10): sigma only in the blocks of `block`^3 cells the iso-surface crosses.
+// lin: device tables (n0 / n1 / n2 entries); vol: the dense (n0,n1,n2) volume; `eval` is the fused MLP, sigma only, on at
+// most chunk_points explicit points per call.  ws: sparse_sweep_ws_bytes(s) bytes of the handle's grow-only workspace.
+struct SparseSweep {
+  int n0 = 0, n1 = 0, n2 = 0, block = 0;
+  const float* lin[3] = {nullptr, nullptr, nullptr};
+  float* vol = nullptr;
+  long long chunk_points = 0;
+  std::function<int(const float* pts, long long M, float* sigma)> eval;
+};
+size_t sparse_sweep_ws_bytes(const SparseSweep& s);
+// sigma at the lattice points into vol; stats_host = {min, max, std} over them (d_stats: 4 doubles of scratch).  Synchronises.
+int sparse_sweep_lattice(const SparseSweep& s, void* ws, double* d_stats, float* stats_host, cudaStream_t st, int64_t* launches);
+// seeds, rounds to the fixpoint, fill, on a volume that holds the lattice values.  counts_host = {lattice points, active
+// blocks, blocks, evaluated points, rounds}.  Synchronises once per round.
+int sparse_sweep_run(const SparseSweep& s, float iso, void* ws, int64_t* counts_host, int num_sms, cudaStream_t st, int64_t* launches);
+// copies of the last run's evaluated mask (n0*n1*ceil(n2/32) words) and block states (bit 0: sign inside, bit 1: active)
+int sparse_sweep_state(const SparseSweep& s, void* ws, uint32_t* mask_out, int32_t* blocks_out, cudaStream_t st);
+
 }  // namespace nm

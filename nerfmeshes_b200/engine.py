@@ -553,6 +553,51 @@ class Engine:
         kv, kf = int(counts[0]), int(counts[1])
         return vo[:kv], no[:kv], fo[:kf], (kv, kf, int(counts[2]), int(counts[3])), labels
 
+    # ------------------------------------------------------------------ sparse density sweep (DESIGN 4.10)
+    def _sparse_args(self, lins, block, out):
+        ls = [np.ascontiguousarray(torch.as_tensor(t).detach().cpu().numpy(), dtype=np.float32) for t in lins]
+        n = tuple(a.size for a in ls)
+        assert out.shape == n and out.is_contiguous() and out.dtype == torch.float32 and out.device == self.device
+        return ls, (self._h, *[a.ctypes.data for a in ls], *n, int(block))
+
+    def sparse_lattice(self, lins, block, out):
+        """Step 1 of the sparse sweep (nm_sparse_sweep_lattice): sigma at the lattice points (every `block`-th grid point of
+        an axis, and its last) into `out` (n0,n1,n2); returns (min, max, std) over the lattice points.  Synchronises."""
+        ls, args = self._sparse_args(lins, block, out)
+        st = (C.c_float * 3)()
+        L.check(self.lib.nm_sparse_sweep_lattice(*args, _ptr(out), st, self._stream()))
+        return float(st[0]), float(st[1]), float(st[2])
+
+    def sparse_run(self, lins, block, iso, out):
+        """Steps 2-5 (nm_sparse_sweep_run) on the volume sparse_lattice wrote: seeds, rounds to the fixpoint, +-inf fill.
+        Returns (lattice points, active blocks, blocks, evaluated points, rounds)."""
+        ls, args = self._sparse_args(lins, block, out)
+        counts = (C.c_int64 * 5)()
+        L.check(self.lib.nm_sparse_sweep_run(*args, float(iso), _ptr(out), counts, self._stream()))
+        return tuple(int(c) for c in counts)
+
+    def sparse_sweep(self, lins, iso_level, block, out):
+        """The sparse counterpart of grid_sigma + volume_stats + clamp_iso_level: fills `out` (n0,n1,n2) with sigma in the
+        blocks of block^3 cells the iso-surface crosses (followed from block to block to a fixpoint) and +-inf elsewhere.
+        The iso level is clamp_iso_level(iso_level, min, max, std) over the LATTICE points: the dense statistics do not
+        exist in this mode.  Returns (iso, counts) with counts as sparse_run's."""
+        from .mesh import clamp_iso_level
+        mn, mx, sd = self.sparse_lattice(lins, block, out)
+        iso = float(clamp_iso_level(iso_level, np.float32(mn), np.float32(mx), np.float32(sd)))
+        return iso, self.sparse_run(lins, block, iso, out)
+
+    def debug_sparse_state(self, shape, block):
+        """Test hook (nm_debug_sparse_sweep_state): the last sparse_run's evaluated mask as a bool tensor of `shape` and its
+        block states (nb0,nb1,nb2) int32 (bit 0: corners > iso, bit 1: active)."""
+        n0, n1, n2 = shape
+        W = (n2 + 31) // 32
+        nb = [(n - 1 + block - 1) // block for n in shape]
+        words = torch.empty((n0, n1, W), dtype=torch.int32, device=self.device)
+        state = torch.empty(nb, dtype=torch.int32, device=self.device)
+        L.check(self.lib.nm_debug_sparse_sweep_state(self._h, _ptr(words), _ptr(state), self._stream()))
+        bits = (words[..., None] >> torch.arange(32, device=self.device, dtype=torch.int32)) & 1
+        return bits.reshape(n0, n1, W * 32)[..., :n2].bool(), state
+
     # ------------------------------------------------------------------ introspection
     def kernel_flags(self):
         out = (C.c_int32 * 2)()

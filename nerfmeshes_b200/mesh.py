@@ -125,7 +125,8 @@ def extract_geometry(model, device, args):
     one-slab case of the mesh pipeline (parallel._extract_mesh, which lists the stages and what args.super_sampling,
     args.network_normals and args.min_component_faces do), in buffers that die with the call.  Everything downstream
     (cache, appearance, OBJ) sees the filtered mesh.  `device` is the reference's argument and unused: the model's engine
-    device is.  Returns CPU (vertices, triangles, normals) and the (res, res, res) numpy density grid."""
+    device is.  Returns CPU (vertices, triangles, normals) and the (res, res, res) numpy density grid; with
+    args.sparse_sweep that grid holds +inf / -inf at the points the sparse sweep did not evaluate."""
     from .parallel import _extract_mesh      # parallel imports this module for the stage helpers above
     fresh = lambda key, numel, dtype, dev: torch.empty(numel, dtype=dtype, device=dev)
     verts, faces, normals, _, density = _extract_mesh(model, args, 0, 1, None, fresh)
@@ -225,7 +226,8 @@ def mesh_appearance(model, vertices, normals, args):
 def cached_geometry(args, build):
     """The mesh cache of export_marching_cubes (src/mesh_nerf.py:141-158): a torch.save'd tuple
     (vertices, triangles, normals, density) at save_dir/cache_name, loaded when --use-cached-mesh is set and the file
-    exists, (re)written when it was requested but missing or --override-cache-mesh is set.  `build()` produces the tuple."""
+    exists, (re)written when it was requested but missing or --override-cache-mesh is set.  `build()` produces the tuple.
+    With args.sparse_sweep the cached density holds +-inf at the points the sparse sweep did not evaluate."""
     import os
     use = bool(getattr(args, "use_cached_mesh", False))
     name = getattr(args, "cache_name", None)

@@ -262,9 +262,16 @@ def _gathered_stats(eng, own, world, group):
 
 def _extract_mesh(model, args, rank, world, group, alloc, timings=None, halo="exchange"):
     """The mesh pipeline, written once: slab `rank` of `world` x-slabs of the grid (SURVEY 8e), one slab being the whole grid.
-      1. sweep: this rank's planes of sigma (fused MLP, grid front-end) into its slab buffer;
+      1. sweep: this rank's planes of sigma (fused MLP, grid front-end) into its slab buffer; with args.sparse_sweep (one
+         slab only, opt-in; DESIGN 4.10) sigma only in the blocks of args.sparse_block^3 cells (4, 8 or 16; default 8) the
+         surface crosses, found from a lattice of every sparse_block-th point and followed from block to block to a
+         fixpoint, and +-inf (the block's side of iso) everywhere else: every vertex, normal and face of that mesh is the
+         dense mesh's bit for bit, and what is missing are whole components of the dense mesh, those that fit between
+         lattice points and touch no block the sweep reached;
       2. halo planes: 3 planes per interior rank by send/recv from the neighbours (`halo="exchange"`), or recomputed;
       3. iso level: min / max / std over the whole grid (every plane is owned exactly once), clamped by mesh.clamp_iso_level;
+         with args.sparse_sweep the statistics are those of the lattice points (the dense ones do not exist; on lego at iso 32 the
+         clamp does not bind from 256^3 up, but a small lattice can clamp the level differently from the dense grid);
       4. marching cubes, count step; the (n_vertices, n_triangles) pairs of all ranks give every rank's index offset;
       5. marching cubes, emit step, straight into this rank's segment [vertices | normals | faces] of the exchange buffer
          (padded to the largest slab); with args.super_sampling = s >= 1 (mesh_nerf.py:95-128) through nm_mc_emit_ss: same
@@ -292,14 +299,24 @@ def _extract_mesh(model, args, rank, world, group, alloc, timings=None, halo="ex
         (lambda a: a[1] - a[0] >= 2)(slab_layout(res, r, world)) for r in range(world))
     # without an exchange the halo planes are recomputed (bit-identical to the owner's); one slab has none
     p0, p1 = (own0, own1) if exchange else (buf0, buf1)
-    eng.grid_sigma(tiles, p0, p1, out=buf[p0 - buf0:p1 - buf0])
+    sparse = bool(getattr(args, "sparse_sweep", False))
+    if sparse and world > 1:
+        raise NotImplementedError("sparse_sweep runs on one slab: the block fixpoint does not cross slab boundaries yet")
+    if sparse:
+        block = int(getattr(args, "sparse_block", 8) or 8)
+        iso, (n_lat, n_act, n_blk, n_eval, rounds) = eng.sparse_sweep(tiles, args.iso_level, block, buf)
+        print(f"sparse sweep (block {block}): {n_act} of {n_blk} blocks active, {n_eval} of {buf.numel()} points evaluated "
+              f"({n_lat} on the lattice), {rounds} rounds")
+    else:
+        eng.grid_sigma(tiles, p0, p1, out=buf[p0 - buf0:p1 - buf0])
     tm.mark("sweep")
     if exchange:
         exchange_halo_planes(buf, res, rank, world, group)
     own = buf[own0 - buf0:own1 - buf0]
     tm.mark("halo")
-    smin, smax, sstd = _gathered_stats(eng, own, world, group) if world > 1 else eng.volume_stats(own)
-    iso = float(mesh.clamp_iso_level(args.iso_level, np.float32(smin), np.float32(smax), np.float32(sstd)))
+    if not sparse:
+        smin, smax, sstd = _gathered_stats(eng, own, world, group) if world > 1 else eng.volume_stats(own)
+        iso = float(mesh.clamp_iso_level(args.iso_level, np.float32(smin), np.float32(smax), np.float32(sstd)))
     tm.mark("stats")
     shard = (iso, buf0, res, own0 - buf0, own1 - buf0)
     nv, nt = eng.mc_count(buf, *shard)
