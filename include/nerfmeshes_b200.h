@@ -237,6 +237,24 @@ int nm_mesh_components(NmHandle h, const float* verts_dev, const float* normals_
                        int64_t F, int64_t min_faces, float* verts_out_dev, float* normals_out_dev, int32_t* faces_out_dev,
                        int32_t* labels_out_dev_or_null, int64_t* counts_host, void* stream);
 
+/* Quadric-error decimation of an indexed mesh (no reference counterpart; DESIGN §4.11): rounds of edge collapses chosen as an
+ * independent set by Garland–Heckbert cost, until at most target_faces faces remain or no collapse is legal.  verts (V,3)
+ * fp32 in index coordinates, normals (V,3), faces (F,3) int32.  Vertices on an open or non-manifold edge, in a face with a
+ * repeated index, or with more than 32 faces are never moved or removed; a collapse must keep the link condition, at most
+ * 32 faces at the survivor, and every surviving face's orientation.  The round that would cross target_faces collapses only
+ * the ceil((F - target)/2) cheapest of its edges, so the result has target or target - 1 faces unless it runs out of legal
+ * collapses first; target_faces >= F copies the input bit for bit.  Outputs are caller-allocated with room for V vertices /
+ * F faces: the surviving vertices in ascending input order, the surviving faces in input order re-indexed, and
+ * source_out (V',) int32 (the input row of every output vertex) unless NULL.  A vertex whose position kept its bits keeps
+ * its input normal; a moved one gets the normalised area-weighted sum of its faces' winding normals.  counts_host =
+ * {V', F', rounds, collapses}; synchronises once and then once per round.  Deterministic: the same bits on every run.
+ * Argument errors (null pointers, negative sizes or target_faces, sizes >= 2^31, 3F >= 2^31) are rejected before anything
+ * is launched; V = F = 0 launches nothing.  A face index outside [0,V) is reported through the device-side error word
+ * (nm_check_flags raises it, once) and the input is copied unchanged. */
+int nm_mesh_decimate(NmHandle h, const float* verts_dev, const float* normals_dev, int64_t V, const int32_t* faces_dev, int64_t F,
+                     int64_t target_faces, float* verts_out_dev, float* normals_out_dev, int32_t* faces_out_dev,
+                     int32_t* source_out_dev_or_null, int64_t* counts_host, void* stream);
+
 /* Sparse density sweep for mesh extraction (no reference counterpart: the reference sweeps the whole grid; these two calls
  * stand in for the extract_radiance interface, src/mesh_nerf.py:27-53, where resolution should cost in proportion to the
  * surface; DESIGN §4.10).  Grid and tables as nm_grid_sigma's (host tables of n0 / n1 / n2 entries), the finest network at

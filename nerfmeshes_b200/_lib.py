@@ -64,6 +64,7 @@ _SIGNATURES = {
     "nm_chamfer": (C.c_int, [_P, _P, _L, _P, _L, _P, _P]),
     "nm_debug_nearest_brute": (C.c_int, [_P, _P, _L, _P, _L, _P, _P, _P]),
     "nm_mesh_components": (C.c_int, [_P, _P, _P, _L, _P, _L, _L, _P, _P, _P, _P, C.POINTER(C.c_int64), _P]),
+    "nm_mesh_decimate": (C.c_int, [_P, _P, _P, _L, _P, _L, _L, _P, _P, _P, _P, C.POINTER(C.c_int64), _P]),
     "nm_sparse_sweep_lattice": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P]),
     "nm_sparse_sweep_run": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _F, _P, C.POINTER(C.c_int64), _P]),
     "nm_debug_sparse_sweep_state": (C.c_int, [_P, _P, _P, _P]),

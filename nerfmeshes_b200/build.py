@@ -26,6 +26,7 @@ SOURCES = {
     "nm_mc.cu": ["-fmad=false"],
     "nm_chamfer.cu": ["-fmad=false"],
     "nm_components.cu": [],
+    "nm_decimate.cu": ["-fmad=false"],       # double arithmetic in the written order: tests/_decimate_ref.py restates it
     "nm_sparse_sweep.cu": [],
     "nm_train.cu": [],
     "nm_sigma_grad.cu": [],

@@ -50,7 +50,8 @@ struct NmHandle_t {
   int lin_n[3] = {0, 0, 0};
   int* d_err = nullptr;       // [0] tensor-core pipeline watchdog code, [1] aabb hit-list overflow, [2] mesh input error
                               // (mesh sampler 1: face index out of range, 2: total area not positive; component filter
-                              // 3: face index out of range; cleared when reported)
+                              // 3: face index out of range; decimation 4: face index out of range; cleared when
+                              // reported)
                               // (device alias of h_err)
   int* h_err = nullptr;       // mapped pinned host memory: still readable after a device-side trap
   double* d_stats = nullptr;
@@ -67,6 +68,8 @@ struct NmHandle_t {
   Buf ss_tab, ss_ws;               // super-sampled emit: the six coordinate tables; chunk points (M,3) + sigma (M,)
   Buf ms_ws, nn_ws;                // chamfer evaluation: surface sampler (areas, cdf); grid nearest-neighbour search
   Buf cc_ws;                       // small-component removal: labels, sizes, masks and scans (~28 B per vertex + 8 B per face)
+  Buf dc_ws;                       // decimation: positions, quadrics, vertex-face lists, candidate edges (~150 B per vertex
+                                   // + 90 B per face)
   Buf sp_ws;                       // sparse sweep (nm_sparse_sweep.cu): block flags, two bit-volumes, scans, one chunk of points
   int sp_grid[4] = {0, 0, 0, 0};   // {n0, n1, n2, block} of the last nm_sparse_sweep_lattice, and the volume it wrote:
   const float* sp_vol = nullptr;   // what nm_sparse_sweep_run must be called with
@@ -146,7 +149,8 @@ int check_kernel_flags(NmHandle h) {
     h->h_err[2] = 0;
     NM_CHECK(false, c == 1   ? "mesh sampler: a face index lies outside [0, V)"
                     : c == 2 ? "mesh sampler: the total face area is not positive and finite"
-                             : "mesh components: a face index lies outside [0, V) (the face was dropped)");
+                    : c == 3 ? "mesh components: a face index lies outside [0, V) (the face was dropped)"
+                             : "mesh decimate: a face index lies outside [0, V) (the mesh was returned unchanged)");
   }
   return 0;
 }
@@ -513,7 +517,7 @@ int nm_destroy(NmHandle h) {
   for (int i = 0; i < 2; ++i) { h->g_wt[i].release(); h->g_bias[i].release(); h->g_head[i].release(); h->tr_rgb[i].release(); h->tr_drgb[i].release(); }
   h->train_ws.release(); h->dout.release(); h->trans.release();
   h->ss_tab.release(); h->ss_ws.release(); h->ms_ws.release(); h->nn_ws.release(); h->sg_ws.release();
-  h->cc_ws.release(); h->sp_ws.release(); h->mc_ws.release(); h->mc_ws2.release();
+  h->cc_ws.release(); h->dc_ws.release(); h->sp_ws.release(); h->mc_ws.release(); h->mc_ws2.release();
   if (h->h_err) cudaFreeHost(h->h_err);
   cudaFree(h->d_stats);
   for (cudaEvent_t e : h->ev) cudaEventDestroy(e);
@@ -994,6 +998,27 @@ int nm_mesh_components(NmHandle h, const float* verts_dev, const float* normals_
   if (int e = h->cc_ws.ensure(components_ws_bytes(V, F))) return e;
   return mesh_components(verts_dev, normals_dev, V, faces_dev, F, min_faces, verts_out_dev, normals_out_dev, faces_out_dev,
                          labels_out_dev_or_null, counts_host, h->cc_ws.p, h->d_err + 2, (cudaStream_t)stream, &h->launches);
+}
+
+// ---------------------------------------------------------------------------------------------- quadric-error decimation
+// Argument checks come before the handle is touched, so a bad call is rejected without a device.
+int nm_mesh_decimate(NmHandle h, const float* verts_dev, const float* normals_dev, int64_t V, const int32_t* faces_dev, int64_t F,
+                     int64_t target_faces, float* verts_out_dev, float* normals_out_dev, int32_t* faces_out_dev,
+                     int32_t* source_out_dev_or_null, int64_t* counts_host, void* stream) {
+  NM_CHECK(V >= 0 && F >= 0, "mesh decimate: negative size (V = %lld, F = %lld)", (long long)V, (long long)F);
+  NM_CHECK(target_faces >= 0, "mesh decimate: negative target_faces %lld", (long long)target_faces);
+  NM_CHECK(V < (1ll << 31) && F < (1ll << 31), "mesh decimate: sizes must be below 2^31");
+  NM_CHECK(3 * F < (1ll << 31), "mesh decimate: 3F = %lld face corners must be below 2^31 (int vertex-face lists)", 3ll * F);
+  NM_CHECK(counts_host, "mesh decimate: null counts pointer");
+  NM_CHECK(V == 0 || (verts_dev && normals_dev && verts_out_dev && normals_out_dev), "mesh decimate: null vertex pointer");
+  NM_CHECK(F == 0 || (faces_dev && faces_out_dev), "mesh decimate: null face pointer");
+  NM_CHECK(h != nullptr, "null handle");
+  for (int i = 0; i < 4; ++i) counts_host[i] = 0;
+  if (V == 0 && F == 0) return 0;
+  if (int e = bind_checked(h)) return e;
+  if (int e = h->dc_ws.ensure(decimate_ws_bytes(V, F))) return e;
+  return mesh_decimate(verts_dev, normals_dev, V, faces_dev, F, target_faces, verts_out_dev, normals_out_dev, faces_out_dev,
+                       source_out_dev_or_null, counts_host, h->dc_ws.p, h->d_err + 2, (cudaStream_t)stream, &h->launches);
 }
 
 // ---------------------------------------------------------------------------------------------- sparse density sweep

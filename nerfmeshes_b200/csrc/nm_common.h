@@ -272,6 +272,14 @@ int mesh_components(const float* verts, const float* normals, long long V, const
                     float* verts_out, float* normals_out, int32_t* faces_out, int32_t* labels_out, int64_t* counts_host, void* ws,
                     int* d_err, cudaStream_t st, int64_t* launches);
 
+// quadric-error decimation (nm_decimate.cu, DESIGN §4.11).  ws: decimate_ws_bytes(V, F) bytes of the handle's grow-only
+// workspace.  A face index outside [0,V) sets *d_err = 4 (device-side, mapped memory) and the input is copied unchanged.
+// counts_host = {output vertices, output faces, rounds, collapses}; synchronises once, then once per round.
+size_t decimate_ws_bytes(long long V, long long F);
+int mesh_decimate(const float* verts, const float* normals, long long V, const int32_t* faces, long long F, long long target,
+                  float* verts_out, float* normals_out, int32_t* faces_out, int32_t* source_out, int64_t* counts_host, void* ws,
+                  int* d_err, cudaStream_t st, int64_t* launches);
+
 // sparse density sweep (nm_sparse_sweep.cu, DESIGN §4.10): sigma only in the blocks of `block`^3 cells the iso-surface crosses.
 // lin: device tables (n0 / n1 / n2 entries); vol: the dense (n0,n1,n2) volume; `eval` is the fused MLP, sigma only, on at
 // most chunk_points explicit points per call.  ws: sparse_sweep_ws_bytes(s) bytes of the handle's grow-only workspace.

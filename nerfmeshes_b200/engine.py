@@ -553,6 +553,29 @@ class Engine:
         kv, kf = int(counts[0]), int(counts[1])
         return vo[:kv], no[:kv], fo[:kf], (kv, kf, int(counts[2]), int(counts[3])), labels
 
+    # ------------------------------------------------------------------ quadric-error decimation (DESIGN 4.11)
+    def mesh_decimate(self, verts, normals, faces, target_faces: int, want_source=False):
+        """Collapse edges of the mesh until at most target_faces faces remain or no collapse is legal (nm_mesh_decimate):
+        (verts (v,3), normals (v,3), faces (f,3) int32, counts, source) with the surviving vertices in input order, faces
+        in input order re-indexed; counts = (v, f, rounds, collapses); source (v,) int32 = the input row of every output
+        vertex when want_source, else None.  Synchronises, and raises if a face index lies outside [0, V)."""
+        v = _f32c(verts, self.device).reshape(-1, 3)
+        n = _f32c(normals, self.device).reshape(-1, 3)
+        f = torch.as_tensor(faces).to(self.device, torch.int32).contiguous().reshape(-1, 3)
+        V, F = v.shape[0], f.shape[0]
+        if n.shape[0] != V:
+            raise L.NmError(f"mesh decimate: {n.shape[0]} normals for {V} vertices")
+        vo, no = torch.empty_like(v), torch.empty_like(n)
+        fo = torch.empty_like(f)
+        source = torch.empty((V,), dtype=torch.int32, device=self.device) if want_source else None
+        counts = (C.c_int64 * 4)()
+        p = lambda t: _ptr(t) if t is not None and t.numel() else None
+        L.check(self.lib.nm_mesh_decimate(self._h, p(v), p(n), V, p(f), F, int(target_faces), p(vo), p(no), p(fo), p(source),
+                                          counts, self._stream()))
+        self.check_flags()
+        kv, kf = int(counts[0]), int(counts[1])
+        return vo[:kv], no[:kv], fo[:kf], (kv, kf, int(counts[2]), int(counts[3])), (source[:kv] if want_source else None)
+
     # ------------------------------------------------------------------ sparse density sweep (DESIGN 4.10)
     def _sparse_args(self, lins, block, out):
         ls = [np.ascontiguousarray(torch.as_tensor(t).detach().cpu().numpy(), dtype=np.float32) for t in lins]

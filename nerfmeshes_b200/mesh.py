@@ -113,6 +113,27 @@ def remove_small_components(eng, verts, normals, faces, m):
     return v, n, f
 
 
+def decimate(eng, verts, normals, faces, target_faces, network=None):
+    """Quadric-error decimation to at most target_faces faces (nm_mesh_decimate, DESIGN 4.11), on index-coordinate
+    vertices.  Surviving vertices stay in input order; an unmoved vertex keeps its normal row, a moved one gets its faces'
+    area-weighted winding normal, or with network = (which, lins) the network's normal at its new position
+    (network_normals).  target_faces <= 0 returns the inputs as they are.  Prints one line."""
+    if target_faces <= 0:
+        return verts, normals, faces
+    F = faces.shape[0]
+    v, n, f, (_, kf, rounds, _), src = eng.mesh_decimate(verts, normals, faces, target_faces, want_source=network is not None)
+    stuck = " (no legal collapse left)" if kf > target_faces else ""
+    print(f"decimated {F} → {kf} faces in {rounds} rounds{stuck}")
+    if network is not None and v.shape[0]:
+        vin = verts.to(v.device)[src.long()]
+        moved = torch.nonzero((v.view(torch.int32) != vin.view(torch.int32)).any(1)).reshape(-1)
+        if moved.numel():
+            nn, fb = network_normals(eng, network[0], v[moved], network[1], n[moved])
+            n[moved] = nn
+            _report_fallback(fb, int(moved.numel()))
+    return v, n, f
+
+
 def rescale_vertices(verts, limit, res):
     """Index coordinates -> (-limit, limit) with the reference's res/2 scale (src/mesh_nerf.py:82-90), on the host like the
     reference's CPU tensors so the rounding is identical (torch's CUDA division by a python scalar multiplies by the
@@ -123,8 +144,8 @@ def rescale_vertices(verts, limit, res):
 def extract_geometry(model, device, args):
     """src/mesh_nerf.py:68-92: sigma sweep -> adaptive iso -> marching cubes -> rescale to (-limit, limit).  This is the
     one-slab case of the mesh pipeline (parallel._extract_mesh, which lists the stages and what args.super_sampling,
-    args.network_normals and args.min_component_faces do), in buffers that die with the call.  Everything downstream
-    (cache, appearance, OBJ) sees the filtered mesh.  `device` is the reference's argument and unused: the model's engine
+    args.network_normals, args.min_component_faces and args.decimate_faces do), in buffers that die with the call.
+    Everything downstream (cache, appearance, OBJ) sees the filtered and decimated mesh.  `device` is the reference's argument and unused: the model's engine
     device is.  Returns CPU (vertices, triangles, normals) and the (res, res, res) numpy density grid; with
     args.sparse_sweep that grid holds +inf / -inf at the points the sparse sweep did not evaluate."""
     from .parallel import _extract_mesh      # parallel imports this module for the stage helpers above

@@ -281,7 +281,10 @@ def _extract_mesh(model, args, rank, world, group, alloc, timings=None, halo="ex
          grid normals with super_sampling >= 1 (vertices on the network's surface) but not at s = 0;
       7. gather: ONE all_gather of the segments leaves the whole mesh on every rank;
       8. args.min_component_faces = m >= 1: components with fewer than m faces (floaters) are removed AFTER the gather
-         (components cross slab boundaries; DESIGN 4.9); every rank filters the identical gathered mesh.
+         (components cross slab boundaries; DESIGN 4.9); every rank filters the identical gathered mesh;
+      9. args.decimate_faces = T >= 1: quadric-error decimation to at most T faces (DESIGN 4.11), after the filter so that
+         no collapse is spent on a floater; every rank decimates the identical mesh, so the result is the single-GPU one.
+         Moved vertices get their faces' winding normal, or with args.network_normals the network's at their new position.
     `world > 1` guards nothing but the collectives (halo exchange, statistics, counts, mesh): with one slab the segment is
     the mesh, the index offset is 0 and the gather is the identity.  A vertex belongs to the rank that owns its grid point,
     and the last owned cell layer addresses the next rank's vertices by the ids that rank assigns (nm_mc_count /
@@ -358,6 +361,11 @@ def _extract_mesh(model, args, rank, world, group, alloc, timings=None, halo="ex
     if m > 0:
         v, n, f = mesh.remove_small_components(eng, v, n, f, m)
         tm.mark("components")
+    T = int(getattr(args, "decimate_faces", 0) or 0)
+    if T > 0:
+        net = (model.get_model()._owner[1], tiles) if getattr(args, "network_normals", False) else None
+        v, n, f = mesh.decimate(eng, v, n, f, T, net)
+        tm.mark("decimate")
     tm.finish()
     return v, f, n, iso, buf
 
