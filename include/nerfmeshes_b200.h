@@ -282,12 +282,50 @@ int nm_sparse_sweep_run(NmHandle h, const float* lin0_host, const float* lin1_ho
  * corners are > iso, bit 1: active); either may be NULL. */
 int nm_debug_sparse_sweep_state(NmHandle h, uint32_t* mask_out_dev_or_null, int32_t* blocks_out_dev_or_null, void* stream);
 
+/* Texture bake of a mesh's appearance (no reference counterpart: the reference colours vertices, src/mesh_nerf.py:160-192;
+ * DESIGN §4.12).  N = texels along a triangle leg, 2 <= N <= 64.  Face f owns one right-triangle patch of K = N(N+1)/2 texels in
+ * half f % 2 of square cell f / 2 of C = N + 2 texels; P = ceil(F/2) cells, Q = the smallest integer with Q^2 >= P cells per
+ * row, a W = Q*C by H = ceil(P/Q)*C atlas (row 0 on top), cell c at pixel ((c % Q)*C, (c / Q)*C).  Half 0 holds texel (i, j),
+ * i + j <= N - 1, at in-cell pixel (i, j) with corners 0, 1, 2 of the face at (0,0), (N-1,0), (0,N-1); half 1 the same patch
+ * at (C-1-i, C-1-j).  Texels are numbered face-major, then row j, then i.
+ * nm_texture_layout: out4 = {Q, rows, W, H}; host only.  Rejects N outside [2, 64], F outside [0, 2^31) and a W or H above
+ * 16384 (naming the largest N that fits).
+ * nm_bake_texture: one appearance query per texel, as mesh_appearance builds one per vertex: with weights w1 = i/(N-1),
+ * w2 = j/(N-1), w0 = (1-w1)-w2 the point p = (w0 v0 + w1 v1) + w2 v2 and normal n = m/|m|, m = (w0 n0 + w1 n1) + w2 n2 (the
+ * corner of largest weight, lowest on ties, where |m| is 0 or not finite), fp32 in that order; corner texels take v_k and n_k
+ * unchanged.  d = -n.  mode 0: a ray from p - view_disparity*d along d through the render path of nm_render_rays with `flags`,
+ * near_far_host and seed 0; mode 1: nm_point_mlp of network `which` at (p, d), rgb columns.  verts / normals (V,3), faces (F,3)
+ * int32; outputs caller-allocated: atlas_f32 (H,W,3) with every texel of a triangle its query's colour, every ring texel
+ * (i + j = N in half 0's coordinates) the mean of its in-triangle 4-neighbours (i-1,j) and (i,j-1) as (a+b)*0.5f or the one
+ * that exists, every other texel 0; atlas_u8 = floorf(clamp(c, 0, 1)*255 + 0.5f); uv (F,3,2) = the centre of each corner
+ * texel, ((x+0.5)/W, 1-(y+0.5)/H); vertex_rgb (V,3) = the corner texel of the lowest (face, corner slot) that references the
+ * vertex, or for a vertex no face references, a query of its own built the same way.  counts_host = {W, H, queries rendered,
+ * vertices without a face}; synchronises once.  Faces are walked in chunks of NM_TEXTURE_CHUNK_TEXELS texels (default 4 Mi,
+ * read per call); the result is the same bits for every chunk size and on every run.  Argument errors (null pointers, N or
+ * atlas out of range, sizes >= 2^31, an unknown mode, NM_FLAG_TEACHER_T) are rejected before anything is launched; V = F = 0
+ * launches nothing.  A face index outside [0,V) is reported through the device-side error word (nm_check_flags raises it,
+ * once) and nothing is baked.
+ * nm_debug_texture_rays: test hook, the queries of faces [f0, f1) (K per face; origins_out = the ray origins in mode 0, the
+ * points in mode 1) and their atlas pixels (x, y) int32 unless pixel_xy_out is NULL. */
+int nm_texture_layout(int64_t F, int N, int64_t* out4);
+int nm_bake_texture(NmHandle h, const float* verts_dev, const float* normals_dev, int64_t V, const int32_t* faces_dev, int64_t F,
+                    int N, int mode, int which, int flags, float view_disparity, const float* near_far_host, float* atlas_f32_dev,
+                    uint8_t* atlas_u8_dev, float* uv_dev, float* vertex_rgb_dev, int64_t* counts_host, void* stream);
+int nm_debug_texture_rays(NmHandle h, const float* verts_dev, const float* normals_dev, int64_t V, const int32_t* faces_dev, int64_t F,
+                          int N, int mode, float view_disparity, int64_t f0, int64_t f1, float* origins_out_dev,
+                          float* dirs_out_dev, int32_t* pixel_xy_out_dev, void* stream);
+
 /* Replaces export_obj (src/nerf/nerf_helpers.py:86-111): `v x y z [r g b]`, `vn x y z`, `f i//i j//j k//k` (1-based) with
  * byte-identical number formatting (python repr of the float32 widened to double).  Host arrays, no GPU involved;
  * diffuse may be NULL or shorter than the vertex list (vertices beyond it get no colour, like the reference's
  * len(diffuse) > idx test). */
 int nm_export_obj(const char* path, const float* verts_host, int64_t n_verts, const int32_t* faces_host, int64_t n_faces,
                   const float* diffuse_host, int64_t n_diffuse, const float* normals_host, int64_t n_normals);
+/* nm_export_obj with a texture: `mtllib <mtl_name>`, the same `v` lines, `vt u v` for uv_host (n_faces,3,2) face-major, the
+ * same `vn` lines, `usemtl texture`, then `f a/t/a b/u/b c/w/c` with t = 3f+k+1. */
+int nm_export_obj_textured(const char* path, const float* verts_host, int64_t n_verts, const int32_t* faces_host, int64_t n_faces,
+                           const float* diffuse_host, int64_t n_diffuse, const float* normals_host, int64_t n_normals,
+                           const float* uv_host, const char* mtl_name);
 
 /* ---- hot path, host buffers (what a reference-side caller holding CPU tensors binds) ------------------ */
 /* model.query(ray_batch) with host tensors (src/eval_nerf.py:62-69): copies H2D, renders, copies D2H, syncs. */

@@ -28,6 +28,7 @@ SOURCES = {
     "nm_components.cu": [],
     "nm_decimate.cu": ["-fmad=false"],       # double arithmetic in the written order: tests/_decimate_ref.py restates it
     "nm_sparse_sweep.cu": [],
+    "nm_texture.cu": ["-fmad=false"],        # fp32 texel positions and rays in the written order: tests/_texture_ref.py
     "nm_train.cu": [],
     "nm_sigma_grad.cu": [],
     "nm_gemm_tc.cu": [],

@@ -50,8 +50,8 @@ struct NmHandle_t {
   int lin_n[3] = {0, 0, 0};
   int* d_err = nullptr;       // [0] tensor-core pipeline watchdog code, [1] aabb hit-list overflow, [2] mesh input error
                               // (mesh sampler 1: face index out of range, 2: total area not positive; component filter
-                              // 3: face index out of range; decimation 4: face index out of range; cleared when
-                              // reported)
+                              // 3: face index out of range; decimation 4: face index out of range; texture bake 5:
+                              // face index out of range; cleared when reported)
                               // (device alias of h_err)
   int* h_err = nullptr;       // mapped pinned host memory: still readable after a device-side trap
   double* d_stats = nullptr;
@@ -70,6 +70,8 @@ struct NmHandle_t {
   Buf cc_ws;                       // small-component removal: labels, sizes, masks and scans (~28 B per vertex + 8 B per face)
   Buf dc_ws;                       // decimation: positions, quadrics, vertex-face lists, candidate edges (~150 B per vertex
                                    // + 90 B per face)
+  Buf tx_ws;                       // texture bake: first references, unreferenced-vertex list, one chunk's queries and colours
+                                   // (~40 B per chunk texel: 160 MB at the default 4 Mi)
   Buf sp_ws;                       // sparse sweep (nm_sparse_sweep.cu): block flags, two bit-volumes, scans, one chunk of points
   int sp_grid[4] = {0, 0, 0, 0};   // {n0, n1, n2, block} of the last nm_sparse_sweep_lattice, and the volume it wrote:
   const float* sp_vol = nullptr;   // what nm_sparse_sweep_run must be called with
@@ -94,6 +96,14 @@ long long ss_chunk_points() {
 // it, read per call (the tests use values below one round's point list)
 long long sparse_chunk_points() {
   const char* e = getenv("NM_SPARSE_CHUNK_POINTS");
+  const long long x = e ? atoll(e) : 0;
+  return x > 0 ? x : (1ll << 22);
+}
+
+// texels per chunk of the texture bake (40 B of workspace each: 160 MB at 4 Mi); NM_TEXTURE_CHUNK_TEXELS overrides it, read
+// per call (the tests cross chunk boundaries with small values)
+long long texture_chunk_texels() {
+  const char* e = getenv("NM_TEXTURE_CHUNK_TEXELS");
   const long long x = e ? atoll(e) : 0;
   return x > 0 ? x : (1ll << 22);
 }
@@ -150,7 +160,8 @@ int check_kernel_flags(NmHandle h) {
     NM_CHECK(false, c == 1   ? "mesh sampler: a face index lies outside [0, V)"
                     : c == 2 ? "mesh sampler: the total face area is not positive and finite"
                     : c == 3 ? "mesh components: a face index lies outside [0, V) (the face was dropped)"
-                             : "mesh decimate: a face index lies outside [0, V) (the mesh was returned unchanged)");
+                    : c == 4 ? "mesh decimate: a face index lies outside [0, V) (the mesh was returned unchanged)"
+                             : "texture bake: a face index lies outside [0, V) (nothing was baked)");
   }
   return 0;
 }
@@ -517,7 +528,7 @@ int nm_destroy(NmHandle h) {
   for (int i = 0; i < 2; ++i) { h->g_wt[i].release(); h->g_bias[i].release(); h->g_head[i].release(); h->tr_rgb[i].release(); h->tr_drgb[i].release(); }
   h->train_ws.release(); h->dout.release(); h->trans.release();
   h->ss_tab.release(); h->ss_ws.release(); h->ms_ws.release(); h->nn_ws.release(); h->sg_ws.release();
-  h->cc_ws.release(); h->dc_ws.release(); h->sp_ws.release(); h->mc_ws.release(); h->mc_ws2.release();
+  h->cc_ws.release(); h->dc_ws.release(); h->sp_ws.release(); h->tx_ws.release(); h->mc_ws.release(); h->mc_ws2.release();
   if (h->h_err) cudaFreeHost(h->h_err);
   cudaFree(h->d_stats);
   for (cudaEvent_t e : h->ev) cudaEventDestroy(e);
@@ -1019,6 +1030,79 @@ int nm_mesh_decimate(NmHandle h, const float* verts_dev, const float* normals_de
   if (int e = h->dc_ws.ensure(decimate_ws_bytes(V, F))) return e;
   return mesh_decimate(verts_dev, normals_dev, V, faces_dev, F, target_faces, verts_out_dev, normals_out_dev, faces_out_dev,
                        source_out_dev_or_null, counts_host, h->dc_ws.p, h->d_err + 2, (cudaStream_t)stream, &h->launches);
+}
+
+// ---------------------------------------------------------------------------------------------- texture bake
+namespace {
+// Argument checks come before the handle is touched, so a bad call is rejected without a device.
+int texture_setup(NmHandle h, const float* verts, const float* normals, int64_t V, const int32_t* faces, int64_t F, int N, int mode,
+                  float view_disparity, TextureBake* b, long long layout[4]) {
+  NM_CHECK(V >= 0 && F >= 0, "texture bake: negative size (V = %lld, F = %lld)", (long long)V, (long long)F);
+  NM_CHECK(V < (1ll << 31) && F < (1ll << 31), "texture bake: sizes must be below 2^31");
+  NM_CHECK(mode == 0 || mode == 1, "texture bake: mode %d is neither 0 (rays) nor 1 (points)", mode);
+  if (int e = texture_layout(F, N, layout)) return e;
+  NM_CHECK(V == 0 || (verts && normals), "texture bake: null vertex pointer");
+  NM_CHECK(F == 0 || faces, "texture bake: null face pointer");
+  b->verts = verts; b->normals = normals; b->V = V; b->faces = faces; b->F = F; b->N = N; b->mode = mode;
+  b->disparity = view_disparity;
+  b->chunk_texels = texture_chunk_texels();
+  return 0;
+}
+}  // namespace
+
+int nm_bake_texture(NmHandle h, const float* verts_dev, const float* normals_dev, int64_t V, const int32_t* faces_dev, int64_t F,
+                    int N, int mode, int which, int flags, float view_disparity, const float* near_far_host, float* atlas_f32_dev,
+                    uint8_t* atlas_u8_dev, float* uv_dev, float* vertex_rgb_dev, int64_t* counts_host, void* stream) {
+  TextureBake b;
+  long long lay[4];
+  if (int e = texture_setup(h, verts_dev, normals_dev, V, faces_dev, F, N, mode, view_disparity, &b, lay)) return e;
+  NM_CHECK(counts_host, "texture bake: null counts pointer");
+  NM_CHECK(V == 0 || vertex_rgb_dev, "texture bake: null vertex colour pointer");
+  NM_CHECK(F == 0 || (atlas_f32_dev && atlas_u8_dev && uv_dev), "texture bake: null atlas or uv pointer");
+  NM_CHECK(mode == 1 || near_far_host, "texture bake: null near/far bounds");
+  NM_CHECK(!(flags & NM_FLAG_TEACHER_T), "texture bake: NM_FLAG_TEACHER_T takes caller samples, which a bake does not have");
+  NM_CHECK(h != nullptr, "null handle");
+  counts_host[0] = lay[2]; counts_host[1] = lay[3]; counts_host[2] = 0; counts_host[3] = 0;
+  if (V == 0 && F == 0) return 0;
+  if (int e = bind_checked(h)) return e;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (mode == 0) {
+    NM_CHECK(h->s_table.p != nullptr, "sampler tables missing");
+    const float nf[2] = {near_far_host[0], near_far_host[1]};
+    b.rgb_stride = 3;
+    b.render = [h, nf, flags, st](const float* o, const float* d, long long n, float* rgb) -> int {
+      NmRenderOut out{};
+      out.rgb = rgb;
+      return render_rays_impl(h, o, 3, d, n, nf, nullptr, nullptr, flags, 0, out, st);     // seed 0: model.query in eval mode
+    };
+  } else {
+    NM_CHECK(which == NM_NET_COARSE || (which == NM_NET_FINE && h->has_fine), "network slot %d not present", which);
+    NM_CHECK(h->nets[which].loaded, "weights of network %d not loaded", which);
+    b.rgb_stride = 4;
+    b.render = [h, which, st](const float* p, const float* d, long long n, float* rgb) -> int {
+      MlpInput in{};
+      in.mode = IN_POINTS; in.pts = p; in.dirs = d; in.M = n;
+      return run_mlp(h, which, false, in, rgb, st);
+    };
+  }
+  if (int e = h->tx_ws.ensure(texture_ws_bytes(b))) return e;
+  return bake_texture(b, atlas_f32_dev, atlas_u8_dev, uv_dev, vertex_rgb_dev, counts_host, h->tx_ws.p, h->d_err + 2, h->h_err + 2,
+                      st, &h->launches);
+}
+
+int nm_debug_texture_rays(NmHandle h, const float* verts_dev, const float* normals_dev, int64_t V, const int32_t* faces_dev, int64_t F,
+                          int N, int mode, float view_disparity, int64_t f0, int64_t f1, float* origins_out_dev,
+                          float* dirs_out_dev, int32_t* pixel_xy_out_dev, void* stream) {
+  TextureBake b;
+  long long lay[4];
+  if (int e = texture_setup(h, verts_dev, normals_dev, V, faces_dev, F, N, mode, view_disparity, &b, lay)) return e;
+  NM_CHECK(0 <= f0 && f0 <= f1 && f1 <= F, "texture bake: face range [%lld, %lld) outside [0, %lld)", (long long)f0, (long long)f1,
+           (long long)F);
+  NM_CHECK(f0 == f1 || (origins_out_dev && dirs_out_dev), "texture bake: null ray output pointer");
+  NM_CHECK(h != nullptr, "null handle");
+  if (f0 == f1) return 0;
+  if (int e = bind_checked(h)) return e;
+  return texture_rays(b, f0, f1, origins_out_dev, dirs_out_dev, pixel_xy_out_dev, h->d_err + 2, (cudaStream_t)stream, &h->launches);
 }
 
 // ---------------------------------------------------------------------------------------------- sparse density sweep

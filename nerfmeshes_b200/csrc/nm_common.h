@@ -299,4 +299,30 @@ int sparse_sweep_run(const SparseSweep& s, float iso, void* ws, int64_t* counts_
 // copies of the last run's evaluated mask (n0*n1*ceil(n2/32) words) and block states (bit 0: sign inside, bit 1: active)
 int sparse_sweep_state(const SparseSweep& s, void* ws, uint32_t* mask_out, int32_t* blocks_out, cudaStream_t st);
 
+// texture bake (nm_texture.cu, DESIGN §4.12): N texels per triangle leg, one right-triangle patch per face, two per cell.
+// out = {Q cells per row, rows, W, H}; rejects N outside [2, 64], F outside [0, 2^31) and an atlas side above 16384.
+constexpr int kTexMinN = 2, kTexMaxN = 64, kTexMaxSide = 16384;
+int texture_layout(long long F, int N, long long out[4]);
+// mode 0: a = ray origins p - c*d for `render` (the handle's render path), mode 1: a = points p for the point MLP; d = -n.
+// `render` writes the colour of ray / point t at rgb[t * rgb_stride + 0..2], for at most chunk_rays(b) of them per call.
+struct TextureBake {
+  const float* verts = nullptr;
+  const float* normals = nullptr;
+  long long V = 0;
+  const int32_t* faces = nullptr;
+  long long F = 0;
+  int N = 0, mode = 0, rgb_stride = 3;
+  float disparity = 0.f;
+  long long chunk_texels = 0;
+  std::function<int(const float* a, const float* d, long long n, float* rgb)> render;
+};
+size_t texture_ws_bytes(const TextureBake& b);
+// the texel queries of faces [f0, f1) (texel-major, K = N(N+1)/2 per face) and their atlas pixels (x, y) unless xy_out is null
+int texture_rays(const TextureBake& b, long long f0, long long f1, float* a_out, float* d_out, int32_t* xy_out, int* d_err,
+                 cudaStream_t st, int64_t* launches);
+// the whole bake; ws: texture_ws_bytes(b) bytes.  A face index outside [0, V) sets *d_err = 5 (device-side, mapped memory;
+// h_err is its host view) and nothing is baked.  counts_host = {W, H, queries rendered, unreferenced vertices}; synchronises once.
+int bake_texture(const TextureBake& b, float* atlas_f32, uint8_t* atlas_u8, float* uv, float* vertex_rgb, int64_t* counts_host,
+                 void* ws, int* d_err, const volatile int* h_err, cudaStream_t st, int64_t* launches);
+
 }  // namespace nm

@@ -73,10 +73,10 @@ char* put_int(long long v, char* out) {
   return out;
 }
 
-}  // namespace
-
-extern "C" int nm_export_obj(const char* path, const float* verts, int64_t n_verts, const int32_t* faces, int64_t n_faces,
-                             const float* diffuse, int64_t n_diffuse, const float* normals, int64_t n_normals) {
+// nm_export_obj's text, or with uv != nullptr its textured variant (include/nerfmeshes_b200.h): the v and vn lines are
+// written by the same code in both
+int write_obj(const char* path, const float* verts, int64_t n_verts, const int32_t* faces, int64_t n_faces, const float* diffuse,
+              int64_t n_diffuse, const float* normals, int64_t n_normals, const float* uv, const char* mtl_name) {
   NM_CHECK(path && (verts || n_verts == 0) && (faces || n_faces == 0) && (normals || n_normals == 0), "null argument");
   FILE* f = fopen(path, "wb");
   NM_CHECK(f != nullptr, "cannot open '%s' for writing", path);
@@ -88,10 +88,18 @@ extern "C" int nm_export_obj(const char* path, const float* verts, int64_t n_ver
   auto triple = [&](const float* a) {
     for (int c = 0; c < 3; ++c) { *p++ = ' '; p = py_repr((double)a[c], p); }
   };
+  auto text = [&](const char* s) { flush(); ok = ok && fputs(s, f) >= 0; };
+  if (uv) { text("mtllib "); text(mtl_name); text("\n"); }
   for (int64_t i = 0; i < n_verts; ++i) {
     *p++ = 'v';
     triple(verts + 3 * i);
     if (diffuse && i < n_diffuse) triple(diffuse + 3 * i);
+    *p++ = '\n';
+    if (p > lim) flush();
+  }
+  for (int64_t i = 0; uv && i < 3 * n_faces; ++i) {
+    *p++ = 'v'; *p++ = 't';
+    for (int c = 0; c < 2; ++c) { *p++ = ' '; p = py_repr((double)uv[2 * i + c], p); }
     *p++ = '\n';
     if (p > lim) flush();
   }
@@ -101,13 +109,16 @@ extern "C" int nm_export_obj(const char* path, const float* verts, int64_t n_ver
     *p++ = '\n';
     if (p > lim) flush();
   }
+  if (uv) text("usemtl texture\n");
   for (int64_t i = 0; i < n_faces; ++i) {
     *p++ = 'f';
     for (int c = 0; c < 3; ++c) {
       const long long idx = (long long)faces[3 * i + c] + 1;
       *p++ = ' ';
       p = put_int(idx, p);
-      *p++ = '/'; *p++ = '/';
+      *p++ = '/';
+      if (uv) p = put_int(3 * i + c + 1, p);
+      *p++ = '/';
       p = put_int(idx, p);
     }
     *p++ = '\n';
@@ -117,4 +128,20 @@ extern "C" int nm_export_obj(const char* path, const float* verts, int64_t n_ver
   ok = (fclose(f) == 0) && ok;
   NM_CHECK(ok, "short write to '%s'", path);
   return 0;
+}
+
+}  // namespace
+
+extern "C" int nm_export_obj(const char* path, const float* verts, int64_t n_verts, const int32_t* faces, int64_t n_faces,
+                             const float* diffuse, int64_t n_diffuse, const float* normals, int64_t n_normals) {
+  return write_obj(path, verts, n_verts, faces, n_faces, diffuse, n_diffuse, normals, n_normals, nullptr, nullptr);
+}
+
+extern "C" int nm_export_obj_textured(const char* path, const float* verts, int64_t n_verts, const int32_t* faces, int64_t n_faces,
+                                      const float* diffuse, int64_t n_diffuse, const float* normals, int64_t n_normals,
+                                      const float* uv, const char* mtl_name) {
+  NM_CHECK(uv || n_faces == 0, "null uv pointer");
+  NM_CHECK(mtl_name && *mtl_name && !strpbrk(mtl_name, "\r\n"), "the material file name must be one non-empty line");
+  static const float kNoUv[2] = {0.f, 0.f};            // a face-less mesh still gets its mtllib / usemtl lines
+  return write_obj(path, verts, n_verts, faces, n_faces, diffuse, n_diffuse, normals, n_normals, uv ? uv : kNoUv, mtl_name);
 }

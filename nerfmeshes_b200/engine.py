@@ -576,6 +576,55 @@ class Engine:
         kv, kf = int(counts[0]), int(counts[1])
         return vo[:kv], no[:kv], fo[:kf], (kv, kf, int(counts[2]), int(counts[3])), (source[:kv] if want_source else None)
 
+    # ------------------------------------------------------------------ texture bake (DESIGN 4.12)
+    @staticmethod
+    def texture_layout(F: int, N: int):
+        """(Q cells per row, rows, W, H) of the texture atlas of F faces at N texels per triangle leg (nm_texture_layout).
+        Raises for N outside [2, 64] or an atlas side above 16384."""
+        out = (C.c_int64 * 4)()
+        L.check(L.load().nm_texture_layout(int(F), int(N), out))
+        return tuple(int(x) for x in out)
+
+    def _texture_mesh(self, verts, normals, faces):
+        v = _f32c(verts, self.device).reshape(-1, 3)
+        n = _f32c(normals, self.device).reshape(-1, 3)
+        f = torch.as_tensor(faces).to(self.device, torch.int32).contiguous().reshape(-1, 3)
+        if n.shape[0] != v.shape[0]:
+            raise L.NmError(f"texture bake: {n.shape[0]} normals for {v.shape[0]} vertices")
+        return v, n, f
+
+    def bake_texture(self, verts, normals, faces, N: int, *, mode=0, which=0, flags=0, view_disparity=0.0, near_far=(0.0, 0.0)):
+        """One appearance query per texel of the atlas (nm_bake_texture): mode 0 a ray from p + view_disparity*n along -n
+        rendered with `flags` and near_far, mode 1 network `which` at (p, -n).  Returns (atlas_u8 (H,W,3) uint8, atlas_f32
+        (H,W,3), uv (F,3,2), vertex_rgb (V,3), counts (W, H, queries, unreferenced vertices)) device tensors.  Synchronises,
+        and raises if a face index lies outside [0, V)."""
+        v, n, f = self._texture_mesh(verts, normals, faces)
+        V, F = v.shape[0], f.shape[0]
+        _, _, W, H = self.texture_layout(F, N)
+        atlas = torch.empty((H, W, 3), dtype=torch.float32, device=self.device)
+        u8 = torch.empty((H, W, 3), dtype=torch.uint8, device=self.device)
+        uv = torch.empty((F, 3, 2), dtype=torch.float32, device=self.device)
+        rgb = torch.empty((V, 3), dtype=torch.float32, device=self.device)
+        counts = (C.c_int64 * 4)()
+        p = lambda t: _ptr(t) if t.numel() else None
+        L.check(self.lib.nm_bake_texture(self._h, p(v), p(n), V, p(f), F, int(N), int(mode), int(which), int(flags),
+                                         float(view_disparity), (C.c_float * 2)(*near_far), p(atlas), p(u8), p(uv), p(rgb),
+                                         counts, self._stream()))
+        self.check_flags()
+        return u8, atlas, uv, rgb, tuple(int(c) for c in counts)
+
+    def debug_texture_rays(self, verts, normals, faces, N: int, f0: int, f1: int, *, mode=0, view_disparity=0.0):
+        """Test hook (nm_debug_texture_rays): the queries of faces [f0, f1), N(N+1)/2 per face: (origins (mode 0) or points
+        (mode 1) (n,3), directions (n,3), atlas pixels (x, y) (n,2) int32)."""
+        v, n, f = self._texture_mesh(verts, normals, faces)
+        m = (int(f1) - int(f0)) * (N * (N + 1) // 2)
+        a = torch.empty((max(m, 0), 3), dtype=torch.float32, device=self.device)
+        d, xy = torch.empty_like(a), torch.empty((max(m, 0), 2), dtype=torch.int32, device=self.device)
+        p = lambda t: _ptr(t) if t.numel() else None
+        L.check(self.lib.nm_debug_texture_rays(self._h, p(v), p(n), v.shape[0], p(f), f.shape[0], int(N), int(mode),
+                                               float(view_disparity), int(f0), int(f1), p(a), p(d), p(xy), self._stream()))
+        return a, d, xy
+
     # ------------------------------------------------------------------ sparse density sweep (DESIGN 4.10)
     def _sparse_args(self, lins, block, out):
         ls = [np.ascontiguousarray(torch.as_tensor(t).detach().cpu().numpy(), dtype=np.float32) for t in lins]

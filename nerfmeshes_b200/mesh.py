@@ -244,6 +244,61 @@ def mesh_appearance(model, vertices, normals, args):
     return model.query((ray_origins.cuda(), directions.cuda(), ray_bounds)).rgb_map.cpu().numpy()
 
 
+def bake_texture(model, vertices, triangles, normals, args):
+    """mesh_appearance per texel instead of per vertex (nm_bake_texture, DESIGN 4.12): args.texture_texels = N texels along
+    each triangle leg, the query of every texel built from its face's barycentric point and normal with mesh_appearance's
+    mode, bounds and disparity.  vertices: world coordinates (what extract_geometry returns and the cache stores).  Returns
+    numpy (atlas_u8 (H,W,3) uint8, uv (F,3,2) float32, diffuse (V,3) float32); diffuse is the colour of each vertex's corner
+    texel, which is mesh_appearance's colour of that vertex bit for bit."""
+    from .models import _cfg_get
+    eng = model._engine()
+    mode = 1 if getattr(args, "no_view_dependence", False) else 0
+    buff = hasattr(model, "tree")
+    if mode == 0 and buff:                        # what BuFFModel.forward does before it renders
+        model._sync_tree(eng)
+        eng.voxel_random = bool(_cfg_get(model.cfg, "tree.use_random_sampling", False))
+    u8, _, uv, rgb, _ = eng.bake_texture(vertices, normals, triangles, int(args.texture_texels), mode=mode,
+                                         which=model.get_model()._owner[1], flags=eng._flags(model.training, buff),
+                                         view_disparity=float(args.view_disparity),
+                                         near_far=(0.0, float(getattr(args, "view_disparity_max_bound", 0.0))))
+    return u8.cpu().numpy(), uv.cpu().numpy(), rgb.cpu().numpy()
+
+
+def write_png(path, rgb):
+    """An 8-bit RGB PNG of rgb (H,W,3) uint8, row 0 on top: every scanline with filter 0, one zlib stream."""
+    import struct
+    import zlib
+    a = np.ascontiguousarray(rgb, dtype=np.uint8)
+    H, W, _ = a.shape
+    raw = np.concatenate([np.zeros((H, 1), np.uint8), a.reshape(H, W * 3)], 1).tobytes()
+
+    def chunk(tag, data):
+        return struct.pack(">I", len(data)) + tag + data + struct.pack(">I", zlib.crc32(tag + data) & 0xFFFFFFFF)
+    with open(path, "wb") as fh:
+        fh.write(b"\x89PNG\r\n\x1a\n" + chunk(b"IHDR", struct.pack(">IIBBBBB", W, H, 8, 2, 0, 0, 0)) +
+                 chunk(b"IDAT", zlib.compress(raw, 6)) + chunk(b"IEND", b""))
+
+
+def export_textured_obj(vertices, triangles, diffuse, normals, uv, atlas_u8, filename):
+    """export_obj with a texture: the OBJ through nm_export_obj_textured (its `v` / `vn` lines are export_obj's bytes for
+    float32 inputs), `<stem>.mtl` naming `<stem>.png`, and the atlas as that PNG.  Returns the three paths."""
+    import ctypes as C
+    import os
+    stem = os.path.splitext(str(filename))[0]
+    base = os.path.basename(stem)
+    arr = lambda a, dt: np.ascontiguousarray(a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a), dtype=dt)
+    v, n, d, t = arr(vertices, np.float32), arr(normals, np.float32), arr(diffuse, np.float32), arr(triangles, np.int32)
+    w = arr(uv, np.float32)
+    assert w.shape == (t.shape[0], 3, 2), (w.shape, t.shape)
+    ptr = lambda a: C.c_void_p(a.ctypes.data) if a.size else None
+    L.check(L.load().nm_export_obj_textured(str(filename).encode(), ptr(v), v.shape[0], ptr(t), t.shape[0], ptr(d),
+                                            d.shape[0] if d.size else 0, ptr(n), n.shape[0], ptr(w), (base + ".mtl").encode()))
+    with open(stem + ".mtl", "w") as fh:
+        fh.write(f"newmtl texture\nKa 1.0 1.0 1.0\nKd 1.0 1.0 1.0\nKs 0.0 0.0 0.0\nillum 1\nmap_Kd {base}.png\n")
+    write_png(stem + ".png", atlas_u8)
+    return str(filename), stem + ".mtl", stem + ".png"
+
+
 def cached_geometry(args, build):
     """The mesh cache of export_marching_cubes (src/mesh_nerf.py:141-158): a torch.save'd tuple
     (vertices, triangles, normals, density) at save_dir/cache_name, loaded when --use-cached-mesh is set and the file
@@ -266,10 +321,18 @@ def export_marching_cubes(model, args, cfg=None, device="cuda"):
     """src/mesh_nerf.py:131-201: geometry (or its cache) -> appearance -> OBJ.  With args.super_sampling >= 1 the geometry
     comes from super-sampled marching cubes (extract_geometry) and the cache stores the refined vertices.  The reference's
     branch would have written a geometry-only OBJ through PyMCubes but raises before it runs, so there is no behaviour to
-    match: the refined mesh goes through the same appearance pass and OBJ writer as s = 0."""
+    match: the refined mesh goes through the same appearance pass and OBJ writer as s = 0.  With args.texture_texels = N > 0
+    the appearance is baked into a texture instead (bake_texture) and the OBJ comes with `<stem>.mtl` and `<stem>.png`; its
+    vertex colours are the ones mesh_appearance would give.  A mesh without faces gets the untextured OBJ."""
     import os
     vertices, triangles, normals, density = cached_geometry(args, lambda: extract_geometry(model, device, args))
-    diffuse = mesh_appearance(model, vertices, normals, args)
     path = os.path.join(args.save_dir, args.mesh_name)
+    if int(getattr(args, "texture_texels", 0) or 0) > 0:
+        if len(triangles):
+            atlas, uv, diffuse = bake_texture(model, vertices, triangles, normals, args)
+            export_textured_obj(vertices, triangles, diffuse, normals, uv, atlas, path)
+            return path
+        print("texture bake: the mesh has no faces; writing the untextured OBJ")
+    diffuse = mesh_appearance(model, vertices, normals, args)
     export_obj(vertices, triangles, diffuse, normals, path)
     return path
