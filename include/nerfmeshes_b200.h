@@ -315,6 +315,30 @@ int nm_debug_texture_rays(NmHandle h, const float* verts_dev, const float* norma
                           int N, int mode, float view_disparity, int64_t f0, int64_t f1, float* origins_out_dev,
                           float* dirs_out_dev, int32_t* pixel_xy_out_dev, void* stream);
 
+/* Mesh rasterizer (no reference counterpart; DESIGN §4.13): an image of a world-coordinate mesh through the pinhole camera of
+ * nm_render_image without NDC (pose_host the 3x4 camera-to-world, H x W pixels, focal), so that mesh pixel (c, r) lies on the
+ * ray NeRF pixel (c, r) renders.  verts (V,3) fp32, faces (F,3) int32.  Corner v goes to camera coordinates p = R^T (v - t),
+ * depth z = -p2 and the screen point X = W/2 + focal p0/z, Y = H/2 - focal p1/z; pixel (c, r) samples the point (c, r).  A
+ * face with a corner at z <= z_near, a non-finite coordinate or |X| or |Y| above 2^20 is culled; both windings are drawn.
+ * Coverage is exact (corners snapped to 1/256 pixel, int64 edge functions, a top-left rule): a sample on an edge two faces
+ * share is covered once.  The nearest face wins by perspective-correct depth, the lower face id on ties.  mode 0: the
+ * perspective-correct interpolation of vertex_rgb (V,3); mode 1: a bilinear lookup in atlas (fp32, the layout of
+ * nm_texture_layout for F faces at N texels per leg, as nm_bake_texture writes it: the caller must pass an atlas of exactly
+ * that H' x W' x 3 for this F and N, which the library cannot check).  Outputs (any may be NULL): rgb (H,W,3),
+ * depth (H,W) = the distance along the pixel's ray (what NeRF's depth map estimates), face (H,W) int32; an uncovered pixel
+ * gets background_host (3 floats), depth 0 and face -1.  counts_host = {covered pixels, faces drawn (not culled), faces
+ * culled}; synchronises once.  Every step is fixed fp32 / integer arithmetic and the depth test an atomicMin of (depth, face)
+ * keys, so the image is the same bits on every run and for every NM_RASTER_BIG_FACE_PIXELS (faces whose bounding box holds at
+ * least that many pixel samples, default 256, read per call, are drawn per screen tile instead of per thread).  Argument
+ * errors (null pointers, H or W outside [1, 16384], focal or z_near not positive and finite, sizes >= 2^31, an unknown mode,
+ * mode 1 with an N nm_texture_layout rejects for F) are rejected before anything is launched; F = 0 launches only the
+ * background fill.  A face index outside [0,V) is never read through; it is reported through the device-side error word
+ * (nm_check_flags raises it, once), and nothing is drawn: every pixel gets the background and the counts are 0. */
+int nm_rasterize_mesh(NmHandle h, const float* verts_dev, int64_t V, const int32_t* faces_dev, int64_t F, const float* pose_host,
+                      int H, int W, float focal, float z_near, int mode, const float* vertex_rgb_dev_or_null,
+                      const float* atlas_dev_or_null, int N, const float* background_host, float* rgb_out_or_null,
+                      float* depth_out_or_null, int32_t* face_out_or_null, int64_t* counts_host, void* stream);
+
 /* Replaces export_obj (src/nerf/nerf_helpers.py:86-111): `v x y z [r g b]`, `vn x y z`, `f i//i j//j k//k` (1-based) with
  * byte-identical number formatting (python repr of the float32 widened to double).  Host arrays, no GPU involved;
  * diffuse may be NULL or shorter than the vertex list (vertices beyond it get no colour, like the reference's

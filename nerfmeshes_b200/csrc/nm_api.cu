@@ -1,6 +1,7 @@
 // C ABI of libnerfmeshes_b200.so (include/nerfmeshes_b200.h): handle lifecycle, weight loading, and the orchestration
 // of the hot path — the body of NeRFModel.forward / BuFFModel.forward (src/models/model_nerf.py:37-78,
 // model_buff.py:34-69) and extract_radiance (src/mesh_nerf.py:27-53) as stream-ordered kernel sequences.
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -51,7 +52,7 @@ struct NmHandle_t {
   int* d_err = nullptr;       // [0] tensor-core pipeline watchdog code, [1] aabb hit-list overflow, [2] mesh input error
                               // (mesh sampler 1: face index out of range, 2: total area not positive; component filter
                               // 3: face index out of range; decimation 4: face index out of range; texture bake 5:
-                              // face index out of range; cleared when reported)
+                              // face index out of range; mesh raster 6: face index out of range; cleared when reported)
                               // (device alias of h_err)
   int* h_err = nullptr;       // mapped pinned host memory: still readable after a device-side trap
   double* d_stats = nullptr;
@@ -72,6 +73,8 @@ struct NmHandle_t {
                                    // + 90 B per face)
   Buf tx_ws;                       // texture bake: first references, unreferenced-vertex list, one chunk's queries and colours
                                    // (~40 B per chunk texel: 160 MB at the default 4 Mi)
+  Buf rs_ws;                       // mesh raster: one depth-and-face key per pixel, one record per face (8 B per pixel + 52 B
+                                   // per face)
   Buf sp_ws;                       // sparse sweep (nm_sparse_sweep.cu): block flags, two bit-volumes, scans, one chunk of points
   int sp_grid[4] = {0, 0, 0, 0};   // {n0, n1, n2, block} of the last nm_sparse_sweep_lattice, and the volume it wrote:
   const float* sp_vol = nullptr;   // what nm_sparse_sweep_run must be called with
@@ -98,6 +101,15 @@ long long sparse_chunk_points() {
   const char* e = getenv("NM_SPARSE_CHUNK_POINTS");
   const long long x = e ? atoll(e) : 0;
   return x > 0 ? x : (1ll << 22);
+}
+
+// faces of the mesh raster whose bounding box holds at least this many pixel samples are drawn one screen tile per CTA
+// instead of one face per thread; NM_RASTER_BIG_FACE_PIXELS overrides it, read per call (the tests use 1, every face on the
+// tile pass, and 2^30, none)
+long long raster_big_face_pixels() {
+  const char* e = getenv("NM_RASTER_BIG_FACE_PIXELS");
+  const long long x = e ? atoll(e) : 0;
+  return x > 0 ? x : 256;
 }
 
 // texels per chunk of the texture bake (40 B of workspace each: 160 MB at 4 Mi); NM_TEXTURE_CHUNK_TEXELS overrides it, read
@@ -161,7 +173,8 @@ int check_kernel_flags(NmHandle h) {
                     : c == 2 ? "mesh sampler: the total face area is not positive and finite"
                     : c == 3 ? "mesh components: a face index lies outside [0, V) (the face was dropped)"
                     : c == 4 ? "mesh decimate: a face index lies outside [0, V) (the mesh was returned unchanged)"
-                             : "texture bake: a face index lies outside [0, V) (nothing was baked)");
+                    : c == 5 ? "texture bake: a face index lies outside [0, V) (nothing was baked)"
+                             : "mesh raster: a face index lies outside [0, V) (nothing was drawn)");
   }
   return 0;
 }
@@ -528,7 +541,7 @@ int nm_destroy(NmHandle h) {
   for (int i = 0; i < 2; ++i) { h->g_wt[i].release(); h->g_bias[i].release(); h->g_head[i].release(); h->tr_rgb[i].release(); h->tr_drgb[i].release(); }
   h->train_ws.release(); h->dout.release(); h->trans.release();
   h->ss_tab.release(); h->ss_ws.release(); h->ms_ws.release(); h->nn_ws.release(); h->sg_ws.release();
-  h->cc_ws.release(); h->dc_ws.release(); h->sp_ws.release(); h->tx_ws.release(); h->mc_ws.release(); h->mc_ws2.release();
+  h->cc_ws.release(); h->dc_ws.release(); h->sp_ws.release(); h->tx_ws.release(); h->rs_ws.release(); h->mc_ws.release(); h->mc_ws2.release();
   if (h->h_err) cudaFreeHost(h->h_err);
   cudaFree(h->d_stats);
   for (cudaEvent_t e : h->ev) cudaEventDestroy(e);
@@ -1103,6 +1116,42 @@ int nm_debug_texture_rays(NmHandle h, const float* verts_dev, const float* norma
   if (f0 == f1) return 0;
   if (int e = bind_checked(h)) return e;
   return texture_rays(b, f0, f1, origins_out_dev, dirs_out_dev, pixel_xy_out_dev, h->d_err + 2, (cudaStream_t)stream, &h->launches);
+}
+
+// ---------------------------------------------------------------------------------------------- mesh raster
+// Argument checks come before the handle is touched, so a bad call is rejected without a device.
+int nm_rasterize_mesh(NmHandle h, const float* verts_dev, int64_t V, const int32_t* faces_dev, int64_t F, const float* pose_host,
+                      int H, int W, float focal, float z_near, int mode, const float* vertex_rgb_dev_or_null,
+                      const float* atlas_dev_or_null, int N, const float* background_host, float* rgb_out_or_null,
+                      float* depth_out_or_null, int32_t* face_out_or_null, int64_t* counts_host, void* stream) {
+  NM_CHECK(V >= 0 && F >= 0, "mesh raster: negative size (V = %lld, F = %lld)", (long long)V, (long long)F);
+  NM_CHECK(V < (1ll << 31) && F < (1ll << 31), "mesh raster: sizes must be below 2^31");
+  NM_CHECK(pose_host && background_host && counts_host, "mesh raster: null pose, background or counts pointer");
+  NM_CHECK(H >= 1 && H <= 16384 && W >= 1 && W <= 16384, "mesh raster: image %d x %d outside [1, 16384]", H, W);
+  NM_CHECK(focal > 0.f && std::isfinite(focal), "mesh raster: focal length %g is not positive and finite", (double)focal);
+  NM_CHECK(z_near > 0.f && std::isfinite(z_near), "mesh raster: z_near %g is not positive and finite", (double)z_near);
+  NM_CHECK(mode == 0 || mode == 1, "mesh raster: mode %d is neither 0 (vertex colours) nor 1 (texture atlas)", mode);
+  if (mode == 1) {
+    long long lay[4];
+    if (int e = texture_layout(F, N, lay)) return e;
+  }
+  NM_CHECK(V == 0 || verts_dev, "mesh raster: null vertex pointer");
+  NM_CHECK(F == 0 || faces_dev, "mesh raster: null face pointer");
+  NM_CHECK(!rgb_out_or_null || mode == 1 || V == 0 || vertex_rgb_dev_or_null, "mesh raster: null vertex colour pointer");
+  NM_CHECK(!rgb_out_or_null || mode == 0 || F == 0 || atlas_dev_or_null, "mesh raster: null atlas pointer");
+  NM_CHECK(h != nullptr, "null handle");
+  counts_host[0] = counts_host[1] = counts_host[2] = 0;
+  if (int e = bind_checked(h)) return e;
+  RasterMesh m;
+  m.verts = verts_dev; m.V = V; m.faces = faces_dev; m.F = F;
+  memcpy(m.pose, pose_host, sizeof(m.pose));
+  m.H = H; m.W = W; m.focal = focal; m.z_near = z_near; m.mode = mode; m.N = N;
+  m.vertex_rgb = vertex_rgb_dev_or_null; m.atlas = atlas_dev_or_null;
+  for (int k = 0; k < 3; ++k) m.bg[k] = background_host[k];
+  m.rgb = rgb_out_or_null; m.depth = depth_out_or_null; m.face = face_out_or_null;
+  m.big_pixels = raster_big_face_pixels();
+  if (int e = h->rs_ws.ensure(raster_ws_bytes(m))) return e;
+  return rasterize_mesh(m, counts_host, h->rs_ws.p, h->d_err + 2, (cudaStream_t)stream, &h->launches);
 }
 
 // ---------------------------------------------------------------------------------------------- sparse density sweep

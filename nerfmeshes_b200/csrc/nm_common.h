@@ -325,4 +325,29 @@ int texture_rays(const TextureBake& b, long long f0, long long f1, float* a_out,
 int bake_texture(const TextureBake& b, float* atlas_f32, uint8_t* atlas_u8, float* uv, float* vertex_rgb, int64_t* counts_host,
                  void* ws, int* d_err, const volatile int* h_err, cudaStream_t st, int64_t* launches);
 
+// mesh rasterizer (nm_raster.cu, DESIGN §4.13): world-coordinate triangles through nm_render_image's pinhole camera.  mode 0
+// colours by vertex_rgb (V,3), mode 1 by the §4.12 atlas of N texels per leg; any output may be null.  A face whose bounding
+// box holds >= big_pixels pixel samples is drawn by the tile pass (the same bits either way).
+struct RasterMesh {
+  const float* verts = nullptr;
+  long long V = 0;
+  const int32_t* faces = nullptr;
+  long long F = 0;
+  float pose[12] = {};
+  int H = 0, W = 0;
+  float focal = 0.f, z_near = 0.f;
+  int mode = 0, N = 0;
+  const float* vertex_rgb = nullptr;
+  const float* atlas = nullptr;
+  float bg[3] = {0.f, 0.f, 0.f};
+  float* rgb = nullptr;
+  float* depth = nullptr;
+  int32_t* face = nullptr;
+  long long big_pixels = 0;
+};
+size_t raster_ws_bytes(const RasterMesh& m);
+// ws: raster_ws_bytes(m) bytes.  A face index outside [0, V) sets *d_err = 6 (device-side, mapped memory) and nothing is
+// drawn: every pixel gets the background.  counts_host = {covered pixels, faces drawn, faces culled}; synchronises once.
+int rasterize_mesh(const RasterMesh& m, int64_t* counts_host, void* ws, int* d_err, cudaStream_t st, int64_t* launches);
+
 }  // namespace nm

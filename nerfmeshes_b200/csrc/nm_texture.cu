@@ -13,6 +13,7 @@
 #include <cmath>
 
 #include "nm_common.h"
+#include "nm_texture.cuh"
 
 namespace nm {
 namespace {
@@ -24,25 +25,11 @@ constexpr int kNoRef = 0x7f7f7f7f;    // vfirst of a vertex no face references (
 unsigned blocks_for(long long n) { return (unsigned)((n + kBlock - 1) / kBlock); }
 size_t align_up(size_t x) { return (x + 255) & ~(size_t)255; }
 
-struct TexLayout {
-  int N, C, K;
-  long long Q, W;
-};
-
 // local texel index r in [0, K) -> (i, j): row j holds N - j texels
 __device__ __forceinline__ void texel_ij(int r, int N, int* i, int* j) {
   int jj = 0;
   while (r >= N - jj) { r -= N - jj; ++jj; }
   *i = r; *j = jj;
-}
-
-// atlas pixel of texel (i, j) of face f: half 0 at (i, j) in its cell, half 1 point-mirrored through the cell
-__device__ __forceinline__ long long texel_pixel(long long f, int i, int j, const TexLayout& L) {
-  const long long c = f >> 1;
-  const long long x0 = (c % L.Q) * L.C, y0 = (c / L.Q) * L.C;
-  const bool h1 = f & 1;
-  const long long x = x0 + (h1 ? L.C - 1 - i : i), y = y0 + (h1 ? L.C - 1 - j : j);
-  return y * L.W + x;
 }
 
 // corner k of the patch, or -1: (0,0), (N-1,0), (0,N-1)
@@ -194,10 +181,10 @@ __global__ void __launch_bounds__(kBlock) tex_uv_kernel(long long F, TexLayout L
   uv[2 * t + 1] = 1.0f - ((float)(px / L.W) + 0.5f) / (float)H;
 }
 
-TexLayout tex_layout(const TextureBake& b) {
-  long long lay[4];
-  texture_layout(b.F, b.N, lay);
-  return TexLayout{b.N, b.N + 2, b.N * (b.N + 1) / 2, lay[0], lay[2]};
+TexLayout bake_layout(const TextureBake& b) {
+  TexLayout L{};
+  nm::tex_layout(b.F, b.N, &L);
+  return L;
 }
 
 // rays per chunk: whole faces of chunk_texels texels (at least one face), no more than the mesh needs
@@ -261,7 +248,7 @@ size_t texture_ws_bytes(const TextureBake& b) {
 
 int texture_rays(const TextureBake& b, long long f0, long long f1, float* a_out, float* d_out, int32_t* xy_out, int* d_err,
                  cudaStream_t st, int64_t* launches) {
-  const TexLayout L = tex_layout(b);
+  const TexLayout L = bake_layout(b);
   const long long n = (f1 - f0) * L.K;
   if (n == 0) return 0;
   tex_rays_kernel<<<blocks_for(n), kBlock, 0, st>>>(b.verts, b.normals, b.V, b.faces, f0, n, L, b.mode, b.disparity, a_out, d_out,
@@ -273,7 +260,7 @@ int texture_rays(const TextureBake& b, long long f0, long long f1, float* a_out,
 
 int bake_texture(const TextureBake& b, float* atlas_f32, uint8_t* atlas_u8, float* uv, float* vertex_rgb, int64_t* counts_host,
                  void* ws, int* d_err, const volatile int* h_err, cudaStream_t st, int64_t* launches) {
-  const TexLayout L = tex_layout(b);
+  const TexLayout L = bake_layout(b);
   long long lay[4];
   if (int e = texture_layout(b.F, b.N, lay)) return e;
   const long long V = b.V, F = b.F, R = chunk_rays(b), H = lay[3];

@@ -57,6 +57,15 @@ def _f32c(t, device=None) -> torch.Tensor:
     return t.detach().to(torch.float32).contiguous()
 
 
+def raster_faces(faces, device) -> torch.Tensor:
+    """(F,3) int32 faces on `device` for nm_rasterize_mesh.  A wider index outside int32 would wrap to another vertex in the
+    cast, so it is reported here with the message the library gives an index outside [0, V)."""
+    f = torch.as_tensor(faces)
+    if f.dtype != torch.int32 and f.numel() and (int(f.min()) < -2 ** 31 or int(f.max()) >= 2 ** 31):
+        raise L.NmError("mesh raster: a face index lies outside [0, V) (nothing was drawn)")
+    return f.to(device, torch.int32).contiguous().reshape(-1, 3)
+
+
 class Engine:
     """Owns one library handle on one CUDA device."""
 
@@ -624,6 +633,45 @@ class Engine:
         L.check(self.lib.nm_debug_texture_rays(self._h, p(v), p(n), v.shape[0], p(f), f.shape[0], int(N), int(mode),
                                                float(view_disparity), int(f0), int(f1), p(a), p(d), p(xy), self._stream()))
         return a, d, xy
+
+    # ------------------------------------------------------------------ mesh raster (DESIGN 4.13)
+    def rasterize_mesh(self, verts, faces, pose, H: int, W: int, focal: float, *, colors=None, atlas=None, N: int = 0,
+                       z_near: float = 1e-3, background=(0.0, 0.0, 0.0), want=("rgb", "depth", "face")):
+        """An image of the world-coordinate mesh verts (V,3) / faces (F,3) through render_image's camera (nm_rasterize_mesh):
+        mode 0 with colors (V,3), mode 1 with a floating-point atlas of N texels per leg in nm_bake_texture's layout for these
+        F faces (texture_layout(F, N): (H', W', 3) with W', H' its width and height; a uint8 atlas goes through
+        mesh.render_mesh, which scales it by 1/255).  Returns ({"rgb": (H,W,3), "depth": (H,W) ray distance, "face": (H,W)
+        int32} for the keys in `want`, (covered pixels, faces drawn, faces culled)).  Uncovered pixels hold the background,
+        depth 0 and face -1.  Synchronises, and raises if a face index lies outside [0, V) or the atlas does not fit the mesh."""
+        v = _f32c(verts, self.device).reshape(-1, 3)
+        f = raster_faces(faces, self.device)
+        p = np.ascontiguousarray(torch.as_tensor(pose).detach().cpu().numpy()[:3, :4], dtype=np.float32)
+        mode = 1 if atlas is not None else 0
+        col = None if colors is None else _f32c(colors, self.device).reshape(-1, 3)
+        if col is not None and col.shape[0] != v.shape[0]:
+            raise L.NmError(f"mesh raster: {col.shape[0]} colours for {v.shape[0]} vertices")
+        tex = None
+        if atlas is not None:
+            a = torch.as_tensor(atlas)
+            if not a.dtype.is_floating_point:
+                raise L.NmError(f"mesh raster: a {a.dtype} atlas; pass colours in [0, 1] as floats (mesh.render_mesh scales a "
+                                "uint8 atlas by 1/255)")
+            _, _, aw, ah = self.texture_layout(f.shape[0], N)       # raises for an N the layout rejects
+            if f.shape[0] and tuple(a.shape) != (ah, aw, 3):
+                raise L.NmError(f"mesh raster: a {tuple(a.shape)} atlas does not fit {f.shape[0]} faces at N = {N}, which need "
+                                f"({ah}, {aw}, 3): was it baked for another mesh or another N?")
+            tex = _f32c(a, self.device)
+        shapes = dict(rgb=((H, W, 3), torch.float32), depth=((H, W), torch.float32), face=((H, W), torch.int32))
+        outs = {k: torch.empty(shapes[k][0], dtype=shapes[k][1], device=self.device) for k in want}
+        bg = (C.c_float * 3)(*[float(x) for x in background])
+        counts = (C.c_int64 * 3)()
+        ptr = lambda t: _ptr(t) if t is not None and t.numel() else None
+        L.check(self.lib.nm_rasterize_mesh(self._h, ptr(v), v.shape[0], ptr(f), f.shape[0], p.ctypes.data, int(H), int(W),
+                                           float(focal), float(z_near), mode, ptr(col), ptr(tex), int(N), bg,
+                                           ptr(outs.get("rgb")), ptr(outs.get("depth")), ptr(outs.get("face")), counts,
+                                           self._stream()))
+        self.check_flags()
+        return outs, tuple(int(c) for c in counts)
 
     # ------------------------------------------------------------------ sparse density sweep (DESIGN 4.10)
     def _sparse_args(self, lins, block, out):

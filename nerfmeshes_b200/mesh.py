@@ -299,6 +299,87 @@ def export_textured_obj(vertices, triangles, diffuse, normals, uv, atlas_u8, fil
     return str(filename), stem + ".mtl", stem + ".png"
 
 
+def _raster_inputs(eng, vertices, triangles, diffuse, texture):
+    """The mesh and its colouring on the engine's device, once: vertices fp32, faces int32, colours fp32, and the atlas in fp32
+    (a uint8 atlas, as bake_texture returns it, divided by 255 on the device)."""
+    if (diffuse is None) == (texture is None):
+        raise ValueError("render_mesh needs exactly one of diffuse= and texture=")
+    from .engine import raster_faces
+    v = torch.as_tensor(vertices).to(eng.device, torch.float32).contiguous()
+    f = raster_faces(triangles, eng.device)
+    col = None if diffuse is None else torch.as_tensor(diffuse).to(eng.device, torch.float32).contiguous()
+    atlas, N = (None, 0) if texture is None else texture
+    if atlas is not None:
+        atlas = torch.as_tensor(atlas).to(eng.device)
+        atlas = atlas.to(torch.float32) / 255.0 if atlas.dtype == torch.uint8 else atlas.to(torch.float32)
+    return v, f, col, atlas, int(N)
+
+
+def render_mesh(model_or_engine, vertices, triangles, pose, H, W, focal, *, diffuse=None, texture=None, background=(0.0, 0.0, 0.0)):
+    """An image of the mesh from a camera pose (nm_rasterize_mesh, DESIGN 4.13), through the pinhole camera render_image uses
+    without NDC, so that pixel (c, r) lies on the ray NeRF pixel (c, r) renders.  vertices: world coordinates (what
+    extract_geometry returns and the cache stores); colours from diffuse (V,3) (mesh_appearance's output) or texture =
+    (atlas, N) (bake_texture's atlas of these faces, uint8 or float).  Returns {"rgb": (H,W,3), "depth": (H,W) distance along
+    the ray, "face": (H,W) int32, -1 where the mesh is not seen, "counts": (covered pixels, faces drawn, faces culled)}, device
+    tensors."""
+    from .engine import Engine
+    eng = model_or_engine if isinstance(model_or_engine, Engine) else model_or_engine._engine()
+    v, f, col, atlas, N = _raster_inputs(eng, vertices, triangles, diffuse, texture)
+    outs, counts = eng.rasterize_mesh(v, f, pose, int(H), int(W), float(focal), colors=col, atlas=atlas, N=N, background=background)
+    outs["counts"] = counts
+    return outs
+
+
+def _psnr(mse):
+    return float("inf") if mse == 0 else -10.0 * float(np.log10(mse))
+
+
+def compare_with_nerf(model, vertices, triangles, poses, H, W, focal, near, far, *, diffuse=None, texture=None):
+    """Score a mesh against the NeRF it came from, view by view: for each pose the NeRF image (render_image) and the mesh image
+    (render_mesh) on the same background (white when the model's config asks for it, else black).  Per view: PSNR of the mesh
+    image against the NeRF image over all pixels; PSNR over the pixels both cover (mesh face != -1 and NeRF acc > 0.5);
+    silhouette IoU of the mesh's coverage against acc > 0.5; mean |depth difference| over the pixels both cover, against the
+    NeRF's expected hit distance depth_raw / acc; and the number of pixels both cover.  A view where no pixel is covered by
+    both has NaN for the masked values.  Returns {"psnr", "psnr_masked", "iou", "depth_mae", "both": per-view lists, "mean":
+    the means over the views where a value exists}.  NDC scenes raise NotImplementedError."""
+    from .models import _cfg_get
+    if _cfg_get(model.cfg, "dataset.use_ndc", False):
+        raise NotImplementedError("compare_with_nerf: the scene uses NDC rays, so its mesh lives in NDC space; mapping it back "
+                                  "to world space is not implemented")
+    eng = model._engine()
+    buff = hasattr(model, "tree")
+    if buff:                                           # what BuFFModel.forward does before it renders
+        model._sync_tree(eng)
+        eng.voxel_random = bool(_cfg_get(model.cfg, "tree.use_random_sampling", False))
+    bg = (1.0, 1.0, 1.0) if model.volume_renderer.white_background else (0.0, 0.0, 0.0)
+    v, f, col, atlas, N = _raster_inputs(eng, vertices, triangles, diffuse, texture)
+    out = dict(psnr=[], psnr_masked=[], iou=[], depth_mae=[], both=[])
+    for pose in poses:
+        n = eng.render_image(pose, H, W, focal, near, far, buff=buff, want=("rgb", "depth_raw", "acc"))
+        m, _ = eng.rasterize_mesh(v, f, pose, int(H), int(W), float(focal), colors=col, atlas=atlas, N=N, background=bg)
+        n_rgb, acc = n["rgb"].view(H, W, 3).double(), n["acc"].view(H, W)
+        m_rgb = m["rgb"].double()
+        mesh_in, nerf_in = m["face"] >= 0, acc > 0.5
+        both, union = mesh_in & nerf_in, mesh_in | nerf_in
+        err2 = (m_rgb - n_rgb) ** 2
+        out["psnr"].append(_psnr(float(err2.mean())))
+        nb = int(both.sum())
+        out["both"].append(nb)
+        out["psnr_masked"].append(_psnr(float(err2[both].mean())) if nb else float("nan"))
+        nu = int(union.sum())
+        out["iou"].append(nb / nu if nu else float("nan"))
+        nerf_depth = n["depth_raw"].view(H, W).double() / acc.double()
+        out["depth_mae"].append(float((m["depth"].double() - nerf_depth)[both].abs().mean()) if nb else float("nan"))
+    out["mean"] = {k: _mean_defined(v_) for k, v_ in out.items()}
+    return out
+
+
+def _mean_defined(xs):
+    """The mean of the values that are not NaN, or NaN when none is."""
+    xs = [x for x in xs if not np.isnan(x)]
+    return float(np.mean(xs)) if xs else float("nan")
+
+
 def cached_geometry(args, build):
     """The mesh cache of export_marching_cubes (src/mesh_nerf.py:141-158): a torch.save'd tuple
     (vertices, triangles, normals, density) at save_dir/cache_name, loaded when --use-cached-mesh is set and the file
