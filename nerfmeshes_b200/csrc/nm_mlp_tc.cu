@@ -84,8 +84,9 @@ struct TcParams {
 static_assert(sizeof(TcParams) <= 4096, "TcParams must fit the 4 KB kernel-parameter window");
 
 // NM_MLP_STALLS=1 (diagnostic build: NM_NVCC_EXTRA=-DNM_MLP_STALLS=1): thread 0 of each consumer warpgroup splits its
-// clock64() time into weight-ring full waits, the MMA main loop (its waits excluded) and the rest (encodings, epilogues,
-// compositor), and the first two and the last CTA of a launch printf the totals at exit.  The counters live in shared
+// clock64() time into weight-ring full waits, the MMA main loop (its waits excluded), the encodings, the layer epilogues
+// (from the end of the MMA loop, so including the first barrier's wait for the other warps' last MMAs), the compositor and
+// the rest, and the first two and the last CTA of a launch printf the totals at exit.  The counters live in shared
 // memory after the barriers to keep register pressure down; the instrumented kernel still spills more than the shipped
 // one, so its split is approximate.
 #ifndef NM_MLP_STALLS
@@ -97,8 +98,9 @@ static_assert(sizeof(TcParams) <= 4096, "TcParams must fit the 4 KB kernel-param
 #define NM_ST(...)
 #endif
 
-// barrier slots (8 B each) relative to off_bars (+ the NM_MLP_STALLS counters: wait, mma, start per warpgroup)
-constexpr uint32_t kBarWFull = 0, kBarWEmpty = 64, kBarStalls = 128, kBarBytes = 128 + (NM_MLP_STALLS ? 64 : 0);
+// barrier slots (8 B each) relative to off_bars (+ the NM_MLP_STALLS counters, 8 per warpgroup: wait, mma, start, encoding,
+// epilogue, compositor)
+constexpr uint32_t kBarWFull = 0, kBarWEmpty = 64, kBarStalls = 128, kBarBytes = 128 + (NM_MLP_STALLS ? 128 : 0);
 
 enum : int { ERR_ALIGN = 1, ERR_W_EMPTY = 2, ERR_W_FULL = 3 };
 
@@ -220,11 +222,12 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
   int slot = 0;
   uint32_t ph = 0;
   float acc[128];
-  NM_ST(volatile long long* const st = reinterpret_cast<volatile long long*>(smem + P.off_bars + kBarStalls) + 4 * wg;
-        if (t == 0) { st[0] = 0; st[1] = 0; st[2] = clock64(); })
+  NM_ST(volatile long long* const st = reinterpret_cast<volatile long long*>(smem + P.off_bars + kBarStalls) + 8 * wg;
+        if (t == 0) { st[0] = 0; st[1] = 0; st[2] = clock64(); st[3] = 0; st[4] = 0; st[5] = 0; })
 
   // encoding of this tile's points (xyz or view direction) -> the encoding buffer, columns past the width zeroed
   auto encode = [&](long long tile, bool dir) {
+    NM_ST(const long long c0 = clock64();)
     ptx::named_bar_sync(bar_id, 128);          // every wgmma of the warpgroup that read the buffer has completed
     if (t < 64) {
       long long m = tile * kTileM + t;
@@ -249,6 +252,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
     }
     ptx::fence_proxy_async_smem();
     ptx::named_bar_sync(bar_id, 128);
+    NM_ST(if (t == 0) st[3] += clock64() - c0;)
   };
 
   // Fused compositor on tile `itp` of this warpgroup, whose last layer is staged in shared memory.  Same arithmetic, in the
@@ -443,6 +447,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
         }
       }
       // ------------------------------------------------------------ epilogue, straight from the accumulator fragments
+      NM_ST(const long long ce = clock64();)
       const int NC = L.n_out >> 6;
       const bool writes_a = (L.kind == KIND_HIDDEN) || (L.kind == KIND_SIGMA && !L.is_final) || (L.kind == KIND_LOAD) ||
                             (L.kind == KIND_BWD && !L.is_final);
@@ -455,119 +460,132 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
         dsg[1] = val1 ? P.dout[(size_t)m1 * 4 + 3] : 0.f;
       }
       if (writes_a) ptx::named_bar_sync(bar_id, 128);    // every warp of the warpgroup is past this layer's MMAs
+      // The layer's 64-column chunks.  PLAIN (mode 0, a layer without a head whose outputs go back to the activation buffer:
+      // every hidden layer) is the same code with those two decisions fixed at compile time: each 8-column step is then one
+      // basic block, and the scheduler overlaps the shared-memory loads and the fp16 split chains of consecutive steps.
+      auto chunks = [&](auto plain) {
+        constexpr bool PLAIN = decltype(plain)::value;
+        const int heads_c = PLAIN ? 0 : heads;
+        const bool writes_c = PLAIN || writes_a;
 #pragma unroll
-      for (int nc = 0; nc < 4; ++nc) {
-        if (nc >= NC) continue;
-        uint32_t mk_in[2][2] = {{0xffffffffu, 0xffffffffu}, {0xffffffffu, 0xffffffffu}};   // mode 2: [row][32-column word]
-        if (MODE == 2 && L.kind == KIND_BWD && L.relu) {
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const long long m = e ? m1 : m0;
-            if (e ? val1 : val0) {
-              const uint2 bw = *reinterpret_cast<const uint2*>(P.emit.bits[li] + (size_t)m * (size_t)(L.n_out >> 5) + (size_t)(nc * 2));
-              mk_in[e][0] = bw.x; mk_in[e][1] = bw.y;
-            }
-          }
-        }
-        uint32_t mk_out[2][2] = {{0u, 0u}, {0u, 0u}};
-#pragma unroll
-        for (int j8 = 0; j8 < 8; ++j8) {
-          const int col = nc * 64 + j8 * 8 + cq;
-          float x[2][2];
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const bool valid = e ? val1 : val0;
-            const long long m = e ? m1 : m0;
-            if (MODE == 2 && L.kind == KIND_LOAD) {
-              // top of the data-gradient chain: dZ of the last forward layer, from HBM (rows past M are zero)
-              const float2 z = valid ? *reinterpret_cast<const float2*>(P.dz_in + (size_t)m * P.dz_ld + col) : make_float2(0.f, 0.f);
-              x[e][0] = z.x; x[e][1] = z.y;
-            } else if (MODE == 2) {
-              // dA = dZ W (+ d sigma * w_alpha), masked by relu' of the forward layer below.  (Its column sums — the bias
-              // gradient — are taken by the weight-gradient GEMM from the pack emitted below: nm_gemm_tc.cu a_rowsum.)
-#pragma unroll
-              for (int u = 0; u < 2; ++u) {
-                float y = acc[nc * 32 + j8 * 4 + 2 * e + u] * so;
-                if (L.aux2) y = fmaf(dsg[e], s_head[L.head_off + col + u], y);
-                const uint32_t w = valid ? mk_in[e][j8 >> 2] : 0u;
-                x[e][u] = ((w >> ((col + u) & 31)) & 1u) ? y : 0.f;
-              }
-            } else {
-#pragma unroll
-              for (int u = 0; u < 2; ++u) {
-                float y = fmaf(acc[nc * 32 + j8 * 4 + 2 * e + u], so, s_bias[L.bias_off + col + u]);
-                if (L.relu) y = fmaxf(y, 0.f);
-                x[e][u] = y;
-              }
-            }
-          }
-#pragma unroll
-          for (int hh = 0; hh < 4; ++hh) {
-            if (hh >= heads) break;
-            const float* w = s_head + L.head_off + hh * L.n_out + col;
+        for (int nc = 0; nc < 4; ++nc) {
+          if (nc >= NC) continue;
+          uint32_t mk_in[2][2] = {{0xffffffffu, 0xffffffffu}, {0xffffffffu, 0xffffffffu}};   // mode 2: [row][32-column word]
+          if (MODE == 2 && L.kind == KIND_BWD && L.relu) {
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
-              part[e][hh] = fmaf(w[0], x[e][0], part[e][hh]);
-              part[e][hh] = fmaf(w[1], x[e][1], part[e][hh]);
+              const long long m = e ? m1 : m0;
+              if (e ? val1 : val0) {
+                const uint2 bw = *reinterpret_cast<const uint2*>(P.emit.bits[li] + (size_t)m * (size_t)(L.n_out >> 5) + (size_t)(nc * 2));
+                mk_in[e][0] = bw.x; mk_in[e][1] = bw.y;
+              }
             }
           }
+          uint32_t mk_out[2][2] = {{0u, 0u}, {0u, 0u}};
 #pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const bool valid = e ? val1 : val0;
-            const long long m = e ? m1 : m0;
-            const int row = r0 + 8 * e;
-            if (MODE == 1) {
-              // by-products for the training backward: relu mask bits and the fp32 copy (layers the head kernels read)
-              mk_out[e][j8 >> 2] |= ((x[e][0] > 0.f ? 1u : 0u) | (x[e][1] > 0.f ? 2u : 0u)) << (col & 31);
-              if (P.emit.act[li] && valid) *reinterpret_cast<float2*>(P.emit.act[li] + (size_t)m * L.n_out + col) = make_float2(x[e][0], x[e][1]);
-            }
-            if (writes_a) {
-              uint32_t hi, lo;
-              const float a0 = x[e][0] * si, a1 = x[e][1] * si;
-              if (MODE == 2) {            // gradients: bf16 hi/lo (fp32's exponent range)
-                split_bf16x2(a0, a1, &hi, &lo);
-              } else {
-                hi = ptx::pack_f16x2_sat(a0, a1);
-                const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hi));
-                lo = ptx::pack_f16x2_sat(a0 - f.x, a1 - f.y);
-              }
-              if (n_passes != 3) lo = 0u;
-              const uint32_t off = (uint32_t)nc * kKBlock + swz_off(row, col & 63);
-              *reinterpret_cast<uint32_t*>(act + off) = hi;
-              *reinterpret_cast<uint32_t*>(act + 8192u + off) = lo;
-              if (MODE >= 1 && packT) {
-                // the weight-gradient operand is the A operand's value (hi + lo), as bf16 hi / lo; rows past M as zeros
-                uint32_t ph2 = 0u, pl2 = 0u;
-                if (valid) {
-                  if (MODE == 2) {
-                    ph2 = hi; pl2 = lo;
-                  } else {
-                    const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(&hi));
-                    const float2 fl = __half22float2(*reinterpret_cast<const __half2*>(&lo));
-                    split_bf16x2((fh.x + fl.x) * so, (fh.y + fl.y) * so, &ph2, &pl2);
-                  }
+          for (int j8 = 0; j8 < 8; ++j8) {
+            const int col = nc * 64 + j8 * 8 + cq;
+            float x[2][2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const bool valid = e ? val1 : val0;
+              const long long m = e ? m1 : m0;
+              if (MODE == 2 && L.kind == KIND_LOAD) {
+                // top of the data-gradient chain: dZ of the last forward layer, from HBM (rows past M are zero)
+                const float2 z = valid ? *reinterpret_cast<const float2*>(P.dz_in + (size_t)m * P.dz_ld + col) : make_float2(0.f, 0.f);
+                x[e][0] = z.x; x[e][1] = z.y;
+              } else if (MODE == 2) {
+                // dA = dZ W (+ d sigma * w_alpha), masked by relu' of the forward layer below.  (Its column sums — the bias
+                // gradient — are taken by the weight-gradient GEMM from the pack emitted below: nm_gemm_tc.cu a_rowsum.)
+#pragma unroll
+                for (int u = 0; u < 2; ++u) {
+                  float y = acc[nc * 32 + j8 * 4 + 2 * e + u] * so;
+                  if (L.aux2) y = fmaf(dsg[e], s_head[L.head_off + col + u], y);
+                  const uint32_t w = valid ? mk_in[e][j8 >> 2] : 0u;
+                  x[e][u] = ((w >> ((col + u) & 31)) & 1u) ? y : 0.f;
                 }
+              } else {
+#pragma unroll
+                for (int u = 0; u < 2; ++u) {
+                  float y = fmaf(acc[nc * 32 + j8 * 4 + 2 * e + u], so, s_bias[L.bias_off + col + u]);
+                  if (L.relu) y = fmaxf(y, 0.f);
+                  x[e][u] = y;
+                }
+              }
+            }
+#pragma unroll
+            for (int hh = 0; hh < 4; ++hh) {
+              if (hh >= heads_c) break;
+              const float* w = s_head + L.head_off + hh * L.n_out + col;
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                part[e][hh] = fmaf(w[0], x[e][0], part[e][hh]);
+                part[e][hh] = fmaf(w[1], x[e][1], part[e][hh]);
+              }
+            }
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const bool valid = e ? val1 : val0;
+              const long long m = e ? m1 : m0;
+              const int row = r0 + 8 * e;
+              if (MODE == 1) {
+                // by-products for the training backward: relu mask bits and the fp32 copy (layers the head kernels read)
+                mk_out[e][j8 >> 2] |= ((x[e][0] > 0.f ? 1u : 0u) | (x[e][1] > 0.f ? 2u : 0u)) << (col & 31);
+                if (P.emit.act[li] && valid) *reinterpret_cast<float2*>(P.emit.act[li] + (size_t)m * L.n_out + col) = make_float2(x[e][0], x[e][1]);
+              }
+              if (writes_c) {
+                uint32_t hi, lo;
+                const float a0 = x[e][0] * si, a1 = x[e][1] * si;
+                if (MODE == 2) {            // gradients: bf16 hi/lo (fp32's exponent range)
+                  split_bf16x2(a0, a1, &hi, &lo);
+                } else {
+                  hi = ptx::pack_f16x2_sat(a0, a1);
+                  const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+                  lo = ptx::pack_f16x2_sat(a0 - f.x, a1 - f.y);
+                }
+                if (n_passes != 3) lo = 0u;
+                const uint32_t off = (uint32_t)nc * kKBlock + swz_off(row, col & 63);
+                *reinterpret_cast<uint32_t*>(act + off) = hi;
+                *reinterpret_cast<uint32_t*>(act + 8192u + off) = lo;
+                if (MODE >= 1 && packT) {
+                  // the weight-gradient operand is the A operand's value (hi + lo), as bf16 hi / lo; rows past M as zeros
+                  uint32_t ph2 = 0u, pl2 = 0u;
+                  if (valid) {
+                    if (MODE == 2) {
+                      ph2 = hi; pl2 = lo;
+                    } else {
+                      const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+                      const float2 fl = __half22float2(*reinterpret_cast<const __half2*>(&lo));
+                      split_bf16x2((fh.x + fl.x) * so, (fh.y + fl.y) * so, &ph2, &pl2);
+                    }
+                  }
+                  emit_pack(packT, col, tile * kTileM + row, ph2, pl2);
+                }
+              } else if (MODE >= 1 && packT) {
+                uint32_t ph2, pl2;
+                split_bf16x2(valid ? x[e][0] : 0.f, valid ? x[e][1] : 0.f, &ph2, &pl2);
                 emit_pack(packT, col, tile * kTileM + row, ph2, pl2);
               }
-            } else if (MODE >= 1 && packT) {
-              uint32_t ph2, pl2;
-              split_bf16x2(valid ? x[e][0] : 0.f, valid ? x[e][1] : 0.f, &ph2, &pl2);
-              emit_pack(packT, col, tile * kTileM + row, ph2, pl2);
             }
           }
-        }
-        if (MODE == 1 && P.emit.bits[li]) {     // relu mask: the four lanes of a quad hold the 32 bits of a row's word
+          if (MODE == 1 && P.emit.bits[li]) {     // relu mask: the four lanes of a quad hold the 32 bits of a row's word
 #pragma unroll
-          for (int e = 0; e < 2; ++e)
+            for (int e = 0; e < 2; ++e)
 #pragma unroll
-            for (int g = 0; g < 2; ++g) {
-              uint32_t w = mk_out[e][g];
-              w |= __shfl_xor_sync(0xffffffffu, w, 1);
-              w |= __shfl_xor_sync(0xffffffffu, w, 2);
-              const long long m = e ? m1 : m0;
-              if ((lane & 3) == 0 && (e ? val1 : val0)) P.emit.bits[li][(size_t)m * (size_t)(L.n_out >> 5) + (size_t)(nc * 2 + g)] = w;
-            }
+              for (int g = 0; g < 2; ++g) {
+                uint32_t w = mk_out[e][g];
+                w |= __shfl_xor_sync(0xffffffffu, w, 1);
+                w |= __shfl_xor_sync(0xffffffffu, w, 2);
+                const long long m = e ? m1 : m0;
+                if ((lane & 3) == 0 && (e ? val1 : val0)) P.emit.bits[li][(size_t)m * (size_t)(L.n_out >> 5) + (size_t)(nc * 2 + g)] = w;
+              }
+          }
         }
+      };
+      if constexpr (MODE == 0) {
+        if (heads == 0 && writes_a) chunks(IntC<1>{}); else chunks(IntC<0>{});
+      } else {
+        chunks(IntC<0>{});
       }
       if (writes_a) {
         ptx::fence_proxy_async_smem();           // the next layer's wgmmas read what the generic proxy wrote
@@ -609,12 +627,17 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
           }
         }
       }
+      NM_ST(if (t == 0) st[4] += clock64() - ce;)
     }
-    if (MODE == 0 && P.comp_on) composite_tile(it, tile);
+    if (MODE == 0 && P.comp_on) {
+      NM_ST(const long long c0 = clock64();)
+      composite_tile(it, tile);
+      NM_ST(if (t == 0) st[5] += clock64() - c0;)
+    }
   }
   NM_ST(if (t == 0 && (blockIdx.x < 2 || blockIdx.x + 1 == gridDim.x))
-          printf("mlp_stalls mode %d cta %d wg %d wait %lld mma %lld other %lld\n", MODE, (int)blockIdx.x, wg, st[0], st[1],
-                 clock64() - st[2] - st[0] - st[1]);)
+          printf("mlp_stalls mode %d cta %d wg %d wait %lld mma %lld encode %lld epilogue %lld composite %lld other %lld\n", MODE,
+                 (int)blockIdx.x, wg, st[0], st[1], st[3], st[4], st[5], clock64() - st[2] - st[0] - st[1] - st[3] - st[4] - st[5]);)
 }
 
 }  // namespace
