@@ -339,6 +339,22 @@ int nm_rasterize_mesh(NmHandle h, const float* verts_dev, int64_t V, const int32
                       const float* atlas_dev_or_null, int N, const float* background_host, float* rgb_out_or_null,
                       float* depth_out_or_null, int32_t* face_out_or_null, int64_t* counts_host, void* stream);
 
+/* Surface points of one rendered view (the algorithm of the reference's dead src/mesh_surface_ray.py:66-141; DESIGN §4.14).
+ * depth_raw, acc (H*W) and rgb (H*W,3) are nm_render_image's outputs for pose_host (3x4 camera-to-world), H x W and focal
+ * without NDC; d(r,c) is the direction that render used (raygen's bits) and o = pose[:,3].  Per pixel t = depth_raw where
+ * acc >= min_acc, else 0, and P = o + d*t per component in fp32 (two roundings).  The count of pixel (r,c) is the number
+ * of offsets (a,b) in [-step, step]^2 whose neighbour (clamp(r+a, 0, H-1), clamp(c+b, 0, W-1)) has
+ * (dx*dx + dy*dy) + dz*dz < dist_threshold, with d the fp32 difference to P(r,c) (an edge pixel counts itself again; a NaN
+ * point counts nothing).  A pixel is kept when count >= min_count and t > 0.  Outputs are caller-allocated with room for
+ * H*W rows: per kept pixel in row-major order points (P), normals (-d), colors (rgb), and pixel_out (r*W + c, int32) unless
+ * NULL.  count_host = the number of kept pixels; synchronises once.  The same bits on every run.  Argument errors (null
+ * pointers, H or W below 1, H*W >= 2^31, step outside [0, 8], min_count below 1, focal not positive and finite, a NaN
+ * min_acc or dist_threshold) are rejected before anything is launched. */
+int nm_surface_points(NmHandle h, const float* pose_host, int H, int W, float focal, const float* depth_raw_dev,
+                      const float* acc_dev, const float* rgb_dev, float min_acc, int step, float dist_threshold, int min_count,
+                      float* points_out_dev, float* normals_out_dev, float* colors_out_dev, int32_t* pixel_out_dev_or_null,
+                      int64_t* count_host, void* stream);
+
 /* Replaces export_obj (src/nerf/nerf_helpers.py:86-111): `v x y z [r g b]`, `vn x y z`, `f i//i j//j k//k` (1-based) with
  * byte-identical number formatting (python repr of the float32 widened to double).  Host arrays, no GPU involved;
  * diffuse may be NULL or shorter than the vertex list (vertices beyond it get no colour, like the reference's
@@ -350,6 +366,13 @@ int nm_export_obj(const char* path, const float* verts_host, int64_t n_verts, co
 int nm_export_obj_textured(const char* path, const float* verts_host, int64_t n_verts, const int32_t* faces_host, int64_t n_faces,
                            const float* diffuse_host, int64_t n_diffuse, const float* normals_host, int64_t n_normals,
                            const float* uv_host, const char* mtl_name);
+/* Replaces export_ply (src/mesh_surface_ray.py:45-57): a point cloud with normals and colours as PLY.  Header `ply`,
+ * `format ascii 1.0` (binary = 0) or `format binary_little_endian 1.0` (binary = 1), `element vertex n`, `property float`
+ * x y z nx ny nz, `property uchar` red green blue, `end_header`.  Colours are quantised as trunc(fl32(c*255)) clamped to
+ * [0, 255], NaN to 0.  Text rows are the nine values as %.18g separated by single spaces; binary rows are packed 27-byte
+ * little-endian records.  Host arrays (n,3) fp32, no GPU involved. */
+int nm_export_ply(const char* path, const float* points_host, const float* colors_host, const float* normals_host, int64_t n,
+                  int binary);
 
 /* ---- hot path, host buffers (what a reference-side caller holding CPU tensors binds) ------------------ */
 /* model.query(ray_batch) with host tensors (src/eval_nerf.py:62-69): copies H2D, renders, copies D2H, syncs. */

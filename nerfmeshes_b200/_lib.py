@@ -73,6 +73,8 @@ _SIGNATURES = {
     "nm_debug_texture_rays": (C.c_int, [_P, _P, _P, _L, _P, _L, _I, _I, _F, _L, _L, _P, _P, _P, _P]),
     "nm_rasterize_mesh": (C.c_int, [_P, _P, _L, _P, _L, _P, _I, _I, _F, _F, _I, _P, _P, _I, _P, _P, _P, _P, C.POINTER(C.c_int64),
                                     _P]),
+    "nm_surface_points": (C.c_int, [_P, _P, _I, _I, _F, _P, _P, _P, _F, _I, _F, _I, _P, _P, _P, _P, C.POINTER(C.c_int64), _P]),
+    "nm_export_ply": (C.c_int, [C.c_char_p, _P, _P, _P, _L, _I]),
     "nm_export_obj": (C.c_int, [C.c_char_p, _P, _L, _P, _L, _P, _L, _P, _L]),
     "nm_export_obj_textured": (C.c_int, [C.c_char_p, _P, _L, _P, _L, _P, _L, _P, _L, _P, C.c_char_p]),
     "nm_query_host": (C.c_int, [_P, _P, _I, _P, _L, _P, _I, C.c_uint64, C.POINTER(NmRenderOut)]),

@@ -75,6 +75,7 @@ struct NmHandle_t {
                                    // (~40 B per chunk texel: 160 MB at the default 4 Mi)
   Buf rs_ws;                       // mesh raster: one depth-and-face key per pixel, one record per face (8 B per pixel + 52 B
                                    // per face)
+  Buf sf_ws;                       // surface points: one view's ray directions, keep mask and its scan (20 B per pixel)
   Buf sp_ws;                       // sparse sweep (nm_sparse_sweep.cu): block flags, two bit-volumes, scans, one chunk of points
   int sp_grid[4] = {0, 0, 0, 0};   // {n0, n1, n2, block} of the last nm_sparse_sweep_lattice, and the volume it wrote:
   const float* sp_vol = nullptr;   // what nm_sparse_sweep_run must be called with
@@ -541,7 +542,7 @@ int nm_destroy(NmHandle h) {
   for (int i = 0; i < 2; ++i) { h->g_wt[i].release(); h->g_bias[i].release(); h->g_head[i].release(); h->tr_rgb[i].release(); h->tr_drgb[i].release(); }
   h->train_ws.release(); h->dout.release(); h->trans.release();
   h->ss_tab.release(); h->ss_ws.release(); h->ms_ws.release(); h->nn_ws.release(); h->sg_ws.release();
-  h->cc_ws.release(); h->dc_ws.release(); h->sp_ws.release(); h->tx_ws.release(); h->rs_ws.release(); h->mc_ws.release(); h->mc_ws2.release();
+  h->cc_ws.release(); h->dc_ws.release(); h->sp_ws.release(); h->tx_ws.release(); h->rs_ws.release(); h->sf_ws.release(); h->mc_ws.release(); h->mc_ws2.release();
   if (h->h_err) cudaFreeHost(h->h_err);
   cudaFree(h->d_stats);
   for (cudaEvent_t e : h->ev) cudaEventDestroy(e);
@@ -1152,6 +1153,34 @@ int nm_rasterize_mesh(NmHandle h, const float* verts_dev, int64_t V, const int32
   m.big_pixels = raster_big_face_pixels();
   if (int e = h->rs_ws.ensure(raster_ws_bytes(m))) return e;
   return rasterize_mesh(m, counts_host, h->rs_ws.p, h->d_err + 2, (cudaStream_t)stream, &h->launches);
+}
+
+// ---------------------------------------------------------------------------------------------- surface points
+// Argument checks come before the handle is touched, so a bad call is rejected without a device.
+int nm_surface_points(NmHandle h, const float* pose_host, int H, int W, float focal, const float* depth_raw_dev,
+                      const float* acc_dev, const float* rgb_dev, float min_acc, int step, float dist_threshold, int min_count,
+                      float* points_out_dev, float* normals_out_dev, float* colors_out_dev, int32_t* pixel_out_dev_or_null,
+                      int64_t* count_host, void* stream) {
+  NM_CHECK(H >= 1 && W >= 1, "surface points: image %d x %d is empty", H, W);
+  NM_CHECK((long long)H * W < (1ll << 31), "surface points: %d x %d pixels is 2^31 or more", H, W);
+  NM_CHECK(step >= 0 && step <= kSurfaceMaxStep, "surface points: step %d outside [0, %d]", step, kSurfaceMaxStep);
+  NM_CHECK(min_count >= 1, "surface points: min_count %d is below 1", min_count);
+  NM_CHECK(focal > 0.f && std::isfinite(focal), "surface points: focal length %g is not positive and finite", (double)focal);
+  NM_CHECK(!std::isnan(min_acc) && !std::isnan(dist_threshold), "surface points: min_acc or dist_threshold is NaN");
+  NM_CHECK(pose_host && count_host, "surface points: null pose or count pointer");
+  NM_CHECK(depth_raw_dev && acc_dev && rgb_dev, "surface points: null depth_raw, acc or rgb pointer");
+  NM_CHECK(points_out_dev && normals_out_dev && colors_out_dev, "surface points: null output pointer");
+  NM_CHECK(h != nullptr, "null handle");
+  *count_host = 0;
+  if (int e = bind_checked(h)) return e;
+  SurfaceView v;
+  memcpy(v.pose, pose_host, sizeof(v.pose));
+  v.H = H; v.W = W; v.focal = focal;
+  v.depth_raw = depth_raw_dev; v.acc = acc_dev; v.rgb = rgb_dev;
+  v.min_acc = min_acc; v.dist_threshold = dist_threshold; v.step = step; v.min_count = min_count;
+  if (int e = h->sf_ws.ensure(surface_ws_bytes(H, W))) return e;
+  return surface_points(v, points_out_dev, normals_out_dev, colors_out_dev, pixel_out_dev_or_null, count_host, h->sf_ws.p,
+                        (cudaStream_t)stream, &h->launches);
 }
 
 // ---------------------------------------------------------------------------------------------- sparse density sweep

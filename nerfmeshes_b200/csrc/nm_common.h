@@ -350,4 +350,22 @@ size_t raster_ws_bytes(const RasterMesh& m);
 // drawn: every pixel gets the background.  counts_host = {covered pixels, faces drawn, faces culled}; synchronises once.
 int rasterize_mesh(const RasterMesh& m, int64_t* counts_host, void* ws, int* d_err, cudaStream_t st, int64_t* launches);
 
+// surface points of one rendered view (nm_surface.cu, DESIGN §4.14): depth_raw / acc (H*W), rgb (H*W,3) of nm_render_image
+// without NDC for this pose; the kept pixels' points, -directions, colours and pixel indices (pix may be null) in row-major
+// order.  ws: surface_ws_bytes(H, W) bytes.  *count_host = kept pixels; synchronises once.
+constexpr int kSurfaceMaxStep = 8;
+struct SurfaceView {
+  float pose[12] = {};
+  int H = 0, W = 0;
+  float focal = 0.f;
+  const float* depth_raw = nullptr;
+  const float* acc = nullptr;
+  const float* rgb = nullptr;
+  float min_acc = 1.f, dist_threshold = 0.f;
+  int step = 0, min_count = 1;
+};
+size_t surface_ws_bytes(long long H, long long W);
+int surface_points(const SurfaceView& v, float* pts, float* nrm, float* col, int32_t* pix, int64_t* count_host, void* ws,
+                   cudaStream_t st, int64_t* launches);
+
 }  // namespace nm

@@ -130,7 +130,52 @@ int write_obj(const char* path, const float* verts, int64_t n_verts, const int32
   return 0;
 }
 
+// trunc(fl32(c*255)) clamped to [0, 255], NaN to 0
+uint8_t ply_colour(float c) {
+  const float v = c * 255.0f;
+  if (!(v > 0.f)) return 0;
+  return v >= 255.f ? 255 : (uint8_t)v;
+}
+
 }  // namespace
+
+extern "C" int nm_export_ply(const char* path, const float* points, const float* colors, const float* normals, int64_t n,
+                             int binary) {
+  NM_CHECK(path && n >= 0 && (n == 0 || (points && colors && normals)), "null argument or negative count");
+  NM_CHECK(binary == 0 || binary == 1, "binary must be 0 or 1");
+  FILE* f = fopen(path, "wb");
+  NM_CHECK(f != nullptr, "cannot open '%s' for writing", path);
+  bool ok = fprintf(f,
+                    "ply\nformat %s 1.0\nelement vertex %lld\nproperty float x\nproperty float y\nproperty float z\n"
+                    "property float nx\nproperty float ny\nproperty float nz\nproperty uchar red\nproperty uchar green\n"
+                    "property uchar blue\nend_header\n",
+                    binary ? "binary_little_endian" : "ascii", (long long)n) > 0;
+  std::vector<char> buf(1 << 22);
+  char* p = buf.data();
+  char* const lim = buf.data() + buf.size() - 512;
+  auto flush = [&]() { ok = ok && fwrite(buf.data(), 1, (size_t)(p - buf.data()), f) == (size_t)(p - buf.data()); p = buf.data(); };
+  for (int64_t i = 0; i < n; ++i) {
+    const float* src[2] = {points + 3 * i, normals + 3 * i};
+    uint8_t q[3];
+    for (int c = 0; c < 3; ++c) q[c] = ply_colour(colors[3 * i + c]);
+    if (binary) {                                  // x86-64 and aarch64 hosts are little-endian, as the format is
+      for (int k = 0; k < 2; ++k) { memcpy(p, src[k], 12); p += 12; }
+      memcpy(p, q, 3); p += 3;
+    } else {
+      for (int k = 0; k < 2; ++k)
+        for (int c = 0; c < 3; ++c) {
+          p = std::to_chars(p, lim + 512, (double)src[k][c], std::chars_format::general, 18).ptr;   // printf's %.18g
+          *p++ = ' ';
+        }
+      for (int c = 0; c < 3; ++c) { p = put_int(q[c], p); *p++ = c < 2 ? ' ' : '\n'; }
+    }
+    if (p > lim) flush();
+  }
+  flush();
+  ok = (fclose(f) == 0) && ok;
+  NM_CHECK(ok, "short write to '%s'", path);
+  return 0;
+}
 
 extern "C" int nm_export_obj(const char* path, const float* verts, int64_t n_verts, const int32_t* faces, int64_t n_faces,
                              const float* diffuse, int64_t n_diffuse, const float* normals, int64_t n_normals) {

@@ -673,6 +673,36 @@ class Engine:
         self.check_flags()
         return outs, tuple(int(c) for c in counts)
 
+    # ------------------------------------------------------------------ surface points (DESIGN 4.14)
+    def surface_points(self, pose, H: int, W: int, focal: float, depth_raw, acc, rgb, *, min_acc: float = 1.0, step: int = 2,
+                       dist_threshold: float = 0.002, min_count: int = 15, out=None):
+        """The depth-consistent surface points of one view (nm_surface_points): depth_raw, acc (H*W) and rgb (H*W,3) are
+        render_image's outputs for this pose without NDC.  `out`: optional dict of caller-owned contiguous device tensors
+        "points", "normals", "colors" (H*W,3) fp32 and "pixel" (H*W,) int32 to write into.  Returns ({"points", "normals",
+        "colors", "pixel"}: the first n rows of those buffers, the kept pixels in row-major order, n).  Synchronises."""
+        p = np.ascontiguousarray(torch.as_tensor(pose).detach().cpu().numpy()[:3, :4], dtype=np.float32)
+        n = int(H) * int(W)
+        dr, ac, cl = _f32c(depth_raw, self.device).reshape(-1), _f32c(acc, self.device).reshape(-1), _f32c(rgb, self.device).reshape(-1, 3)
+        if not (dr.shape[0] == ac.shape[0] == cl.shape[0] == n):
+            raise L.NmError(f"surface points: depth_raw, acc and rgb must hold {H} x {W} pixels "
+                            f"(got {dr.shape[0]}, {ac.shape[0]}, {cl.shape[0]})")
+        shapes = dict(points=((n, 3), torch.float32), normals=((n, 3), torch.float32), colors=((n, 3), torch.float32),
+                      pixel=((n,), torch.int32))
+        outs = {}
+        for k, (shape, dt) in shapes.items():
+            t = None if out is None else out.get(k)
+            if t is None:
+                t = torch.empty(shape, dtype=dt, device=self.device)
+            assert t.dtype == dt and t.is_contiguous() and t.device == self.device and t.shape[0] >= n, (k, t.shape)
+            outs[k] = t
+        count = C.c_int64()
+        L.check(self.lib.nm_surface_points(self._h, p.ctypes.data, int(H), int(W), float(focal), _ptr(dr), _ptr(ac), _ptr(cl),
+                                           float(min_acc), int(step), float(dist_threshold), int(min_count),
+                                           _ptr(outs["points"]), _ptr(outs["normals"]), _ptr(outs["colors"]), _ptr(outs["pixel"]),
+                                           C.byref(count), self._stream()))
+        k = int(count.value)
+        return {name: t[:k] for name, t in outs.items()}, k
+
     # ------------------------------------------------------------------ sparse density sweep (DESIGN 4.10)
     def _sparse_args(self, lins, block, out):
         ls = [np.ascontiguousarray(torch.as_tensor(t).detach().cpu().numpy(), dtype=np.float32) for t in lins]

@@ -417,3 +417,147 @@ def export_marching_cubes(model, args, cfg=None, device="cuda"):
     diffuse = mesh_appearance(model, vertices, normals, args)
     export_obj(vertices, triangles, diffuse, normals, path)
     return path
+
+
+# ---------------------------------------------------------------------------------------------- surface point clouds (DESIGN 4.14)
+def surface_ray_poses(samples_y=8, samples_x=4, radius=4.0):
+    """The ring of src/mesh_surface_ray.py:80-87: pose_spherical(θ, φ, radius) with θ from linspace(-180, 180, samples_y,
+    endpoint=False) on the outer loop and φ from linspace(-90, 90, samples_x) on the inner one.  A list of (4,4) float32."""
+    from .nerf_api import pose_spherical
+    return [pose_spherical(float(th), float(ph), float(radius)) for th in np.linspace(-180, 180, samples_y, endpoint=False)
+            for ph in np.linspace(-90, 90, samples_x)]
+
+
+def surface_min_count(step, prob_threshold):
+    """The neighbour count a pixel needs: the script's `sum > size_samples * prob_threshold` (size_samples = (2s+1)^2 - 1)
+    as an integer bound, floor(size_samples * prob_threshold) + 1, in python double arithmetic."""
+    if not 0.0 <= prob_threshold <= 1.0:
+        raise ValueError(f"prob_threshold {prob_threshold} is outside [0, 1]")
+    size = 2 * int(step) + 1
+    return int(np.floor((size * size - 1) * float(prob_threshold))) + 1
+
+
+def surface_points(model, poses, H, W, focal, near, far, *, step=2, dist_threshold=0.002, prob_threshold=0.6, min_acc=1.0,
+                   network_normals=False):
+    """Depth-consistent surface points of a NeRF seen from `poses` (nm_surface_points, DESIGN 4.14; the algorithm of the
+    reference's dead src/mesh_surface_ray.py).  Each pose is rendered in validation mode (render_image: rgb, depth_raw, acc);
+    a pixel's point is o + d*t with t = depth_raw where acc >= min_acc, and it is kept when t > 0 and at least
+    surface_min_count(step, prob_threshold) of its (2*step+1)^2 clamped pixel neighbours lie within squared distance
+    dist_threshold.  normals = -d, or with network_normals -∇σ/|∇σ| of the net density_gradient uses (-d kept, and counted
+    in a printed line, where the gradient is zero or not finite).  Views are filtered one at a time, so memory is one view's
+    scratch plus the output.  Returns device tensors {"points", "normals", "colors": (N,3), "view", "pixel": (N,) int32, in
+    (view, row, column) order}, and "counts": the kept points per view.  NDC scenes raise NotImplementedError."""
+    from .models import _cfg_get
+    if _cfg_get(model.cfg, "dataset.use_ndc", False):
+        raise NotImplementedError("surface_points: the scene uses NDC rays, whose depths are not world distances; mapping them "
+                                  "back to world space is not implemented")
+    min_count = surface_min_count(step, prob_threshold)
+    eng = model._engine()
+    buff = hasattr(model, "tree")
+    if buff:                                           # what BuFFModel.forward does before it renders
+        model._sync_tree(eng)
+        eng.voxel_random = bool(_cfg_get(model.cfg, "tree.use_random_sampling", False))
+    which = model.get_model()._owner[1]
+    n = int(H) * int(W)
+    scratch = dict(points=torch.empty((n, 3), dtype=torch.float32, device=eng.device),
+                   normals=torch.empty((n, 3), dtype=torch.float32, device=eng.device),
+                   colors=torch.empty((n, 3), dtype=torch.float32, device=eng.device),
+                   pixel=torch.empty((n,), dtype=torch.int32, device=eng.device))
+    parts = {k: [] for k in ("points", "normals", "colors", "view", "pixel")}
+    counts, fallback = [], 0
+    for i, pose in enumerate(poses):
+        r = eng.render_image(pose, H, W, focal, near, far, buff=buff, want=("rgb", "depth_raw", "acc"))
+        outs, k = eng.surface_points(pose, H, W, focal, r["depth_raw"], r["acc"], r["rgb"], min_acc=min_acc, step=step,
+                                     dist_threshold=dist_threshold, min_count=min_count, out=scratch)
+        del r
+        nrm = outs["normals"]
+        if network_normals and k:
+            _, g = eng.sigma_grad(which, outs["points"], want_sigma=False)
+            norm = torch.sqrt(g[:, 0] * g[:, 0] + g[:, 1] * g[:, 1] + g[:, 2] * g[:, 2])
+            ok = torch.isfinite(norm) & (norm > 0)
+            nrm = torch.where(ok[:, None], -g / torch.where(ok, norm, torch.ones_like(norm))[:, None], nrm)
+            fallback += int((~ok).sum())
+        for key in ("points", "colors", "pixel"):
+            parts[key].append(outs[key].clone())
+        parts["normals"].append(nrm.clone())
+        parts["view"].append(torch.full((k,), i, dtype=torch.int32, device=eng.device))
+        counts.append(k)
+    if network_normals and fallback:
+        print(f"network normals: {fallback} of {sum(counts)} surface points have a zero or non-finite density gradient "
+              "and keep -d")
+    res = {key: (torch.cat(v, 0) if v else scratch[key][:0].clone()) for key, v in parts.items() if key != "view"}
+    res["view"] = torch.cat(parts["view"], 0) if parts["view"] else torch.zeros((0,), dtype=torch.int32, device=eng.device)
+    res["counts"] = counts
+    return res
+
+
+def ply_colors(colors):
+    """Colours as PLY uchar: trunc(fl32(c*255)) clamped to [0, 255], NaN to 0 (numpy, any float input cast to float32)."""
+    v = np.asarray(colors, dtype=np.float32) * np.float32(255.0)
+    with np.errstate(invalid="ignore"):
+        q = np.where(v > 0, np.minimum(np.trunc(v), 255.0), 0.0)
+    return q.astype(np.uint8)
+
+
+def ply_header(n, binary=False):
+    fmt = "binary_little_endian" if binary else "ascii"
+    props = "".join(f"property float {p}\n" for p in ("x", "y", "z", "nx", "ny", "nz"))
+    props += "".join(f"property uchar {p}\n" for p in ("red", "green", "blue"))
+    return f"ply\nformat {fmt} 1.0\nelement vertex {n}\n{props}end_header\n".encode()
+
+
+def _export_ply_python(points, colors, normals, filename, binary=False):
+    """Pure-python formatter (any dtype; values become the format's float32 and uchar); the native writer below must
+    produce the same bytes."""
+    arr = lambda a: np.asarray(a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else a, dtype=np.float32).reshape(-1, 3)
+    p, n = arr(points), arr(normals)
+    q = ply_colors(arr(colors))
+    out = [ply_header(p.shape[0], binary)]
+    if binary:
+        rec = np.empty(p.shape[0], dtype=[("p", "<f4", (3,)), ("n", "<f4", (3,)), ("c", "u1", (3,))])
+        rec["p"], rec["n"], rec["c"] = p, n, q
+        out.append(rec.tobytes())
+    else:
+        out.extend((" ".join("%.18g" % x for x in a.tolist() + b.tolist()) + " " + " ".join(str(x) for x in c.tolist())
+                    + "\n").encode() for a, b, c in zip(p.astype(np.float64), n.astype(np.float64), q))
+    with open(filename, "wb") as fh:
+        fh.writelines(out)
+
+
+def export_ply(points, colors, normals, filename, binary=False):
+    """src/mesh_surface_ray.py:45-57's PLY (plyfile's layout): `element vertex N`, float x y z nx ny nz, uchar red green blue.
+    Text rows hold the nine values as %.18g separated by single spaces; binary=True writes binary_little_endian 27-byte
+    records.  Colours become trunc(fl32(c*255)) clamped to [0, 255], NaN 0.  float32 (N,3) inputs go through the library's
+    native writer (nm_export_ply); anything else through the python formatter with the same output."""
+    def arr(a):
+        return a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)
+    p, c, n = arr(points), arr(colors), arr(normals)
+    if not all(x.dtype == np.float32 and x.ndim == 2 and x.shape == p.shape and x.shape[1:] == (3,) for x in (p, c, n)):
+        return _export_ply_python(points, colors, normals, filename, binary)
+    import ctypes as C
+    p, c, n = np.ascontiguousarray(p), np.ascontiguousarray(c), np.ascontiguousarray(n)
+    ptr = lambda a: C.c_void_p(a.ctypes.data) if a.size else None
+    L.check(L.load().nm_export_ply(str(filename).encode(), ptr(p), ptr(c), ptr(n), p.shape[0], int(bool(binary))))
+
+
+def export_surface_points(model, args):
+    """src/mesh_surface_ray.py:66-141 (export_ray_trace) on the fused path: the 32 ring poses of surface_ray_poses at radius
+    4.0, args.img_size x args.img_size pixels (800) at args.focal (1111.1111), near / far from the config's dataset.near /
+    dataset.far, step args.step_size (2), args.dist_threshold (0.002), args.prob_threshold (0.6), args.min_acc (1.0),
+    args.network_normals (False), written by export_ply to save_dir/args.ply_name ('lego-sampling.ply'), binary with
+    args.ply_binary.  Returns the path."""
+    import os
+    from .models import _cfg_get
+    g = lambda k, d: d if getattr(args, k, None) is None else getattr(args, k)
+    size = int(g("img_size", 800))
+    near, far = _cfg_get(model.cfg, "dataset.near"), _cfg_get(model.cfg, "dataset.far")
+    if near is None or far is None:
+        raise ValueError("export_surface_points: the model's config has no dataset.near / dataset.far")
+    r = surface_points(model, surface_ray_poses(), size, size, float(g("focal", 1111.1111)), float(near), float(far),
+                       step=int(g("step_size", 2)), dist_threshold=float(g("dist_threshold", 0.002)),
+                       prob_threshold=float(g("prob_threshold", 0.6)), min_acc=float(g("min_acc", 1.0)),
+                       network_normals=bool(g("network_normals", False)))
+    path = os.path.join(args.save_dir, g("ply_name", "lego-sampling.ply"))
+    export_ply(r["points"], r["colors"], r["normals"], path, binary=bool(g("ply_binary", False)))
+    print(f"surface points: {r['points'].shape[0]} points from {len(r['counts'])} views -> {path}")
+    return path

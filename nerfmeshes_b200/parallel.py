@@ -381,3 +381,23 @@ def extract_geometry_sharded(model, args, group=None, to_host=True, timings=None
     if to_host:
         return mesh.rescale_vertices(v, args.limit, args.res), f.cpu(), n.cpu(), iso
     return v, f, n, iso
+
+
+def surface_points_sharded(model, poses, H, W, focal, near, far, *, group=None, **kw):
+    """mesh.surface_points on N GPUs: this rank renders and filters the contiguous block of poses row_shard(len(poses), rank,
+    world) gives it, then one padded all_gather per output assembles the blocks in rank order, which is pose order.  Views
+    are independent, so every rank returns the single-GPU arrays bit for bit: {"points", "normals", "colors", "view",
+    "pixel", "counts"} as mesh.surface_points documents them (view = the index into `poses`).  `kw`: its keyword options.
+    Works without a process group (one block)."""
+    rank, world = _rank_world(group)
+    v0, v1 = row_shard(len(poses), rank, world)
+    local = mesh.surface_points(model, list(poses)[v0:v1], H, W, focal, near, far, **kw)
+    local["view"] = local["view"] + v0
+    if world == 1:
+        return local
+    dev = local["points"].device
+    out = {k: torch.cat(_all_gather_padded(local[k].contiguous(), group), 0)
+           for k in ("points", "normals", "colors", "view", "pixel")}
+    counts = _all_gather_padded(torch.tensor(local["counts"], dtype=torch.int64, device=dev), group)
+    out["counts"] = [int(c) for part in counts for c in part.tolist()]
+    return out
