@@ -447,6 +447,14 @@ int nm_debug_mlp_backward(NmHandle h, int which, const float* pts_dev, const flo
 int nm_debug_composite_backward(NmHandle h, const float* raw_dev, const float* t_dev, const float* dirs_dev,
                                 const float* d_rgb_dev, int64_t R, int S, float noise_std, uint64_t seed, int white_bg,
                                 float* dout_dev, void* stream);
+/* Test hook for the inverse-CDF resampler alone (invcdf_kernel, nm_render.cu), the call a two-network render makes: from
+ * the coarse depths t_c_dev (R,Nc), ascending per ray, and the coarse weights w_c_dev (R,Nc) it writes t_out_dev (R,Nc+Nf),
+ * the coarse depths and Nf new samples merged in ascending order.  perturb = 0 places the samples at u_dev (Nf); otherwise
+ * u is drawn from the stream `seed` (already salted: a render passes its chunk seed ^ 0x9e3779b9) and u_dev may be NULL.
+ * 3 <= Nc <= 256, 1 <= Nf, Nc + Nf <= 512; argument errors are rejected before anything is launched; R = 0 launches
+ * nothing. */
+int nm_debug_sample_pdf(NmHandle h, const float* t_c_dev, const float* w_c_dev, const float* u_dev, int64_t R, int Nc, int Nf,
+                        int perturb, uint64_t seed, float* t_out_dev, void* stream);
 
 /* ---- host-only debugging aid (no CUDA): the layer program + tensor-core weight blocks (64x64, 128B-swizzled, schedule
  * order), for CPU tests of the schedule / swizzle logic.  program_out receives the internal NetProgram struct
@@ -466,11 +474,13 @@ int nm_debug_pack_wide(const NmNetDesc* desc, int n_tensors, const char* const* 
 int nm_debug_tile_schedule(int samples_per_ray, int64_t n_tiles, int grid, int cta, int64_t* tiles_out, int64_t cap, int64_t* n_out);
 
 /* Device-side error flags, readable even after a kernel trapped: out2[0] = tensor-core pipeline watchdog code (0 = ok),
- * out2[1] = AABB hit-list overflow. */
+ * out2[1] = AABB hit-list overflow (a ray through more than 512 voxels; cleared once nm_check_flags or an entry point has
+ * reported it). */
 int nm_kernel_flags(NmHandle h, int32_t* out2);
 /* Synchronises `stream`, then fails (<0, message in nm_last_error) if a kernel of this handle raised a device-side flag.
  * The asynchronous device-pointer entry points report flags raised by EARLIER calls when they are entered; *_host calls
- * check before they return. */
+ * check before they return.  The watchdog is reported on every call (the device is no longer trusted); the input
+ * conditions, an AABB hit-list overflow and a bad mesh, are reported once and then cleared. */
 int nm_check_flags(NmHandle h, void* stream);
 
 /* ---- introspection ---------------------------------------------------------------------------------- */

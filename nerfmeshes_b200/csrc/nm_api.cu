@@ -49,7 +49,8 @@ struct NmHandle_t {
   // workspace
   Buf t_c, raw_c, w_c, t_f, raw_f, t_u, dirs, origins, lin[3], small, stage_in[3], stage_out[12];
   int lin_n[3] = {0, 0, 0};
-  int* d_err = nullptr;       // [0] tensor-core pipeline watchdog code, [1] aabb hit-list overflow, [2] mesh input error
+  int* d_err = nullptr;       // [0] tensor-core pipeline watchdog code, [1] aabb hit-list overflow (cleared when reported),
+                              // [2] mesh input error
                               // (mesh sampler 1: face index out of range, 2: total area not positive; component filter
                               // 3: face index out of range; decimation 4: face index out of range; texture bake 5:
                               // face index out of range; mesh raster 6: face index out of range; cleared when reported)
@@ -151,11 +152,13 @@ int bind_checked(NmHandle h) {
   return check_kernel_flags(h);
 }
 
-void linspace_host(int n, std::vector<float>* out) {  // torch.linspace(0,1,n) fp32 (ATen's two-sided formula)
+// torch.linspace(0,1,n) fp32: ATen's two-sided formula, whose upper half is one fused multiply-add (torch's values; two
+// roundings there differ by an ulp at about a tenth of the points)
+void linspace_host(int n, std::vector<float>* out) {
   out->resize(n);
   if (n == 1) { (*out)[0] = 0.f; return; }
   const float step = 1.0f / (float)(n - 1);
-  for (int i = 0; i < n; ++i) (*out)[i] = (i < n / 2) ? 0.f + step * (float)i : 1.0f - step * (float)(n - 1 - i);
+  for (int i = 0; i < n; ++i) (*out)[i] = (i < n / 2) ? 0.f + step * (float)i : std::fmaf(-step, (float)(n - 1 - i), 1.0f);
 }
 
 int upload(Buf* b, const void* src, size_t bytes) {
@@ -167,7 +170,10 @@ int upload(Buf* b, const void* src, size_t bytes) {
 int check_kernel_flags(NmHandle h) {
   const volatile int* flags = h->h_err;
   NM_CHECK(flags[0] == 0, "tensor-core pipeline watchdog fired (code %d)", flags[0]);
-  NM_CHECK(flags[1] == 0, "AABB sampler: more than 512 voxel hits on one ray (samples / voxel indices of that ray are truncated)");
+  if (flags[1]) {                   // an input condition too (a ray through too many voxels): reported once
+    h->h_err[1] = 0;
+    NM_CHECK(false, "AABB sampler: more than 512 voxel hits on one ray (samples / voxel indices of that ray are truncated)");
+  }
   if (const int c = flags[2]) {     // a bad input mesh, not a broken device: reported once
     h->h_err[2] = 0;
     NM_CHECK(false, c == 1   ? "mesh sampler: a face index lies outside [0, V)"
@@ -209,6 +215,9 @@ int run_mlp(NmHandle h, int which, bool sigma_only, const MlpInput& in, float* o
 }
 
 constexpr uint64_t kNoiseSaltMain = 0x5bd1e995ull, kNoiseSaltCoarse = 0x7f4a7c15a3c59ac3ull;
+// the random voxel draws (NM_FLAG_RANDOM_VOXELS) and the inverse-CDF jitter of a chunk: streams of their own, so that no
+// two consumers of one chunk seed share a splitmix64 state (tests/test_ray_samplers_reference.py checks every pair)
+constexpr uint64_t kVoxelSalt = 0xd1b54a32d192ed03ull, kInvCdfSalt = 0x9e3779b9ull;
 
 struct RayBatch {
   const float* origins; int o_stride; const float* dirs; long long R;
@@ -273,7 +282,7 @@ int render_chunk(NmHandle h, const RayBatch& rb, int flags, uint64_t seed, const
     float* z = h->t_u.as<float>();
     if (int e = launch_aabb(h->voxels.as<float>(), h->V, rb.origins, rb.o_stride, rb.dirs, R, rb.nf[0], rb.nf[1], Nc,
                             h->s_table.as<float>(), t_c, z, nullptr, h->d_err + 1, st, &h->launches,
-                            (flags & NM_FLAG_RANDOM_VOXELS) ? 1 : 0, seed)) return e;
+                            (flags & NM_FLAG_RANDOM_VOXELS) ? 1 : 0, seed ^ kVoxelSalt)) return e;
     if (o.t_vals) NM_CUDA(cudaMemcpyAsync(o.t_vals, z, (size_t)R * Nc * 4, cudaMemcpyDeviceToDevice, st));
     return mlp_composite(NM_NET_COARSE, h->raw_c, emit_c, z, Nc, o.rgb, o.depth, o.depth_raw, o.acc, o.disp, o.weights, o.mask_weights);
   }
@@ -288,7 +297,7 @@ int render_chunk(NmHandle h, const RayBatch& rb, int flags, uint64_t seed, const
   // inverse-CDF resampling + merge (a8)
   float* t_f = o.t_vals;
   if (!t_f) { if (int e = h->t_f.ensure((size_t)R * S * 4)) return e; t_f = h->t_f.as<float>(); }
-  if (int e = launch_invcdf(t_c, w_c, h->u_table.as<float>(), Nc, Nf, R, c.perturb, seed ^ 0x9e3779b9u, t_f, st, &h->launches)) return e;
+  if (int e = launch_invcdf(t_c, w_c, h->u_table.as<float>(), Nc, Nf, R, c.perturb, seed ^ kInvCdfSalt, t_f, st, &h->launches)) return e;
   return mlp_composite(NM_NET_FINE, h->raw_f, emit_f, t_f, S, o.rgb, o.depth, o.depth_raw, o.acc, o.disp, o.weights, o.mask_weights);
 }
 
@@ -764,6 +773,19 @@ int nm_debug_composite_backward(NmHandle h, const float* raw_dev, const float* t
                                    dout_dev, (cudaStream_t)stream, &h->launches);
 }
 
+int nm_debug_sample_pdf(NmHandle h, const float* t_c_dev, const float* w_c_dev, const float* u_dev, int64_t R, int Nc, int Nf,
+                        int perturb, uint64_t seed, float* t_out_dev, void* stream) {
+  if (int e = bind_checked(h)) return e;
+  NM_CHECK(t_c_dev && w_c_dev && t_out_dev, "null pointer argument");
+  NM_CHECK(R >= 0, "negative ray count %lld", (long long)R);
+  NM_CHECK(Nc >= 3 && Nc <= 256, "coarse samples per ray %d outside [3, 256]", Nc);
+  NM_CHECK(Nf >= 1 && Nc + Nf <= 512, "fine samples per ray %d outside [1, 512 - Nc]", Nf);
+  NM_CHECK(perturb || u_dev, "a deterministic resample needs the u table");
+  if (R == 0) return 0;
+  // the same call as render_chunk's, on the caller's arrays
+  return launch_invcdf(t_c_dev, w_c_dev, u_dev, Nc, Nf, R, perturb, seed, t_out_dev, (cudaStream_t)stream, &h->launches);
+}
+
 // ---------------------------------------------------------------------------------------------- BuFF tree maintenance
 int nm_ray_voxel_indices(NmHandle h, const float* origins_dev, int o_stride, const float* dirs_dev, int64_t R,
                          const float* near_far_host, float* z_out_dev, int32_t* idx_out_dev, void* stream) {
@@ -793,7 +815,7 @@ int nm_ray_voxel_indices_ex(NmHandle h, const float* origins_dev, int o_stride, 
     if (int e = launch_aabb(h->voxels.as<float>(), h->V, origins_dev + (long long)o_stride * r0, o_stride, dirs_dev + 3 * r0, n,
                             near_far_host[0], near_far_host[1], S, h->s_table.as<float>(), t_u ? t_u + r0 * S : nullptr,
                             z_out_dev ? z_out_dev + r0 * S : nullptr, idx_out_dev + r0 * S, h->d_err + 1, st, &h->launches,
-                            (flags & NM_FLAG_RANDOM_VOXELS) ? 1 : 0, seed + (uint64_t)r0)) return e;
+                            (flags & NM_FLAG_RANDOM_VOXELS) ? 1 : 0, (seed + (uint64_t)r0) ^ kVoxelSalt)) return e;
   }
   return 0;
 }

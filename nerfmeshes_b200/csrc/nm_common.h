@@ -163,6 +163,7 @@ struct CompositeArgs {
 int launch_composite(const CompositeArgs& a, cudaStream_t st, int64_t* launches);
 int launch_invcdf(const float* t_c, const float* w_c, const float* u_table, int Nc, int Nf, long long R, int perturb,
                   uint64_t seed, float* t_f, cudaStream_t st, int64_t* launches);
+// random != 0: cfg.tree.use_random_sampling, drawn from the stream `seed` (already salted: the callers pass seed ^ kVoxelSalt)
 int launch_aabb(const float* voxels, int V, const float* origins, int o_stride, const float* dirs, long long R,
                 float near, float far, int S, const float* s_table, const float* t_uniform, float* z_out, int* idx_out,
                 int* d_overflow, cudaStream_t st, int64_t* launches, int random = 0, uint64_t seed = 0);

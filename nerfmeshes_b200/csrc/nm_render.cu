@@ -328,11 +328,11 @@ __global__ void __launch_bounds__(kAabbWarps * 32) aabb_kernel(const float* __re
     // cfg.tree.use_random_sampling (tree.py:280-297): S draws with replacement from a multinomial that weighs every hit voxel 1
     // (and every miss 1e-12: a 1e-9-probability event per draw that would sample a non-intersection's garbage interval —
     // not reproduced), each placed uniformly inside its voxel's [entry, exit]; then the common sort below.  Distributional
-    // parity only: torch's generator stream cannot be matched.
+    // parity only: torch's generator stream cannot be matched.  `seed` is the draws' own stream (kVoxelSalt, nm_api.cu).
     for (int k = lane; k < S; k += 32) {
       const uint64_t c = (uint64_t)(ray * S + k);
-      const int h = min((int)(u01(seed ^ 0x5bd1e995u, 2 * c) * (float)H), H - 1);
-      z[k] = lo[h] + (hi[h] - lo[h]) * u01(seed ^ 0x5bd1e995u, 2 * c + 1);
+      const int h = min((int)(u01(seed, 2 * c) * (float)H), H - 1);
+      z[k] = lo[h] + (hi[h] - lo[h]) * u01(seed, 2 * c + 1);
       bucket[k] = vox[h];
     }
     __syncwarp();

@@ -357,6 +357,20 @@ class Engine:
                                                      int(seed) % 2 ** 64, int(white_bg), _ptr(out), self._stream()))
         return out
 
+    def debug_sample_pdf(self, t_c, w_c, u=None, *, Nf=None, perturb=False, seed=0):
+        """Test hook (nm_debug_sample_pdf): the inverse-CDF resampler alone.  t_c (R,Nc) ascending coarse depths, w_c (R,Nc)
+        coarse weights; u (Nf,) the deterministic positions, or None with `perturb` (drawn from the salted stream `seed`).
+        Returns (R, Nc+Nf): the coarse depths and the new samples, merged in ascending order."""
+        tc, wc = _f32c(t_c, self.device), _f32c(w_c, self.device)
+        uu = None if u is None else _f32c(u, self.device).reshape(-1)
+        Nf = int(uu.numel() if Nf is None else Nf)
+        R, Nc = tc.shape
+        assert wc.shape == (R, Nc) and (uu is None or uu.numel() == Nf), (tc.shape, wc.shape, None if uu is None else uu.shape)
+        out = torch.empty((R, Nc + Nf), dtype=torch.float32, device=self.device)
+        L.check(self.lib.nm_debug_sample_pdf(self._h, _ptr(tc), _ptr(wc), _ptr(uu), R, Nc, Nf, int(bool(perturb)),
+                                             int(seed) % 2 ** 64, _ptr(out), self._stream()))
+        return out
+
     def render_image(self, pose, H, W, focal, near, far, *, ndc=False, rows=None, training=False, buff=False, seed=0,
                      want=None, to_host=False, host_out=None, out=None) -> Dict[str, torch.Tensor]:
         """Rays generated on the device from a 3x4 / 4x4 camera-to-world pose (get_ray_bundle [+ ndc_rays])."""
