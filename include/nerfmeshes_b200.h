@@ -88,8 +88,10 @@ enum {
   NM_FLAG_TRAINING = 1,    /* module.training: no depth threshold, train noise_std            */
   NM_FLAG_BUFF = 2,        /* BuFFModel.forward: AABB-clipped sampling, single net (coarse slot) */
   NM_FLAG_TEACHER_T = 4,   /* t_vals is an INPUT: skip sampling, run net `which`=fine-if-present on it */
-  NM_FLAG_RANDOM_VOXELS = 8 /* with NM_FLAG_BUFF: cfg.tree.use_random_sampling — multinomial voxel draws + uniform depth inside
+  NM_FLAG_RANDOM_VOXELS = 8, /* with NM_FLAG_BUFF: cfg.tree.use_random_sampling — multinomial voxel draws + uniform depth inside
                                the voxel (src/nerf/tree.py:280-297) instead of the deterministic placement; uses `seed` */
+  NM_FLAG_SKIP_EMPTY = 16   /* empty-space skipping (nm_build_occupancy): only the samples the pass's occupancy grid marks go
+                               through the network; inference only (rejected with NM_FLAG_TRAINING / NM_FLAG_TEACHER_T) */
 };
 
 /* ---- lifecycle -------------------------------------------------------------------------------------- */
@@ -373,6 +375,33 @@ int nm_export_obj_textured(const char* path, const float* verts_host, int64_t n_
  * little-endian records.  Host arrays (n,3) fp32, no GPU involved. */
 int nm_export_ply(const char* path, const float* points_host, const float* colors_host, const float* normals_host, int64_t n,
                   int binary);
+
+/* ---- empty-space skipping (DESIGN §4.15) ------------------------------------------------------------------
+ * One occupancy grid per network slot: G x G x G cells over the box [lo, hi) (box = {lo_x, lo_y, lo_z, hi_x, hi_y, hi_z} in
+ * network-input coordinates, NDC ones for an NDC render), one bit per cell, bit (i*G + j)*G + k of uint32 words
+ * (ceil(G^3 / 32) of them).  A point p is EVALUATED when, for some axis a, c_a = floor((p_a - lo_a) * inv_a) is outside [0, G)
+ * or not finite (fp32, a rounded subtract then a rounded multiply; inv_a = G / (hi_a - lo_a) rounded once), or when its cell's
+ * bit is set.  With NM_FLAG_SKIP_EMPTY a render sends only evaluated samples through the network; every other sample enters
+ * the compositor as raw (0,0,0,0), i.e. alpha = 0.  Guarantee: every output of a ray (rgb, depth, depth_raw, acc, disp,
+ * weights, mask_weights, t_vals, coarse_*) is bit-identical to the render without the flag when every sample the grid skipped
+ * on that ray has a dense raw sigma <= 0 or NaN.  A skipping render reads each pass's sample count back to the host (one
+ * small copy and one stream synchronisation per pass per NM_CHUNK_RAYS chunk), so it cannot be captured in a CUDA graph; the
+ * network runs on at most NM_SKIP_CHUNK_POINTS points per launch (default 4 Mi).  Loading a network's weights drops its grid.
+ *
+ * nm_build_occupancy: the grid of network `which` from its own density.  Lattice: torch.linspace(lo_a, hi_a, G+1) per axis,
+ *   sigma from nm_grid_sigma's sigma-only sweep of that network (directions = positions); a cell is raw-occupied when the max
+ *   of its 8 corner sigmas is > threshold or a corner is NaN; the grid is the raw occupancy dilated by `dilate` cells in
+ *   Chebyshev distance (clamped at the box faces).  1 <= G <= 1024, 0 <= dilate <= G, threshold not NaN.  bits_out_dev (the
+ *   ceil(G^3/32) words) or NULL.  Synchronises `stream` once.
+ * nm_set_occupancy: installs caller bits (same layout) for network `which`; bits_dev NULL removes the grid.
+ * nm_occupancy_query: evaluated_out_dev[m] = 1 if point m (pts_dev (M,3)) is evaluated under network `which`'s grid, else 0.
+ * nm_skip_stats: out_host = {samples seen, samples evaluated} of the coarse (or only) pass, then of the fine pass, summed
+ *   over skipping renders since the last call; resets them.  Synchronises the device. */
+int nm_build_occupancy(NmHandle h, int which, const float* box_host, int G, float threshold, int dilate,
+                       uint32_t* bits_out_dev_or_null, void* stream);
+int nm_set_occupancy(NmHandle h, int which, const float* box_host, int G, const uint32_t* bits_dev_or_null);
+int nm_occupancy_query(NmHandle h, int which, const float* pts_dev, int64_t M, uint8_t* evaluated_out_dev, void* stream);
+int nm_skip_stats(NmHandle h, int64_t* out_host);
 
 /* ---- hot path, host buffers (what a reference-side caller holding CPU tensors binds) ------------------ */
 /* model.query(ray_batch) with host tensors (src/eval_nerf.py:62-69): copies H2D, renders, copies D2H, syncs. */

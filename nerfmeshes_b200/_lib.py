@@ -31,7 +31,7 @@ class NmRenderOut(C.Structure):
 
 
 PREC_EXACT, PREC_FAST, PREC_FP32 = 0, 1, 2
-FLAG_TRAINING, FLAG_BUFF, FLAG_TEACHER_T, FLAG_RANDOM_VOXELS = 1, 2, 4, 8
+FLAG_TRAINING, FLAG_BUFF, FLAG_TEACHER_T, FLAG_RANDOM_VOXELS, FLAG_SKIP_EMPTY = 1, 2, 4, 8, 16
 NET_COARSE, NET_FINE = 0, 1
 
 _P, _I, _L, _F = C.c_void_p, C.c_int, C.c_int64, C.c_float
@@ -74,6 +74,10 @@ _SIGNATURES = {
     "nm_rasterize_mesh": (C.c_int, [_P, _P, _L, _P, _L, _P, _I, _I, _F, _F, _I, _P, _P, _I, _P, _P, _P, _P, C.POINTER(C.c_int64),
                                     _P]),
     "nm_surface_points": (C.c_int, [_P, _P, _I, _I, _F, _P, _P, _P, _F, _I, _F, _I, _P, _P, _P, _P, C.POINTER(C.c_int64), _P]),
+    "nm_build_occupancy": (C.c_int, [_P, _I, _P, _I, _F, _I, _P, _P]),
+    "nm_set_occupancy": (C.c_int, [_P, _I, _P, _I, _P]),
+    "nm_occupancy_query": (C.c_int, [_P, _I, _P, _L, _P, _P]),
+    "nm_skip_stats": (C.c_int, [_P, C.POINTER(C.c_int64)]),
     "nm_export_ply": (C.c_int, [C.c_char_p, _P, _P, _P, _L, _I]),
     "nm_export_obj": (C.c_int, [C.c_char_p, _P, _L, _P, _L, _P, _L, _P, _L]),
     "nm_export_obj_textured": (C.c_int, [C.c_char_p, _P, _L, _P, _L, _P, _L, _P, _L, _P, C.c_char_p]),

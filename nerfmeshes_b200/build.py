@@ -31,6 +31,7 @@ SOURCES = {
     "nm_texture.cu": ["-fmad=false"],        # fp32 texel positions and rays in the written order: tests/_texture_ref.py
     "nm_raster.cu": ["-fmad=false"],         # fp32 projection, weights and shading in the written order: tests/_raster_ref.py
     "nm_surface.cu": ["-fmad=false"],        # fp32 surface points and distances in the written order: tests/_surface_ref.py
+    "nm_occupancy.cu": ["-fmad=false"],      # fp32 sample points and cell lookups in the written order: tests/_occupancy_ref.py
     "nm_train.cu": [],
     "nm_sigma_grad.cu": [],
     "nm_gemm_tc.cu": [],

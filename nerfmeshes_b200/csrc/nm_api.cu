@@ -4,6 +4,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
+#include <algorithm>
 #include <cstring>
 #include <vector>
 
@@ -80,6 +81,16 @@ struct NmHandle_t {
   Buf sp_ws;                       // sparse sweep (nm_sparse_sweep.cu): block flags, two bit-volumes, scans, one chunk of points
   int sp_grid[4] = {0, 0, 0, 0};   // {n0, n1, n2, block} of the last nm_sparse_sweep_lattice, and the volume it wrote:
   const float* sp_vol = nullptr;   // what nm_sparse_sweep_run must be called with
+  struct OccGrid {                 // empty-space skipping (nm_occupancy.cu, DESIGN §4.15): one grid per network slot, dropped
+    bool valid = false;            // by a weight load of that slot
+    float lo[3], hi[3], inv[3];
+    int G = 0;
+    Buf bits;
+  } occ[2];
+  Buf oc_ws;                       // grid build: one plane chunk of the sigma lattice, two G^3 byte volumes
+  Buf sk_ws;                       // skipping render: marks, scan, index list (12 B per sample of a chunk pass) + one network
+                                   // launch's points, directions and outputs (40 B per point, 160 MB at the default 4 Mi)
+  int64_t skip_counts[4] = {0, 0, 0, 0};   // samples seen / evaluated, coarse (or only) pass, fine pass (nm_skip_stats)
   Buf sg_ws;                       // density gradient (nm_sigma_grad): one chunk's forward / chain / tail workspace; grow-only,
                                    // held until nm_destroy (~22 KB per chunk point for the 8x256 network, ~5.8 GB at the default)
   // training (nm_train.cu): gradient accumulators per network + scratch
@@ -88,6 +99,11 @@ struct NmHandle_t {
 };
 
 namespace {
+
+constexpr int kOccMaxRes = 1024;     // cells per axis of an occupancy grid (two G^3-byte build volumes: 2 GB at 1024)
+OccLookup occ_lookup(NmHandle_t::OccGrid& g) {
+  return OccLookup{g.bits.as<uint32_t>(), {g.lo[0], g.lo[1], g.lo[2]}, {g.inv[0], g.inv[1], g.inv[2]}, g.G};
+}
 
 // points per network launch of the super-sampled mesh emit (16 B of workspace each: 64 MB at 4 Mi); NM_SS_CHUNK_POINTS
 // overrides it, read per call (the tests cross chunk boundaries with small values)
@@ -128,6 +144,14 @@ long long sigma_grad_chunk_points() {
   const char* e = getenv("NM_SIGMA_GRAD_CHUNK_POINTS");
   const long long x = e ? atoll(e) : 0;
   return x > 0 ? x : (1ll << 18);
+}
+
+// points per network launch of the skipping render (40 B of workspace each: 160 MB at 4 Mi); NM_SKIP_CHUNK_POINTS
+// overrides it, read per call (the tests cross launch boundaries with small values)
+long long skip_chunk_points() {
+  const char* e = getenv("NM_SKIP_CHUNK_POINTS");
+  const long long x = e ? atoll(e) : 0;
+  return x > 0 ? x : (1ll << 22);
 }
 
 // rays per internal chunk (bounds the per-sample workspace: 20 B x 192 samples x 1 Mi rays = 4 GB); NM_CHUNK_RAYS overrides (tests)
@@ -249,6 +273,49 @@ int render_chunk(NmHandle h, const RayBatch& rb, int flags, uint64_t seed, const
   };
   const char* fe = getenv("NM_FUSED_COMPOSITE");       // read per call: the tests flip it to compare the two paths
   const bool fused_env = !fe || atoi(fe) != 0;
+  const bool skip = flags & NM_FLAG_SKIP_EMPTY;
+  if (skip) {
+    NM_CHECK(!training && !teacher && !need_raw && !emit_c && !emit_f,
+             "NM_FLAG_SKIP_EMPTY is an inference path: it takes neither NM_FLAG_TRAINING nor NM_FLAG_TEACHER_T");
+    for (int k = 0; k < ((Nf > 0) ? 2 : 1); ++k)
+      NM_CHECK(h->occ[k].valid, "NM_FLAG_SKIP_EMPTY: no occupancy grid for network %d (nm_build_occupancy / nm_set_occupancy; "
+               "loading that network's weights drops its grid)", k);
+  }
+  // empty-space skipping (DESIGN §4.15): only the samples network `which`'s grid marks go through it, as explicit points in
+  // launches of at most skip_chunk_points(); every other sample enters the compositor as raw (0,0,0,0)
+  auto skip_raw = [&](int which, Buf& raw_buf, const float* t, int s) -> int {
+    NmHandle_t::OccGrid& g = h->occ[which];
+    const long long n = R * s;
+    NM_CHECK(n + 1 < (1ll << 31), "NM_FLAG_SKIP_EMPTY: %lld samples in one chunk exceed the int32 index list (lower NM_CHUNK_RAYS)", n);
+    const long long P = skip_chunk_points();
+    const size_t nb = (size_t)(n + 1) * 4, nblk = (size_t)((n + 1 + kScanBlockEntries - 1) / kScanBlockEntries) * 4;
+    const long long cap = P < n ? P : (n > 0 ? n : 1);
+    const size_t o_pos = (nb + 255) & ~(size_t)255, o_blk = 2 * o_pos, o_idx = o_blk + ((nblk + 255) & ~(size_t)255);
+    const size_t o_pts = o_idx + o_pos, o_dir = o_pts + (((size_t)cap * 12 + 255) & ~(size_t)255);
+    const size_t o_out = o_dir + (((size_t)cap * 12 + 255) & ~(size_t)255), bytes = o_out + (size_t)cap * 16;
+    if (int e = h->sk_ws.ensure(bytes)) return e;
+    uint8_t* ws = h->sk_ws.as<uint8_t>();
+    int* idx = reinterpret_cast<int*>(ws + o_idx);
+    long long M = 0;
+    if (int e = occ_compact(occ_lookup(g), rb.origins, rb.o_stride, rb.dirs, t, R, s, reinterpret_cast<int*>(ws), reinterpret_cast<int*>(ws + o_pos),
+                            reinterpret_cast<int*>(ws + o_blk), idx, &M, st, &h->launches)) return e;
+    h->skip_counts[2 * which] += n;
+    h->skip_counts[2 * which + 1] += M;
+    if (int e = raw_buf.ensure((size_t)n * 16)) return e;
+    NM_CUDA(cudaMemsetAsync(raw_buf.p, 0, (size_t)n * 16, st));
+    float* pts = reinterpret_cast<float*>(ws + o_pts);
+    float* dirs = reinterpret_cast<float*>(ws + o_dir);
+    float* out = reinterpret_cast<float*>(ws + o_out);
+    for (long long j0 = 0; j0 < M; j0 += P) {
+      const long long m = (M - j0 < P) ? M - j0 : P;
+      if (int e = launch_occ_stage(idx + j0, m, s, rb.origins, rb.o_stride, rb.dirs, t, pts, dirs, st, &h->launches)) return e;
+      MlpInput in{};
+      in.mode = IN_POINTS; in.pts = pts; in.dirs = dirs; in.M = m;
+      if (int e = run_mlp(h, which, false, in, out, st)) return e;
+      if (int e = launch_occ_expand(out, idx + j0, m, raw_buf.as<float>(), st, &h->launches)) return e;
+    }
+    return 0;
+  };
   // network `which` on the samples t (R,s) + VolumeRenderer: one launch when eligible, else raw (R,s,4) through `raw_buf`
   auto mlp_composite = [&](int which, Buf& raw_buf, const MlpEmit* emit, const float* t, int s, float* rgb, float* depth,
                            float* depth_raw, float* acc, float* disp, float* w, float* mw, uint64_t salt = kNoiseSaltMain) -> int {
@@ -256,6 +323,11 @@ int render_chunk(NmHandle h, const RayBatch& rb, int flags, uint64_t seed, const
     a.t = t; a.dirs = rb.dirs; a.R = R; a.S = s; a.noise_std = c.noise_std; a.seed = seed ^ salt;
     a.white_bg = c.white_background; a.training = training ? 1 : 0; a.thr = c.attenuation_threshold;
     a.rgb = rgb; a.depth = depth; a.depth_raw = depth_raw; a.acc = acc; a.disp = disp; a.weights = w; a.mask_weights = mw;
+    if (skip) {
+      if (int e = skip_raw(which, raw_buf, t, s)) return e;
+      a.raw = raw_buf.as<float>();
+      return launch_composite(a, st, &h->launches);
+    }
     const bool fuse = fused_env && !need_raw && !emit && c.precision != NM_PREC_FP32 && mlp_tc_composite_group(s) > 0;
     if (fuse) return run_mlp(h, which, false, rays_input(t, s), nullptr, st, nullptr, &a);
     if (int e = raw_buf.ensure((size_t)R * s * 16)) return e;
@@ -551,7 +623,8 @@ int nm_destroy(NmHandle h) {
   for (int i = 0; i < 2; ++i) { h->g_wt[i].release(); h->g_bias[i].release(); h->g_head[i].release(); h->tr_rgb[i].release(); h->tr_drgb[i].release(); }
   h->train_ws.release(); h->dout.release(); h->trans.release();
   h->ss_tab.release(); h->ss_ws.release(); h->ms_ws.release(); h->nn_ws.release(); h->sg_ws.release();
-  h->cc_ws.release(); h->dc_ws.release(); h->sp_ws.release(); h->tx_ws.release(); h->rs_ws.release(); h->sf_ws.release(); h->mc_ws.release(); h->mc_ws2.release();
+  h->cc_ws.release(); h->dc_ws.release(); h->sp_ws.release(); h->tx_ws.release(); h->rs_ws.release(); h->sf_ws.release(); h->oc_ws.release(); h->sk_ws.release();
+  h->occ[0].bits.release(); h->occ[1].bits.release(); h->mc_ws.release(); h->mc_ws2.release();
   if (h->h_err) cudaFreeHost(h->h_err);
   cudaFree(h->d_stats);
   for (cudaEvent_t e : h->ev) cudaEventDestroy(e);
@@ -578,6 +651,7 @@ int nm_load_weights(NmHandle h, int which, int n_tensors, const char* const* nam
   NM_CHECK(which == NM_NET_COARSE || (which == NM_NET_FINE && h->has_fine), "network slot %d not present", which);
   WeightSource src;
   src.n = n_tensors; src.names = names; src.ptrs = tensors_host; src.numel = numel;
+  h->occ[which].valid = false;     // a grid describes the weights it was built from
   return pack_network(h->desc[which], src, &h->nets[which]);
 }
 
@@ -587,6 +661,7 @@ int nm_load_weights_dev(NmHandle h, int which, int n_tensors, const char* const*
   NM_CHECK(which == NM_NET_COARSE || (which == NM_NET_FINE && h->has_fine), "network slot %d not present", which);
   WeightSource src;
   src.n = n_tensors; src.names = names; src.ptrs = tensors_dev; src.numel = numel;
+  h->occ[which].valid = false;     // a grid describes the weights it was built from
   return load_network_dev(h->desc[which], src, &h->nets[which], (cudaStream_t)stream, &h->launches);
 }
 
@@ -1419,6 +1494,112 @@ double nm_mlp_time_ms(NmHandle h, int64_t* points_out, int64_t* launches_out) {
   if (launches_out) *launches_out = h->mlp_launches;
   h->ev_used = 0; h->mlp_points = 0; h->mlp_launches = 0;
   return total;
+}
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------------------------- empty-space skipping
+namespace {
+int occ_params(NmHandle h, int which, const float* box, int G, NmHandle_t::OccGrid* g) {
+  NM_CHECK(which == NM_NET_COARSE || (which == NM_NET_FINE && h->has_fine), "network slot %d not present", which);
+  NM_CHECK(box, "null box");
+  NM_CHECK(G >= 1 && G <= kOccMaxRes, "occupancy resolution %d outside [1, %d]", G, kOccMaxRes);
+  for (int a = 0; a < 3; ++a) {
+    const float lo = box[a], hi = box[3 + a];
+    NM_CHECK(std::isfinite(lo) && std::isfinite(hi) && lo < hi, "occupancy box axis %d: [%g, %g] is not a finite interval", a, lo, hi);
+    const float inv = (float)((double)G / ((double)hi - (double)lo));
+    NM_CHECK(std::isfinite(inv) && inv > 0.f, "occupancy box axis %d: G / (hi - lo) is not finite", a);
+    g->lo[a] = lo; g->hi[a] = hi; g->inv[a] = inv;
+  }
+  g->G = G;
+  return 0;
+}
+size_t occ_words(int G) { return (size_t)(((long long)G * G * G + 31) / 32); }
+}  // namespace
+
+extern "C" {
+
+int nm_build_occupancy(NmHandle h, int which, const float* box_host, int G, float threshold, int dilate,
+                       uint32_t* bits_out_dev_or_null, void* stream) {
+  if (int e = bind_checked(h)) return e;
+  NmHandle_t::OccGrid p{};
+  if (int e = occ_params(h, which, box_host, G, &p)) return e;
+  NM_CHECK(!std::isnan(threshold), "occupancy threshold is NaN");
+  NM_CHECK(dilate >= 0 && dilate <= G, "occupancy dilation %d outside [0, %d]", dilate, G);
+  NmHandle_t::OccGrid& g = h->occ[which];
+  g.valid = false;
+  cudaStream_t st = (cudaStream_t)stream;
+  // torch.linspace(lo, hi, G+1) in fp32: step = (hi - lo) / G, lo + step*i below the midpoint and hi - step*(G-i) from it,
+  // each one fused multiply-add (ATen's two-sided formula; the values torch returns on the CPU and the GPU)
+  const long long n1 = G + 1, plane = n1 * n1;
+  std::vector<float> lins(3 * n1);
+  for (int a = 0; a < 3; ++a) {
+    const float step = (p.hi[a] - p.lo[a]) / (float)G;
+    for (long long i = 0; i < n1; ++i)
+      lins[a * n1 + i] = (i < n1 / 2) ? std::fmaf(step, (float)i, p.lo[a]) : std::fmaf(-step, (float)(G - i), p.hi[a]);
+  }
+  // the lattice is swept in slabs of cells [x0, x1) whose planes [x0, x1] hold at most 4 Mi points (16 MB)
+  const long long cells_per = std::max(1ll, std::min((long long)G, (1ll << 22) / plane - 1));
+  const size_t cube = (size_t)G * G * G;
+  const size_t o_sig = ((size_t)3 * n1 * 4 + 255) & ~(size_t)255;
+  const size_t o_a = o_sig + (((size_t)(cells_per + 1) * plane * 4 + 255) & ~(size_t)255), o_b = o_a + ((cube + 255) & ~(size_t)255);
+  if (int e = h->oc_ws.ensure(o_b + cube)) return e;
+  if (int e = g.bits.ensure(occ_words(G) * 4)) return e;
+  uint8_t* ws = h->oc_ws.as<uint8_t>();
+  float* lin = reinterpret_cast<float*>(ws);
+  NM_CUDA(cudaMemcpyAsync(lin, lins.data(), lins.size() * 4, cudaMemcpyHostToDevice, st));
+  float* sigma = reinterpret_cast<float*>(ws + o_sig);
+  for (long long x0 = 0; x0 < G; x0 += cells_per) {
+    const long long x1 = std::min((long long)G, x0 + cells_per);
+    MlpInput in{};
+    in.mode = IN_GRID;
+    in.lin0 = lin; in.lin1 = lin + n1; in.lin2 = lin + 2 * n1;
+    in.n1 = (int)n1; in.n2 = (int)n1;
+    in.grid_base = x0 * plane;
+    in.M = (x1 - x0 + 1) * plane;
+    if (int e = run_mlp(h, which, true, in, sigma, st)) return e;
+    if (int e = launch_occ_corners(sigma, G, (int)x0, (int)x1, threshold, ws + o_a, st, &h->launches)) return e;
+  }
+  if (int e = launch_occ_dilate_pack(ws + o_a, ws + o_b, G, dilate, g.bits.as<uint32_t>(), st, &h->launches)) return e;
+  if (bits_out_dev_or_null)
+    NM_CUDA(cudaMemcpyAsync(bits_out_dev_or_null, g.bits.p, occ_words(G) * 4, cudaMemcpyDeviceToDevice, st));
+  NM_CUDA(cudaStreamSynchronize(st));      // the host copy of `lins` must outlive its transfer
+  memcpy(g.lo, p.lo, sizeof(p.lo)); memcpy(g.hi, p.hi, sizeof(p.hi)); memcpy(g.inv, p.inv, sizeof(p.inv));
+  g.G = G;
+  g.valid = true;
+  return 0;
+}
+
+int nm_set_occupancy(NmHandle h, int which, const float* box_host, int G, const uint32_t* bits_dev_or_null) {
+  if (int e = bind_checked(h)) return e;
+  NM_CHECK(which == NM_NET_COARSE || (which == NM_NET_FINE && h->has_fine), "network slot %d not present", which);
+  NmHandle_t::OccGrid& g = h->occ[which];
+  g.valid = false;
+  if (!bits_dev_or_null) return 0;
+  NmHandle_t::OccGrid p{};
+  if (int e = occ_params(h, which, box_host, G, &p)) return e;
+  if (int e = g.bits.ensure(occ_words(G) * 4)) return e;
+  NM_CUDA(cudaMemcpy(g.bits.p, bits_dev_or_null, occ_words(G) * 4, cudaMemcpyDeviceToDevice));
+  memcpy(g.lo, p.lo, sizeof(p.lo)); memcpy(g.hi, p.hi, sizeof(p.hi)); memcpy(g.inv, p.inv, sizeof(p.inv));
+  g.G = G;
+  g.valid = true;
+  return 0;
+}
+
+int nm_occupancy_query(NmHandle h, int which, const float* pts_dev, int64_t M, uint8_t* evaluated_out_dev, void* stream) {
+  if (int e = bind_checked(h)) return e;
+  NM_CHECK(which == NM_NET_COARSE || (which == NM_NET_FINE && h->has_fine), "network slot %d not present", which);
+  NM_CHECK(h->occ[which].valid, "no occupancy grid for network %d", which);
+  NM_CHECK(M >= 0 && (M == 0 || (pts_dev && evaluated_out_dev)), "bad arguments");
+  return launch_occ_query(occ_lookup(h->occ[which]), pts_dev, M, evaluated_out_dev, (cudaStream_t)stream, &h->launches);
+}
+
+int nm_skip_stats(NmHandle h, int64_t* out_host) {
+  if (int e = bind_device(h)) return e;
+  NM_CHECK(out_host, "null argument");
+  NM_CUDA(cudaDeviceSynchronize());
+  for (int i = 0; i < 4; ++i) { out_host[i] = h->skip_counts[i]; h->skip_counts[i] = 0; }
+  return 0;
 }
 
 }  // extern "C"

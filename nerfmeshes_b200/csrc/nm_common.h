@@ -369,4 +369,36 @@ size_t surface_ws_bytes(long long H, long long W);
 int surface_points(const SurfaceView& v, float* pts, float* nrm, float* col, int32_t* pix, int64_t* count_host, void* ws,
                    cudaStream_t st, int64_t* launches);
 
+// occupancy grids for empty-space skipping (nm_occupancy.cu, DESIGN §4.15): G^3 cells over [lo, hi), bit (i*G + j)*G + k of
+// uint32 words; inv[a] = G / (hi[a] - lo[a]) rounded once on the host
+struct OccLookup {
+  const uint32_t* bits;
+  float lo[3], inv[3];
+  int G;
+};
+// true when the network must evaluate point p: outside [0, G) on an axis, not finite, or in an occupied cell.  The cell is
+// floor((p_a - lo_a) * inv_a) in round-to-nearest fp32, the restatement tests/_occupancy_ref.py makes.
+__device__ __forceinline__ bool occ_evaluated(const OccLookup& g, const float p[3]) {
+  long long cell = 0;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const float f = floorf(__fmul_rn(__fsub_rn(p[a], g.lo[a]), g.inv[a]));
+    if (!(f >= 0.f && f < (float)g.G)) return true;
+    cell = cell * g.G + (int)f;
+  }
+  return (__ldg(g.bits + (cell >> 5)) >> (cell & 31)) & 1u;
+}
+// build: raw occupancy bytes of cells [x0, x1) x G x G from the sigma lattice planes [x0, x1] ((x1-x0+1) x (G+1) x (G+1));
+// then the dilation by d cells (ping-pong a / b, G^3 bytes each; a holds the raw bytes) and the bit packing
+int launch_occ_corners(const float* sigma, int G, int x0, int x1, float thr, uint8_t* raw, cudaStream_t st, int64_t* launches);
+int launch_occ_dilate_pack(uint8_t* a, uint8_t* b, int G, int d, uint32_t* bits, cudaStream_t st, int64_t* launches);
+// render: the flat indices of the samples of (R,S) t the network must evaluate, ascending, into idx; *count_host = their
+// number.  mark / pos: R*S + 1 ints, blk: ceil((R*S + 1) / kScanBlockEntries) ints.  Synchronises `st` once (the count).
+int occ_compact(const OccLookup& g, const float* origins, int o_stride, const float* dirs, const float* t, long long R, int S,
+                int* mark, int* pos, int* blk, int* idx, long long* count_host, cudaStream_t st, int64_t* launches);
+int launch_occ_stage(const int* idx, long long cnt, int S, const float* origins, int o_stride, const float* dirs, const float* t,
+                     float* pts, float* dirs_out, cudaStream_t st, int64_t* launches);
+int launch_occ_expand(const float* sub, const int* idx, long long cnt, float* raw, cudaStream_t st, int64_t* launches);
+int launch_occ_query(const OccLookup& g, const float* pts, long long M, uint8_t* out, cudaStream_t st, int64_t* launches);
+
 }  // namespace nm

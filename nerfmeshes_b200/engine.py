@@ -69,6 +69,9 @@ def raster_faces(faces, device) -> torch.Tensor:
 class Engine:
     """Owns one library handle on one CUDA device."""
 
+    # the default of render_rays / render_image's skip_empty outside training (BaseModel.build_occupancy_grid sets it)
+    skip_empty = False
+
     def __init__(self, coarse: dict, fine: Optional[dict], settings: RenderSettings, device: int = 0):
         self.lib = L.load()
         if not torch.cuda.is_available():
@@ -80,6 +83,7 @@ class Engine:
         dc = net_desc(**coarse)
         df = net_desc(**fine) if fine is not None else None
         cfg = settings.to_c()
+        self._occupancy = set()         # network slots with a grid built from their current weights (a weight load drops it)
         L.check(self.lib.nm_create(device, C.byref(dc), C.byref(df) if df is not None else None, C.byref(cfg),
                                    C.byref(self._h)))
 
@@ -121,6 +125,7 @@ class Engine:
             keep.append(a)
             names.append(k.encode())
         n = len(names)
+        self._occupancy.discard(which)
         args = (self._h, which, n, (C.c_char_p * n)(*names), (C.c_void_p * n)(*ptrs), (C.c_int64 * n)(*numel))
         if on_dev:
             L.check(self.lib.nm_load_weights_dev(*args, self._stream()))
@@ -202,9 +207,11 @@ class Engine:
     DEFAULT_OUT = ("rgb", "depth", "depth_raw", "acc", "disp", "weights", "mask_weights")
 
     def render_rays(self, origins, dirs, near, far, *, training=False, buff=False, seed=0, want=None,
-                    teacher_t: Optional[torch.Tensor] = None, out=None) -> Dict[str, torch.Tensor]:
+                    teacher_t: Optional[torch.Tensor] = None, out=None, skip_empty=None) -> Dict[str, torch.Tensor]:
         """NeRFModel.forward / BuFFModel.forward on a ray batch.  origins (3,), (1,3) or (R,3); dirs (R,3);
-        near/far python floats / 0-dim tensors, or (R,) tensors (CUDA path only)."""
+        near/far python floats / 0-dim tensors, or (R,) tensors (CUDA path only).  skip_empty: send only the samples the
+        occupancy grids mark through the networks (NM_FLAG_SKIP_EMPTY, DESIGN 4.15); None = `self.skip_empty` outside
+        training."""
         want = tuple(want or self.DEFAULT_OUT)
         dirs_t = torch.as_tensor(dirs)
         host = not dirs_t.is_cuda
@@ -218,7 +225,7 @@ class Engine:
         else:
             assert o.shape == (R, 3), "origins must be (3,), (1,3) or (R,3)"
             o_stride = 3
-        flags = self._flags(training, buff)
+        flags = self._flags(training, buff, skip_empty)
         S = self.num_samples(buff)
         per_ray = isinstance(near, torch.Tensor) and near.dim() > 0 and near.shape[0] == R and near.numel() == R and R > 1
         nf = (C.c_float * 2)(0.0, 0.0)
@@ -297,10 +304,71 @@ class Engine:
         return out
 
     # ------------------------------------------------------------------ BuFF tree maintenance (SURVEY §8f-4)
-    def _flags(self, training, buff):
-        """render-call flags; `voxel_random` mirrors cfg.tree.use_random_sampling (src/nerf/tree.py:280)."""
+    def _flags(self, training, buff, skip_empty=None):
+        """render-call flags; `voxel_random` mirrors cfg.tree.use_random_sampling (src/nerf/tree.py:280).  skip_empty None
+        follows `self.skip_empty` outside training; an explicit True is passed on as asked (the library rejects it in
+        training)."""
+        skip = (self.skip_empty and not training) if skip_empty is None else bool(skip_empty)
+        if skip:
+            for which in ((L.NET_COARSE,) if buff or not self.has_fine else (L.NET_COARSE, L.NET_FINE)):
+                if which not in self._occupancy:
+                    raise L.NmError(f"empty-space skipping: network {which} has no occupancy grid for its current weights "
+                                    "(the weights changed after build_occupancy_grid, or none was built); call "
+                                    "build_occupancy_grid again")
         return ((L.FLAG_TRAINING if training else 0) | (L.FLAG_BUFF if buff else 0) |
-                (L.FLAG_RANDOM_VOXELS if buff and getattr(self, "voxel_random", False) else 0))
+                (L.FLAG_RANDOM_VOXELS if buff and getattr(self, "voxel_random", False) else 0) |
+                (L.FLAG_SKIP_EMPTY if skip else 0))
+
+    # ------------------------------------------------------------------ empty-space skipping (DESIGN 4.15)
+    @staticmethod
+    def occupancy_words(res: int) -> int:
+        return (res ** 3 + 31) // 32
+
+    @staticmethod
+    def _box(box):
+        b = np.ascontiguousarray(np.asarray(box, dtype=np.float32).reshape(-1))
+        if b.size != 6:
+            raise ValueError("an occupancy box is (lo_x, lo_y, lo_z, hi_x, hi_y, hi_z)")
+        return b
+
+    def build_occupancy(self, which: int, box, res: int = 128, threshold: float = 0.0, dilate: int = 0) -> torch.Tensor:
+        """Occupancy grid of network `which` from its own density (nm_build_occupancy): res^3 cells over box (lo3, hi3); a
+        cell is occupied when the max raw sigma of its 8 lattice corners is > threshold (or NaN), dilated by `dilate` cells.
+        Returns the bits, ceil(res^3 / 32) words (int32 device tensor, bit (i*res + j)*res + k)."""
+        b = self._box(box)
+        bits = torch.empty(self.occupancy_words(res), dtype=torch.int32, device=self.device)
+        self._occupancy.discard(which)
+        L.check(self.lib.nm_build_occupancy(self._h, which, b.ctypes.data, int(res), float(threshold), int(dilate), _ptr(bits),
+                                            self._stream()))
+        self._occupancy.add(which)
+        return bits
+
+    def set_occupancy(self, which: int, box, res: int, bits: Optional[torch.Tensor]):
+        """Install caller bits (layout of build_occupancy) as network `which`'s grid; None removes it."""
+        self._occupancy.discard(which)
+        if bits is None:
+            L.check(self.lib.nm_set_occupancy(self._h, which, None, 0, None))
+            return
+        b = self._box(box)
+        w = bits.to(self.device).contiguous()
+        assert w.dtype in (torch.int32, torch.uint32) and w.numel() == self.occupancy_words(res), (w.dtype, w.numel())
+        torch.cuda.current_stream(self.device).synchronize()
+        L.check(self.lib.nm_set_occupancy(self._h, which, b.ctypes.data, int(res), _ptr(w)))
+        self._occupancy.add(which)
+
+    def occupancy_query(self, which: int, pts: torch.Tensor) -> torch.Tensor:
+        """bool (...) per point (...,3): True where a skipping render evaluates the point under network `which`'s grid."""
+        lead = pts.shape[:-1]
+        p = _f32c(pts, self.device).reshape(-1, 3)
+        out = torch.empty(p.shape[0], dtype=torch.uint8, device=self.device)
+        L.check(self.lib.nm_occupancy_query(self._h, which, _ptr(p), p.shape[0], _ptr(out), self._stream()))
+        return out.bool().reshape(lead)
+
+    def skip_stats(self) -> Dict[str, int]:
+        """Samples seen / evaluated per pass by skipping renders since the last call (nm_skip_stats); resets them."""
+        out = (C.c_int64 * 4)()
+        L.check(self.lib.nm_skip_stats(self._h, out))
+        return dict(coarse_seen=out[0], coarse_evaluated=out[1], fine_seen=out[2], fine_evaluated=out[3])
 
     def ray_voxel_indices(self, origins, dirs, near, far, want_z=False, seed=0):
         """(R,S) int32 voxel index of every AABB sample (-1 on rays without a hit) [, (R,S) sample distances].  With
@@ -372,14 +440,15 @@ class Engine:
         return out
 
     def render_image(self, pose, H, W, focal, near, far, *, ndc=False, rows=None, training=False, buff=False, seed=0,
-                     want=None, to_host=False, host_out=None, out=None) -> Dict[str, torch.Tensor]:
-        """Rays generated on the device from a 3x4 / 4x4 camera-to-world pose (get_ray_bundle [+ ndc_rays])."""
+                     want=None, to_host=False, host_out=None, out=None, skip_empty=None) -> Dict[str, torch.Tensor]:
+        """Rays generated on the device from a 3x4 / 4x4 camera-to-world pose (get_ray_bundle [+ ndc_rays]).  skip_empty:
+        as in render_rays."""
         want = tuple(want or ("rgb", "depth", "acc", "disp"))
         row0, row1 = rows if rows is not None else (0, H)
         R = (row1 - row0) * W
         p = np.ascontiguousarray(torch.as_tensor(pose).detach().cpu().numpy()[:3, :4], dtype=np.float32)
         nf = (C.c_float * 2)(float(near), float(far))
-        flags = self._flags(training, buff)
+        flags = self._flags(training, buff, skip_empty)
         S = self.num_samples(buff)
         if to_host:
             if host_out is not None:

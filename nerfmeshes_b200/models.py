@@ -139,6 +139,7 @@ class BaseModel(torch.nn.Module):
 
     precision = L.PREC_EXACT
     act_scale_log2 = 0
+    skip_empty = False          # eval-mode renders skip empty space (build_occupancy_grid sets it; DESIGN 4.15)
 
     def __init__(self, cfg, *args, **kwargs):
         super().__init__()
@@ -208,7 +209,32 @@ class BaseModel(torch.nn.Module):
         s = self._render_settings()
         if s != self._eng.settings:
             self._eng.configure(**s.__dict__)
+        self._eng.skip_empty = bool(self.skip_empty) and not self.training     # training renders stay dense
         return self._eng
+
+    def build_occupancy_grid(self, res: int = 128, box=None, threshold: float = -10.0, dilate: int = 2):
+        """Occupancy grids of every network from its own density (Engine.build_occupancy, DESIGN 4.15), then skip_empty:
+        eval-mode renders (forward, query, eval_poses, render_image_sharded, surface_points, compare_with_nerf) send only
+        the samples in occupied cells, outside the box or not finite through the networks.  A ray's outputs are the dense
+        render's bits whenever every sample skipped on it has raw sigma <= 0 (the defaults are chosen so that this holds
+        for nearly every ray of the lego and fern scenes; DESIGN 4.15 has the numbers).  box: (lo_x, lo_y, lo_z, hi_x, hi_y,
+        hi_z) in network-input coordinates; default [near - mean, far - mean]^3 with mean = (near + far) / 2 (the BuFF
+        tree's root box); an NDC model needs an explicit box.  Changing the weights afterwards makes the next skipping
+        render raise until the grids are built again.  Returns {slot: bits}."""
+        if box is None:
+            if _cfg_get(self.cfg, "dataset.use_ndc", False):
+                raise L.NmError("build_occupancy_grid: an NDC model needs an explicit box (NDC coordinates)")
+            near, far = float(self.cfg.dataset.near), float(self.cfg.dataset.far)
+            mean = (near + far) / 2
+            box = [near - mean] * 3 + [far - mean] * 3
+        eng = self._engine()
+        out = {}
+        for which, net in enumerate(self._nets()):
+            if net is not None:
+                out[which] = eng.build_occupancy(which, box, res, threshold, dilate)
+        self.skip_empty = True
+        self._engine()
+        return out
 
     def _after_engine_created(self):
         pass
