@@ -382,9 +382,9 @@ int nm_export_ply(const char* path, const float* points_host, const float* color
  * (ceil(G^3 / 32) of them).  A point p is EVALUATED when, for some axis a, c_a = floor((p_a - lo_a) * inv_a) is outside [0, G)
  * or not finite (fp32, a rounded subtract then a rounded multiply; inv_a = G / (hi_a - lo_a) rounded once), or when its cell's
  * bit is set.  With NM_FLAG_SKIP_EMPTY a render sends only evaluated samples through the network; every other sample enters
- * the compositor as raw (0,0,0,0), i.e. alpha = 0.  Guarantee: every output of a ray (rgb, depth, depth_raw, acc, disp,
- * weights, mask_weights, t_vals, coarse_*) is bit-identical to the render without the flag when every sample the grid skipped
- * on that ray has a dense raw sigma <= 0 or NaN.  A skipping render reads each pass's sample count back to the host (one
+ * the compositor as raw (0,0,0,-inf), i.e. alpha = 0 whatever the sigma noise.  Guarantee: every output of a ray (rgb, depth,
+ * depth_raw, acc, disp, weights, mask_weights, t_vals, coarse_*) is bit-identical to the render without the flag when every
+ * sample the grid skipped on that ray has a dense noisy pre-activation (raw sigma + the pass's noise) <= 0 or NaN.  A skipping render reads each pass's sample count back to the host (one
  * small copy and one stream synchronisation per pass per NM_CHUNK_RAYS chunk), so it cannot be captured in a CUDA graph; the
  * network runs on at most NM_SKIP_CHUNK_POINTS points per launch (default 4 Mi).  Loading a network's weights drops its grid.
  *
@@ -476,6 +476,15 @@ int nm_debug_mlp_backward(NmHandle h, int which, const float* pts_dev, const flo
 int nm_debug_composite_backward(NmHandle h, const float* raw_dev, const float* t_dev, const float* dirs_dev,
                                 const float* d_rgb_dev, int64_t R, int S, float noise_std, uint64_t seed, int white_bg,
                                 float* dout_dev, void* stream);
+/* Test hook for the inference compositor alone (composite_kernel, nm_render.cu), with the arguments a render pass gives it:
+ * from raw_dev (R,S,4) = (sigmoid rgb, raw sigma), t_dev (R,S) and dirs_dev (R,3) it writes the non-NULL fields rgb, depth,
+ * depth_raw, acc, disp, weights and mask_weights of out_dev (a host struct of device pointers; every other field must be
+ * NULL).  noise_std and seed are the pass's sigma noise, seed already salted (a render passes its chunk seed ^ the pass's
+ * salt); training = 1 leaves depth unthresholded; thr is the mask_weights threshold.  1 <= S <= 512; raw_dev 16-byte
+ * aligned; argument errors are rejected before anything is launched; R = 0 launches nothing. */
+int nm_debug_composite(NmHandle h, const float* raw_dev, const float* t_dev, const float* dirs_dev, int64_t R, int S,
+                       float noise_std, uint64_t seed, int white_bg, int training, float thr, const NmRenderOut* out_dev,
+                       void* stream);
 /* Test hook for the inverse-CDF resampler alone (invcdf_kernel, nm_render.cu), the call a two-network render makes: from
  * the coarse depths t_c_dev (R,Nc), ascending per ray, and the coarse weights w_c_dev (R,Nc) it writes t_out_dev (R,Nc+Nf),
  * the coarse depths and Nf new samples merged in ascending order.  perturb = 0 places the samples at u_dev (Nf); otherwise

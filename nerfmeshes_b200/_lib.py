@@ -94,6 +94,7 @@ _SIGNATURES = {
     "nm_debug_gemm": (C.c_int, [_P, _P, _P, _I, _I, _I, _I, _P, _P]),
     "nm_debug_mlp_backward": (C.c_int, [_P, _I, _P, _P, _L, _P, _P]),
     "nm_debug_composite_backward": (C.c_int, [_P, _P, _P, _P, _P, _L, _I, _F, C.c_uint64, _I, _P, _P]),
+    "nm_debug_composite": (C.c_int, [_P, _P, _P, _P, _L, _I, _F, C.c_uint64, _I, _I, _F, C.POINTER(NmRenderOut), _P]),
     "nm_debug_sample_pdf": (C.c_int, [_P, _P, _P, _P, _L, _I, _I, _I, C.c_uint64, _P, _P]),
     "nm_debug_pack": (C.c_int, [C.POINTER(NmNetDesc), _I, C.POINTER(C.c_char_p), C.POINTER(_P), C.POINTER(C.c_int64), _I, _P,
                                C.c_size_t, _P, C.c_size_t, C.POINTER(C.c_size_t)]),

@@ -282,7 +282,8 @@ int render_chunk(NmHandle h, const RayBatch& rb, int flags, uint64_t seed, const
                "loading that network's weights drops its grid)", k);
   }
   // empty-space skipping (DESIGN §4.15): only the samples network `which`'s grid marks go through it, as explicit points in
-  // launches of at most skip_chunk_points(); every other sample enters the compositor as raw (0,0,0,0)
+  // launches of at most skip_chunk_points(); every other sample enters the compositor as raw (0,0,0,-inf), which the pass's
+  // sigma noise cannot lift above 0
   auto skip_raw = [&](int which, Buf& raw_buf, const float* t, int s) -> int {
     NmHandle_t::OccGrid& g = h->occ[which];
     const long long n = R * s;
@@ -297,12 +298,11 @@ int render_chunk(NmHandle h, const RayBatch& rb, int flags, uint64_t seed, const
     uint8_t* ws = h->sk_ws.as<uint8_t>();
     int* idx = reinterpret_cast<int*>(ws + o_idx);
     long long M = 0;
+    if (int e = raw_buf.ensure((size_t)n * 16)) return e;
     if (int e = occ_compact(occ_lookup(g), rb.origins, rb.o_stride, rb.dirs, t, R, s, reinterpret_cast<int*>(ws), reinterpret_cast<int*>(ws + o_pos),
-                            reinterpret_cast<int*>(ws + o_blk), idx, &M, st, &h->launches)) return e;
+                            reinterpret_cast<int*>(ws + o_blk), idx, raw_buf.as<float>(), &M, st, &h->launches)) return e;
     h->skip_counts[2 * which] += n;
     h->skip_counts[2 * which + 1] += M;
-    if (int e = raw_buf.ensure((size_t)n * 16)) return e;
-    NM_CUDA(cudaMemsetAsync(raw_buf.p, 0, (size_t)n * 16, st));
     float* pts = reinterpret_cast<float*>(ws + o_pts);
     float* dirs = reinterpret_cast<float*>(ws + o_dir);
     float* out = reinterpret_cast<float*>(ws + o_out);
@@ -846,6 +846,26 @@ int nm_debug_composite_backward(NmHandle h, const float* raw_dev, const float* t
   if (int e = h->trans.ensure((size_t)R * S * 4)) return e;
   return launch_composite_backward(raw_dev, t_dev, dirs_dev, d_rgb_dev, R, S, noise_std, seed, white_bg, h->trans.as<float>(),
                                    dout_dev, (cudaStream_t)stream, &h->launches);
+}
+
+int nm_debug_composite(NmHandle h, const float* raw_dev, const float* t_dev, const float* dirs_dev, int64_t R, int S,
+                       float noise_std, uint64_t seed, int white_bg, int training, float thr, const NmRenderOut* out_dev,
+                       void* stream) {
+  if (int e = bind_checked(h)) return e;
+  NM_CHECK(raw_dev && t_dev && dirs_dev && out_dev, "null pointer argument");
+  NM_CHECK(!out_dev->t_vals && !out_dev->coarse_rgb && !out_dev->coarse_acc && !out_dev->coarse_disp && !out_dev->coarse_weights,
+           "the compositor writes rgb, depth, depth_raw, acc, disp, weights and mask_weights only: the other fields must be NULL");
+  NM_CHECK(R >= 0, "negative ray count %lld", (long long)R);
+  NM_CHECK(S >= 1 && S <= 512, "samples per ray %d outside [1, 512]", S);
+  NM_CHECK((reinterpret_cast<uintptr_t>(raw_dev) & 15) == 0, "raw must be a 16-byte aligned (R,S,4) array");
+  if (R == 0) return 0;
+  // the CompositeArgs render_chunk's mlp_composite builds, on the caller's arrays
+  CompositeArgs a{};
+  a.raw = raw_dev; a.t = t_dev; a.dirs = dirs_dev; a.R = R; a.S = S; a.noise_std = noise_std; a.seed = seed;
+  a.white_bg = white_bg ? 1 : 0; a.training = training ? 1 : 0; a.thr = thr;
+  a.rgb = out_dev->rgb; a.depth = out_dev->depth; a.depth_raw = out_dev->depth_raw; a.acc = out_dev->acc; a.disp = out_dev->disp;
+  a.weights = out_dev->weights; a.mask_weights = out_dev->mask_weights;
+  return launch_composite(a, (cudaStream_t)stream, &h->launches);
 }
 
 int nm_debug_sample_pdf(NmHandle h, const float* t_c_dev, const float* w_c_dev, const float* u_dev, int64_t R, int Nc, int Nf,

@@ -393,9 +393,10 @@ __device__ __forceinline__ bool occ_evaluated(const OccLookup& g, const float p[
 int launch_occ_corners(const float* sigma, int G, int x0, int x1, float thr, uint8_t* raw, cudaStream_t st, int64_t* launches);
 int launch_occ_dilate_pack(uint8_t* a, uint8_t* b, int G, int d, uint32_t* bits, cudaStream_t st, int64_t* launches);
 // render: the flat indices of the samples of (R,S) t the network must evaluate, ascending, into idx; *count_host = their
-// number.  mark / pos: R*S + 1 ints, blk: ceil((R*S + 1) / kScanBlockEntries) ints.  Synchronises `st` once (the count).
+// number; every other sample's row of raw (R,S,4) is set to (0,0,0,-inf), which no sigma noise lifts above 0.  mark / pos:
+// R*S + 1 ints, blk: ceil((R*S + 1) / kScanBlockEntries) ints.  Synchronises `st` once (the count).
 int occ_compact(const OccLookup& g, const float* origins, int o_stride, const float* dirs, const float* t, long long R, int S,
-                int* mark, int* pos, int* blk, int* idx, long long* count_host, cudaStream_t st, int64_t* launches);
+                int* mark, int* pos, int* blk, int* idx, float* raw, long long* count_host, cudaStream_t st, int64_t* launches);
 int launch_occ_stage(const int* idx, long long cnt, int S, const float* origins, int o_stride, const float* dirs, const float* t,
                      float* pts, float* dirs_out, cudaStream_t st, int64_t* launches);
 int launch_occ_expand(const float* sub, const int* idx, long long cnt, float* raw, cudaStream_t st, int64_t* launches);

@@ -6,12 +6,12 @@
 //           occ_dilate_kernel     one axis of the Chebyshev dilation by `dilate` cells (three passes, clamped at the faces)
 //           occ_pack_kernel       bit (i*G + j)*G + k of uint32 words
 //   render  occ_mark_kernel       per sample of one pass: 1 when the network must evaluate it (outside the box, not finite,
-//                                 or in an occupied cell)
+//                                 or in an occupied cell); a skipped sample's raw is (0,0,0,-inf) in the compositor's buffer
 //           exclusive_scan        of the marks (the grid search's integer scan, nm_chamfer.cu); one extra zero entry
 //                                 leaves the total at the end
 //           occ_compact_kernel    the evaluated samples' flat indices, ascending
 //           occ_stage_kernel      points o + d*t and directions of a range of the index list, for the IN_POINTS network
-//           occ_expand_kernel     the network's (M,4) raw into the zero-filled (R,S,4) buffer the compositor reads
+//           occ_expand_kernel     the network's (M,4) raw into the evaluated slots of the (R,S,4) buffer the compositor reads
 // Built with -fmad=false; the point and the cell index are explicit round-to-nearest operations in any case, so the sample
 // points equal fetch_point's IN_RAYS ones (nm_frontend.cuh) bit for bit and tests/_occupancy_ref.py restates the lookup.
 #include <math_constants.h>
@@ -86,12 +86,14 @@ __global__ void __launch_bounds__(kBlock) occ_pack_kernel(const uint8_t* __restr
 
 __global__ void __launch_bounds__(kBlock) occ_mark_kernel(const OccLookup g, const float* __restrict__ origins, int o_stride,
                                                            const float* __restrict__ dirs, const float* __restrict__ t, long long R,
-                                                           int S, int* __restrict__ mark) {
+                                                           int S, int* __restrict__ mark, float4* __restrict__ raw) {
   const long long m = (long long)blockIdx.x * kBlock + threadIdx.x;
   if (m >= R * S) return;
   float p[3], d[3];
   ray_point(origins, o_stride, dirs, m / S, __ldg(t + m), p, d);
-  mark[m] = occ_evaluated(g, p) ? 1 : 0;
+  const bool ev = occ_evaluated(g, p);
+  mark[m] = ev ? 1 : 0;
+  if (!ev) raw[m] = make_float4(0.f, 0.f, 0.f, -CUDART_INF_F);    // sigma + noise stays -inf: alpha = 0 whatever the noise
 }
 
 __global__ void __launch_bounds__(kBlock) occ_compact_kernel(const int* __restrict__ mark, const int* __restrict__ pos, long long n,
@@ -155,9 +157,9 @@ int launch_occ_dilate_pack(uint8_t* a, uint8_t* b, int G, int d, uint32_t* bits,
 }
 
 int occ_compact(const OccLookup& g, const float* origins, int o_stride, const float* dirs, const float* t, long long R, int S,
-                int* mark, int* pos, int* blk, int* idx, long long* count_host, cudaStream_t st, int64_t* launches) {
+                int* mark, int* pos, int* blk, int* idx, float* raw, long long* count_host, cudaStream_t st, int64_t* launches) {
   const long long n = R * S;
-  occ_mark_kernel<<<blocks_for(n), kBlock, 0, st>>>(g, origins, o_stride, dirs, t, R, S, mark);
+  occ_mark_kernel<<<blocks_for(n), kBlock, 0, st>>>(g, origins, o_stride, dirs, t, R, S, mark, reinterpret_cast<float4*>(raw));
   NM_CUDA(cudaGetLastError());
   NM_CUDA(cudaMemsetAsync(mark + n, 0, sizeof(int), st));
   if (int e = exclusive_scan(mark, n + 1, blk, pos, st)) return e;

@@ -425,6 +425,23 @@ class Engine:
                                                      int(seed) % 2 ** 64, int(white_bg), _ptr(out), self._stream()))
         return out
 
+    COMPOSITE_OUT = ("rgb", "depth", "depth_raw", "acc", "disp", "weights", "mask_weights")
+
+    def debug_composite(self, raw, t, dirs, *, noise_std=0.0, seed=0, white_bg=False, training=False, thr=1e-5, want=None):
+        """Test hook (nm_debug_composite): the inference compositor alone, as a render pass calls it.  raw (R,S,4) =
+        (sigmoid rgb, raw sigma), t (R,S), dirs (R,3); `seed` is the pass's salted noise stream, `thr` the mask_weights
+        threshold.  Returns the maps of `want` (default all seven: rgb, depth, depth_raw, acc, disp, weights, mask_weights)."""
+        q, tt, d = _f32c(raw, self.device), _f32c(t, self.device), _f32c(dirs, self.device)
+        R, S = tt.shape
+        assert q.shape == (R, S, 4) and d.shape == (R, 3), (q.shape, tt.shape, d.shape)
+        want = tuple(want or self.COMPOSITE_OUT)
+        assert set(want) <= set(self.COMPOSITE_OUT), want
+        outs, block = self._alloc_out(R, S, self.device, want)
+        L.check(self.lib.nm_debug_composite(self._h, _ptr(q), _ptr(tt), _ptr(d), R, S, float(noise_std), int(seed) % 2 ** 64,
+                                            int(bool(white_bg)), int(bool(training)), float(thr), C.byref(block),
+                                            self._stream()))
+        return outs
+
     def debug_sample_pdf(self, t_c, w_c, u=None, *, Nf=None, perturb=False, seed=0):
         """Test hook (nm_debug_sample_pdf): the inverse-CDF resampler alone.  t_c (R,Nc) ascending coarse depths, w_c (R,Nc)
         coarse weights; u (Nf,) the deterministic positions, or None with `perturb` (drawn from the salted stream `seed`).

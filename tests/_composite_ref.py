@@ -323,3 +323,273 @@ def make_rays(R, S, seed, kind_offset=0):
     raw = np.concatenate([c, sigma[..., None]], -1).astype(F32)
     d_rgb = rng.standard_normal((R, 3)).astype(F32)
     return raw, t, dirs, d_rgb, kinds
+
+
+# ===================================================================================================== forward compositor
+# The inference compositor (`composite_kernel`, nm_render.cu, and the compositor fused into the MLP kernel, nm_mlp_tc.cu:
+# both walk nm_composite.cuh's comp_alpha / comp_step / comp_finish): per ray, in sample order, alpha_i and keep_i as
+# above, w_i = alpha_i T_i, mask_i = [T_i > thr], rgb = sum w c (+ 1 - acc with a white background), acc = sum w,
+# depth_raw = sum w t, disp = 1 / max(1e-10f, depth_raw / acc) with NaN -> 0, depth = depth_raw but 0 where acc < 1 in eval.
+#
+# `composite_forward` is its float64 truth from the kernel's fp32 inputs, with the fp32 rules of the adjoint's truth
+# (alpha = 1, keep = 1e-10f once e <= 2^-25; the last dist 1e10f |d|), keep = 1 where alpha = 0, and one documented
+# deviation from
+# oracle.volume_render: a NaN noisy pre-activation gives alpha = 0 (the kernel's fmaxf(sigma, 0) drops the NaN; torch.relu
+# propagates it).  Everything else equals the oracle run in float64 (tests/test_composite_forward_reference.py).
+#
+# `forward_error_scale` bounds the kernel's fp32 error per output; with dpre, de, da, dkeep, rho and dT exactly as in
+# `error_scale` (T's relative rounding growing with the sample index as a log-sum of every factor's uncertainty, the
+# subnormal floor (idx + 8) 2^-149, alpha's 2^-24 grid next to 1, expf's <= 2 ulp inside (3 x + 3) u, the noise mismatch):
+#   dw_i     = alpha dT + (T + dT) da + u w + 2^-149                 (the product's own rounding, normal or subnormal)
+#   a sequential fp32 sum of terms a_i (every partial sum rounded once) errs by <= u sum_k |partial_k| <= u sum_k
+#   cumsum(|a|)_k, plus the propagated error of its terms:
+#   dacc     = sum dw + u sum cumsum(w)
+#   drgb_c   = sum (dw + u w) c + u sum cumsum(w c)         (+ dacc + u (|1 - acc| + |rgb|) with a white background)
+#   ddepth   = sum (dw + u w) |t| + u sum cumsum(w |t|)
+#   ddisp    = |disp| (ddepth / |depth| + dacc / acc + 3 u)         (the division, max's clamp (1-Lipschitz), reciprocal)
+# Outputs the truth makes NaN or +-inf must be the same bits' class (NaN / the same infinity), and are not scaled.
+# The discrete decisions are exact (scale 0) outside their undecided margins (scale inf): the noise gate (|pre| <= GATE_MU
+# |n|, which opens every later bound through dpre), mask_i where |T_i - thr| <= dT_i (+ the T rounding), depth where
+# |acc - 1| <= dacc + u, and disp where acc <= dacc (the kernel's acc may round to 0: 0/0 -> 0).  The mask has no margin
+# while T is exactly 1 in the kernel: at sample 0 (comp_init) and after samples of decided alpha = 0, whose fp32 keep
+# 1 + 1e-10f rounds to 1 (the truth takes keep = 1 there too), so a T == thr = 1 decision pins the strict T > thr.
+#
+# `emulate_forward` is the kernel's order in numpy fp32 and `FWD_FAULTS` its variants with one plausible bug each.
+FLT_MAX = float(np.finfo(np.float32).max)
+FWD_OUT = ("rgb", "depth", "depth_raw", "acc", "disp", "weights", "mask_weights")
+# Tolerance of tests/test_gpu_composite_forward.py: |kernel - truth| <= TAU_FWD * forward_error_scale, >= 4x the worst ratio
+# measured on an H100 80GB HBM3 (700 W limit) over the whole edge matrix [bracketed]; tests/test_composite_forward_reference.py
+# shows that the fp32 emulation stays within EMUL_WORST_FWD and that every variant of FWD_FAULTS exceeds TAU_FWD.
+TAU_FWD = 4.0                       # [0.994]
+EMUL_WORST_FWD = 1.0                # the fp32 emulation against the truth on the CPU edge matrix [0.984]
+
+
+@dataclass
+class Forward:
+    dist: np.ndarray
+    pre: np.ndarray
+    noise: np.ndarray
+    x: np.ndarray
+    e: np.ndarray
+    alpha: np.ndarray
+    keep: np.ndarray
+    T: np.ndarray
+    w: np.ndarray
+    thr: float
+    out: dict              # FWD_OUT -> float64 arrays (mask_weights 0 / 1)
+
+
+def composite_forward(raw, t, dirs, white_bg, training, thr, noise_std=0.0, seed=0) -> Forward:
+    """The float64 truth of the seven forward outputs (section comment above)."""
+    raw = np.asarray(raw, F32)
+    R, S = raw.shape[:2]
+    t = np.asarray(t, F32).astype(np.float64)
+    d = np.asarray(dirs, F32).astype(np.float64)
+    p32, n32 = noisy_pre(raw, noise_std, seed)
+    pre, noise = p32.astype(np.float64), n32.astype(np.float64)
+    with np.errstate(all="ignore"):
+        nrm = np.sqrt((d * d).sum(-1))[:, None]
+        dist = np.concatenate([t[:, 1:] - t[:, :-1], np.full((R, 1), BIG)], 1) * nrm
+        sg = np.where(pre > 0, pre, 0.0)                 # NaN -> 0: the kernel's fmaxf rule, not torch.relu's
+        x = sg * dist
+        e = np.exp(-x)
+        sat = e <= SAT_E
+        alpha = np.where(sat, 1.0, 1.0 - e)
+        keep = np.where(sat, K10, np.where(alpha == 0, 1.0, e + K10))     # fp32 1 + 1e-10f == 1: T stays exactly 1
+        T = np.cumprod(np.concatenate([np.ones((R, 1)), keep[:, :-1]], 1), 1)
+        w = alpha * T
+        c = raw[..., :3].astype(np.float64)
+        rgb = (w[..., None] * c).sum(1)
+        acc = w.sum(1)
+        depth_raw = (w * t).sum(1)
+        ratio = depth_raw / acc
+        disp = 1.0 / np.maximum(K10, ratio)
+        disp = np.where(np.isnan(ratio) | np.isnan(disp), 0.0, disp)
+        depth = depth_raw if training else np.where(acc < 1.0, 0.0, depth_raw)
+        if white_bg:
+            rgb = rgb + (1.0 - acc)[:, None]
+    out = dict(rgb=rgb, depth=depth, depth_raw=depth_raw, acc=acc, disp=disp, weights=w,
+               mask_weights=(T > float(F32(thr))).astype(np.float64))
+    return Forward(dist, pre, noise, x, e, alpha, keep, T, w, float(F32(thr)), out)
+
+
+def _seqsum_err(a):
+    """u sum_k cumsum(|a|)_k along the last axis (+ the subnormal grid of every term): the rounding bound of a sequential
+    fp32 sum of a"""
+    return U * np.cumsum(np.abs(a), -1).sum(-1) + a.shape[-1] * SUB
+
+
+def forward_error_scale(f: Forward, raw, t, white_bg):
+    """dict FWD_OUT -> bound of the kernel's fp32 error (inf where undecided or not applicable; see the section comment)."""
+    raw = np.asarray(raw, F32)
+    R, S = f.pre.shape
+    t = np.asarray(t, F32).astype(np.float64)
+    c = raw[..., :3].astype(np.float64)
+    und = (f.noise != 0) & (np.abs(f.pre) <= GATE_MU * np.abs(f.noise))
+    with np.errstate(all="ignore"):
+        dpre = NOISE_REL * np.abs(f.noise) + 2 * U * np.abs(f.pre)
+        dpre = np.where(und, np.abs(f.pre) + dpre, dpre)
+        dpre = np.where(np.isnan(f.pre), 0.0, dpre)                               # NaN: alpha = 0, decided
+        de = np.where(f.e > 0, f.e * ((3 * f.x + 3) * U + f.dist * dpre), 0.0) + 4 * SUB
+        da = np.where(f.e + de <= SAT_E, 0.0, de + U / 2)
+        dkeep = da + U * f.keep
+        keep_lo = np.maximum(f.keep - dkeep, K10)
+        eps = np.log1p(dkeep / keep_lo) + 2 * U
+        idx = np.arange(S)[None, :]
+        rho = np.concatenate([np.zeros((R, 1)), np.cumsum(eps, 1)[:, :-1]], 1) + (idx + 8) * 2 * U
+        dT = f.T * np.expm1(rho) + (idx + 8) * SUB
+        dw = f.alpha * dT + (f.T + dT) * da + U * f.w + SUB
+        o = f.out
+        dacc = dw.sum(1) + _seqsum_err(f.w)
+        drgb = ((dw + U * f.w)[..., None] * c).sum(1) + _seqsum_err(np.moveaxis(f.w[..., None] * c, 1, -1))
+        if white_bg:
+            drgb = drgb + (dacc + U * np.abs(1.0 - o["acc"]))[:, None] + U * np.abs(o["rgb"])
+        ddepth = ((dw + U * f.w) * np.abs(t)).sum(1) + _seqsum_err(f.w * t)
+        ddisp = np.abs(o["disp"]) * (ddepth / np.abs(o["depth_raw"]) + dacc / o["acc"] + 3 * U)
+        sc = dict(rgb=drgb, depth=ddepth, depth_raw=ddepth, acc=dacc, disp=ddisp, weights=dw, mask_weights=np.zeros_like(f.T))
+        # a NaN bound comes from an inf or NaN in the truth: 0 there, so that the value must match exactly
+        sc = {k: np.where(np.isnan(v), 0.0, v) for k, v in sc.items()}
+        sc["disp"] = np.where(o["acc"] <= dacc, np.inf, sc["disp"])                        # acc may round to 0
+        sc["depth"] = np.where(np.abs(o["acc"] - 1.0) <= dacc + U, np.inf, sc["depth"])    # acc < 1 undecided
+        # T is exactly 1 in the kernel up to and including the first sample whose alpha may be non-zero (comp_init's
+        # T = 1.0f, keep = fl(1 + 1e-10f) = 1 after a decided alpha = 0): the mask is decided there even at T == thr
+        z = (f.x == 0) & ~und
+        one = np.concatenate([np.ones((R, 1), bool), np.cumprod(z[:, :-1], 1).astype(bool)], 1)
+        sc["mask_weights"] = np.where(~one & (np.abs(f.T - f.thr) <= dT + U * f.T), np.inf, 0.0)
+    return sc
+
+
+def forward_ratio(got, ref, scale):
+    """|got - ref| / scale elementwise, with the special values exact (0 where both are NaN or the same infinity, inf where
+    only one is NaN or an infinity differs); 0 where the scale is inf (undecided)."""
+    g = np.asarray(got, np.float64)
+    with np.errstate(all="ignore"):
+        special = np.isnan(ref) | np.isinf(ref) | np.isnan(g) | np.isinf(g)
+        same_special = (np.isnan(ref) & np.isnan(g)) | (np.isinf(ref) & (g == ref))
+        err = np.abs(g - ref)
+        r = np.where(scale > 0, err / scale, np.where(err > 0, np.inf, 0.0))
+        r = np.where(special, np.where(same_special, 0.0, np.inf), r)
+    return np.where(np.isinf(scale), 0.0, r)
+
+
+FWD_FAULTS = (
+    "mask_after_multiply",      # mask_i = [T_i keep_i > thr]: the mask taken after the transmittance update
+    "mask_ge",                  # mask_i = [T_i >= thr]: the comparison not strict
+    "T_inclusive",              # w_i = alpha_i T_{i+1}: an inclusive cumprod
+    "depth_zero_training",      # depth zeroed where acc < 1 in training mode too
+    "disp_from_zeroed_depth",   # disp computed from the thresholded depth
+    "disp_nan_propagates",      # disp = 1 / max(1e-10, ratio) with torch.max's NaN and no zeroing
+    "last_dist_unscaled",       # the last interval 1e10 instead of 1e10 |d|
+    "white_bg_before_acc",      # the white background from the acc before the last sample's weight
+    "keep_no_eps",              # keep = 1 - alpha without + 1e-10
+    "noise_index_plus1",        # the noise drawn at index ray*S + i + 1
+    "noise_other_salt",         # the noise of the other pass's salt
+)
+
+
+def emulate_forward(raw, t, dirs, white_bg, training, thr, noise_std=0.0, seed=0, fault=None):
+    """composite_kernel's order in numpy fp32 (one sequential walk per ray); `fault` one of FWD_FAULTS.  Returns
+    dict FWD_OUT -> fp32 arrays."""
+    raw, t, dirs = np.asarray(raw, F32), np.asarray(t, F32), np.asarray(dirs, F32)
+    R, S = t.shape
+    one, k10, thr = F32(1), F32(0.0 if fault == "keep_no_eps" else 1e-10), F32(thr)
+    if fault == "noise_other_salt":
+        seed = seed ^ SALT_MAIN ^ SALT_COARSE
+    with np.errstate(all="ignore"):
+        pre, _ = noisy_pre(raw, noise_std, seed, 1 if fault == "noise_index_plus1" else 0)
+        nrm = np.sqrt((dirs[:, 0] * dirs[:, 0] + dirs[:, 1] * dirs[:, 1]) + dirs[:, 2] * dirs[:, 2])
+        T = np.ones(R, F32)
+        acc, depth = np.zeros(R, F32), np.zeros(R, F32)
+        rgb = np.zeros((R, 3), F32)
+        w_all, m_all = np.zeros((R, S), F32), np.zeros((R, S), F32)
+        acc_before_last = acc
+        for i in range(S):
+            if i + 1 < S:
+                dist = (t[:, i + 1] - t[:, i]) * nrm
+            else:
+                dist = np.full(R, F32(1e10)) if fault == "last_dist_unscaled" else F32(1e10) * nrm
+            sg = np.fmax(pre[:, i], F32(0))                   # fmaxf: a NaN operand is dropped
+            e = np.exp(-sg * dist)
+            alpha = one - e
+            keep = (one - alpha) + k10
+            Tn = T * keep
+            w = alpha * (Tn if fault == "T_inclusive" else T)
+            Tm = Tn if fault == "mask_after_multiply" else T
+            m_all[:, i] = (Tm >= thr) if fault == "mask_ge" else (Tm > thr)
+            w_all[:, i] = w
+            for k in range(3):
+                rgb[:, k] = rgb[:, k] + w * raw[:, i, k]
+            acc_before_last = acc
+            acc = acc + w
+            depth = depth + w * t[:, i]
+            T = Tn
+        ratio = depth / acc
+        zeroed = np.where(((not training) or fault == "depth_zero_training") & (acc < one), F32(0), depth)
+        if fault == "disp_from_zeroed_depth":
+            ratio = zeroed / acc
+        if fault == "disp_nan_propagates":
+            disp = one / np.maximum(F32(1e-10), ratio)               # np.maximum propagates NaN, like torch.max
+        else:
+            disp = one / np.fmax(F32(1e-10), ratio)
+            disp = np.where(np.isnan(disp) | np.isnan(ratio), F32(0), disp)
+        if white_bg:
+            bg = one - (acc_before_last if fault == "white_bg_before_acc" else acc)
+            rgb = rgb + bg[:, None]
+    return dict(rgb=rgb, depth=zeroed, depth_raw=depth, acc=acc, disp=disp, weights=w_all, mask_weights=m_all)
+
+
+FWD_KINDS = KINDS + ("empty", "acc_one", "behind", "tiny_ratio", "overflow", "zero_dir", "nan_sigma")
+
+
+def make_forward_rays(R, S, seed, kind_offset=0):
+    """fp32 (raw, t, dirs, kinds) with ray r of kind FWD_KINDS[(r + kind_offset) % 14]: the seven adjoint kinds of
+    `make_rays`, and
+    * empty: sigma in [-50, -10] everywhere (no noise of std 0.7 opens a gate): acc = 0 exactly, so disp = depth = rgb = 0
+      (1 with a white background)
+    * acc_one: total optical depth near 17 (T_end near 2^-24: acc just below 1), or one sample with x in [30, 60]
+      (alpha = 1 in fp32: acc 1 + 1e-10 sum T, just above) — acc within a few ulp of 1 on both sides
+    * behind: t in [-6, -2], sigma > 0: depth / acc < 0, disp = 1e10f exactly
+    * tiny_ratio: t in [1e-12, 5e-11]: 0 < depth / acc < 1e-10, disp = 1e10f
+    * overflow: the last t is +inf (the interval before it inf): depth inf, disp 0 where the last weight is > 0, and the
+      NaN of 0 * inf where the sigma before it is 0 (every other ray)
+    * zero_dir: d = 0: every dist 0, acc = 0
+    * nan_sigma: every third sigma NaN (alpha = 0 there: the kernel's rule)"""
+    raw, t, dirs, _, kinds = make_rays(R, S, seed, kind_offset)
+    kinds = (np.arange(R) + kind_offset) % len(FWD_KINDS)
+    rng = np.random.default_rng(seed + 1)
+    K = {n: i for i, n in enumerate(FWD_KINDS)}
+    nd = np.sqrt((dirs.astype(np.float64) ** 2).sum(1))
+    for r in np.flatnonzero(kinds >= len(KINDS)):
+        name = FWD_KINDS[kinds[r]]
+        dist = np.append(np.diff(t[r].astype(np.float64)), 1e10) * nd[r]
+        # start from a `random` ray: x = sigma dist ~ 2 N(0,1), colours in (0.02, 0.98)
+        raw[r, :, :3] = rng.uniform(0.02, 0.98, (S, 3))
+        raw[r, :, 3] = (2.0 * rng.standard_normal(S) / np.maximum(dist, 1e-6)).astype(F32)
+        if name == "empty":
+            raw[r, :, 3] = rng.uniform(-50, -10, S)
+        elif name == "acc_one":
+            if (r // len(FWD_KINDS)) % 2 == 0:
+                x = np.full(S, rng.uniform(16.0, 18.5) / max(S - 1, 1))
+                x[-1] = 0.0 if S > 1 else rng.uniform(16.0, 18.5)
+            else:
+                x = rng.uniform(0, 0.5 / S, S)
+                x[S // 2] = rng.uniform(30, 60)
+            raw[r, :, 3] = (x / np.maximum(dist, 1e-6)).astype(F32)
+        elif name == "behind":
+            t[r] = np.sort(rng.uniform(-6.0, -2.0, S)).astype(F32)
+            raw[r, :, 3] = np.abs(raw[r, :, 3]) + F32(0.05)
+        elif name == "tiny_ratio":
+            t[r] = np.sort(rng.uniform(1e-12, 5e-11, S)).astype(F32)
+            d2 = np.append(np.diff(t[r].astype(np.float64)), 1e10) * nd[r]
+            raw[r, :, 3] = (np.abs(rng.standard_normal(S)) / np.maximum(d2, 1e-30)).astype(F32)
+        elif name == "overflow":
+            t[r, -1] = np.inf
+            # light samples before it, so that the last weight (T after the saturated inf interval: ~1e-10) stays normal
+            raw[r, :, 3] = (rng.uniform(0, 0.5 / S, S) / np.maximum(dist, 1e-6)).astype(F32) + F32(0.05)
+            if S > 1 and (r // len(FWD_KINDS)) % 2 == 0:
+                raw[r, -2, 3] = 0.0
+        elif name == "zero_dir":
+            dirs[r] = 0.0
+        elif name == "nan_sigma":
+            raw[r, ::3, 3] = np.nan
+    return raw, t, dirs, kinds
