@@ -141,16 +141,17 @@ int nm_render_rays(NmHandle h, const float* origins_dev, int o_stride, const flo
                    const NmRenderOut* out_dev, void* stream);
 /* get_ray_bundle (+ ndc_rays) fused with the render for image rows [row0,row1) — the eval_nerf.py:50-98 image
  * loop with the pose, not 7.7 MB of directions, crossing PCIe.  pose_host: 12 floats, c2w[:3,:4] row-major.
- * Outputs are (row1-row0)*W rays. */
-int nm_render_image(NmHandle h, const float* pose_host, int H, int W, float focal, int ndc, int row0, int row1,
+ * Outputs are (row1-row0)*W rays.  focal (and near below) are the caller's python floats, unrounded: ndc_rays forms its
+ * scalars from them in double and rounds each once to fp32; the pixel division uses (float)focal, as torch does. */
+int nm_render_image(NmHandle h, const float* pose_host, int H, int W, double focal, int ndc, int row0, int row1,
                     const float* near_far_host, int flags, uint64_t seed, const NmRenderOut* out_dev, void* stream);
 /* get_ray_bundle / ndc_rays alone (src/nerf/nerf_helpers.py:226-307): dirs (rows,W,3); origins (rows,W,3) only
  * when ndc (else the origin is pose[:,3]). */
-int nm_ray_bundle(NmHandle h, const float* pose_host, int H, int W, float focal, int ndc, float ndc_near, int row0,
+int nm_ray_bundle(NmHandle h, const float* pose_host, int H, int W, double focal, int ndc, double ndc_near, int row0,
                   int row1, float* origins_dev_or_null, float* dirs_dev, void* stream);
 /* ndc_rays(H, W, focal, near, rays_o, rays_d) on caller-supplied rays (src/nerf/nerf_helpers.py:280-307, called positionally
  * by DataBundle.ndc, src/data/data_helpers.py:164-167): n rays, origins with o_stride 0 (one shared origin) or 3. */
-int nm_ndc_rays(NmHandle h, int H, int W, float focal, float near, const float* origins_dev, int o_stride,
+int nm_ndc_rays(NmHandle h, int H, int W, double focal, double near, const float* origins_dev, int o_stride,
                 const float* dirs_dev, int64_t n, float* origins_out_dev, float* dirs_out_dev, void* stream);
 /* extract_radiance (src/mesh_nerf.py:27-53) for grid planes [x0,x1): points from the three linspace tables
  * (host, lengths n0,n1,n2; pass torch.linspace values for bit-identical coordinates), dirs := positions.
@@ -408,7 +409,7 @@ int nm_skip_stats(NmHandle h, int64_t* out_host);
 int nm_query_host(NmHandle h, const float* origins_host, int o_stride, const float* dirs_host, int64_t R,
                   const float* near_far_host, int flags, uint64_t seed, const NmRenderOut* out_host);
 /* one image from a pose, results to host (eval_nerf.py image loop). */
-int nm_render_image_host(NmHandle h, const float* pose_host, int H, int W, float focal, int ndc, int row0, int row1,
+int nm_render_image_host(NmHandle h, const float* pose_host, int H, int W, double focal, int ndc, int row0, int row1,
                          const float* near_far_host, int flags, uint64_t seed, const NmRenderOut* out_host);
 /* model.sample_points with host tensors (src/mesh_nerf.py:43-48). */
 int nm_point_mlp_host(NmHandle h, int which, const float* pts_host, const float* dirs_host, int64_t M,
@@ -444,7 +445,8 @@ int nm_get_grad(NmHandle h, int which, const char* name, float* out_dev, int64_t
  *   (tree.py:280-297) with `seed` — pass the seed of the render call whose samples are being attributed.
  * nm_tree_integrate: TreeSampling.ray_batch_integration (tree.py:177-206) past its step gate: memm[v] +=
  *   (sum of weights / sum of weight masks of the samples in v - memm[v]) / counter for every voxel that received a sample.
- *   idx/weights/mask: n = R*S entries (whole batch, idx -1 skipped, or only the rows of rays that hit). */
+ *   idx/weights/mask: n = R*S entries (whole batch, idx -1 skipped, or only the rows of rays that hit); an idx outside [0, V) is
+ *   skipped.  counter >= 1 and V >= 1; n = 0 launches nothing. */
 int nm_ray_voxel_indices(NmHandle h, const float* origins_dev, int o_stride, const float* dirs_dev, int64_t R,
                          const float* near_far_host, float* z_out_dev, int32_t* idx_out_dev, void* stream);
 int nm_ray_voxel_indices_ex(NmHandle h, const float* origins_dev, int o_stride, const float* dirs_dev, int64_t R,

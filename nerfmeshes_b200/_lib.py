@@ -34,7 +34,7 @@ PREC_EXACT, PREC_FAST, PREC_FP32 = 0, 1, 2
 FLAG_TRAINING, FLAG_BUFF, FLAG_TEACHER_T, FLAG_RANDOM_VOXELS, FLAG_SKIP_EMPTY = 1, 2, 4, 8, 16
 NET_COARSE, NET_FINE = 0, 1
 
-_P, _I, _L, _F = C.c_void_p, C.c_int, C.c_int64, C.c_float
+_P, _I, _L, _F, _D = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_double
 _SIGNATURES = {
     "nm_version": (C.c_int, []),
     "nm_last_error": (C.c_char_p, []),
@@ -49,8 +49,8 @@ _SIGNATURES = {
     "nm_point_mlp": (C.c_int, [_P, _I, _P, _P, _L, _P, _I, _P]),
     "nm_sigma_grad": (C.c_int, [_P, _I, _P, _L, _P, _P, _P]),
     "nm_render_rays": (C.c_int, [_P, _P, _I, _P, _L, _P, _P, _P, _I, C.c_uint64, C.POINTER(NmRenderOut), _P]),
-    "nm_render_image": (C.c_int, [_P, _P, _I, _I, _F, _I, _I, _I, _P, _I, C.c_uint64, C.POINTER(NmRenderOut), _P]),
-    "nm_ray_bundle": (C.c_int, [_P, _P, _I, _I, _F, _I, _F, _I, _I, _P, _P, _P]),
+    "nm_render_image": (C.c_int, [_P, _P, _I, _I, _D, _I, _I, _I, _P, _I, C.c_uint64, C.POINTER(NmRenderOut), _P]),
+    "nm_ray_bundle": (C.c_int, [_P, _P, _I, _I, _D, _I, _D, _I, _I, _P, _P, _P]),
     "nm_grid_sigma": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P]),
     "nm_volume_stats": (C.c_int, [_P, _P, _L, _P]),
     "nm_marching_cubes_count": (C.c_int, [_P, _P, _I, _I, _I, _F, _P, _P]),
@@ -82,7 +82,7 @@ _SIGNATURES = {
     "nm_export_obj": (C.c_int, [C.c_char_p, _P, _L, _P, _L, _P, _L, _P, _L]),
     "nm_export_obj_textured": (C.c_int, [C.c_char_p, _P, _L, _P, _L, _P, _L, _P, _L, _P, C.c_char_p]),
     "nm_query_host": (C.c_int, [_P, _P, _I, _P, _L, _P, _I, C.c_uint64, C.POINTER(NmRenderOut)]),
-    "nm_render_image_host": (C.c_int, [_P, _P, _I, _I, _F, _I, _I, _I, _P, _I, C.c_uint64, C.POINTER(NmRenderOut)]),
+    "nm_render_image_host": (C.c_int, [_P, _P, _I, _I, _D, _I, _I, _I, _P, _I, C.c_uint64, C.POINTER(NmRenderOut)]),
     "nm_point_mlp_host": (C.c_int, [_P, _I, _P, _P, _L, _P, _I]),
     "nm_zero_grad": (C.c_int, [_P, _P]),
     "nm_backward_rays": (C.c_int, [_P, _P, _I, _P, _L, _P, _P, _P, _I, C.c_uint64, _P, _P, _P]),
@@ -102,7 +102,7 @@ _SIGNATURES = {
                                     _P, C.c_size_t, _P, C.c_size_t, C.POINTER(C.c_size_t)]),
     "nm_kernel_flags": (C.c_int, [_P, C.POINTER(C.c_int32)]),
     "nm_check_flags": (C.c_int, [_P, _P]),
-    "nm_ndc_rays": (C.c_int, [_P, _I, _I, _F, _F, _P, _I, _P, _L, _P, _P, _P]),
+    "nm_ndc_rays": (C.c_int, [_P, _I, _I, _D, _D, _P, _I, _P, _L, _P, _P, _P]),
     "nm_launch_count": (C.c_int64, [_P]),
     "nm_debug_tile_schedule": (C.c_int, [_I, _L, _I, _I, _P, _L, _P]),
     "nm_set_timing": (C.c_int, [_P, _I]),

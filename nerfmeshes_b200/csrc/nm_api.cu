@@ -704,7 +704,7 @@ int nm_render_rays(NmHandle h, const float* origins_dev, int o_stride, const flo
                           (cudaStream_t)stream);
 }
 
-int nm_ray_bundle(NmHandle h, const float* pose_host, int H, int W, float focal, int ndc, float ndc_near, int row0,
+int nm_ray_bundle(NmHandle h, const float* pose_host, int H, int W, double focal, int ndc, double ndc_near, int row0,
                   int row1, float* origins_dev, float* dirs_dev, void* stream) {
   if (int e = bind_device(h)) return e;
   NM_CHECK(pose_host && dirs_dev, "null argument");
@@ -716,10 +716,11 @@ int nm_ray_bundle(NmHandle h, const float* pose_host, int H, int W, float focal,
   return launch_raygen(a, origins_dev, dirs_dev, (cudaStream_t)stream, &h->launches);
 }
 
-int nm_render_image(NmHandle h, const float* pose_host, int H, int W, float focal, int ndc, int row0, int row1,
+int nm_render_image(NmHandle h, const float* pose_host, int H, int W, double focal, int ndc, int row0, int row1,
                     const float* near_far_host, int flags, uint64_t seed, const NmRenderOut* out_dev, void* stream) {
   if (int e = bind_checked(h)) return e;
   NM_CHECK(out_dev && pose_host && near_far_host, "null argument");
+  NM_CHECK(0 <= row0 && row0 <= row1 && row1 <= H && W > 0, "bad row range");
   const long long R = (long long)(row1 - row0) * W;
   cudaStream_t st = (cudaStream_t)stream;
   if (int e = h->dirs.ensure((size_t)R * 12)) return e;
@@ -730,7 +731,7 @@ int nm_render_image(NmHandle h, const float* pose_host, int H, int W, float foca
     origins = h->origins.as<float>();
     o_stride = 3;
   }
-  if (int e = nm_ray_bundle(h, pose_host, H, W, focal, ndc, 1.0f, row0, row1, origins, h->dirs.as<float>(), stream)) return e;
+  if (int e = nm_ray_bundle(h, pose_host, H, W, focal, ndc, 1.0, row0, row1, origins, h->dirs.as<float>(), stream)) return e;
   if (!ndc) {
     if (int e = h->small.ensure(64)) return e;
     const float o3[3] = {pose_host[3], pose_host[7], pose_host[11]};
@@ -918,7 +919,7 @@ int nm_ray_voxel_indices_ex(NmHandle h, const float* origins_dev, int o_stride, 
 int nm_tree_integrate(NmHandle h, const int32_t* idx_dev, const float* weights_dev, const float* mask_weights_dev, int64_t n,
                       float* memm_dev, int32_t V, int32_t counter, void* stream) {
   if (int e = bind_checked(h)) return e;
-  NM_CHECK(idx_dev && weights_dev && mask_weights_dev && memm_dev && V > 0 && n >= 0, "bad arguments");
+  NM_CHECK(idx_dev && weights_dev && mask_weights_dev && memm_dev && V > 0 && n >= 0 && counter >= 1, "bad arguments");
   if (int e = h->small.ensure(sizeof(float) * 2 * (size_t)V + 64)) return e;
   return launch_tree_integrate(idx_dev, weights_dev, mask_weights_dev, n, memm_dev, V, counter, h->small.as<float>(),
                                (cudaStream_t)stream, &h->launches);
@@ -1398,10 +1399,11 @@ int nm_query_host(NmHandle h, const float* origins_host, int o_stride, const flo
   return check_kernel_flags(h);
 }
 
-int nm_render_image_host(NmHandle h, const float* pose_host, int H, int W, float focal, int ndc, int row0, int row1,
+int nm_render_image_host(NmHandle h, const float* pose_host, int H, int W, double focal, int ndc, int row0, int row1,
                          const float* near_far_host, int flags, uint64_t seed, const NmRenderOut* out_host) {
   if (int e = bind_device(h)) return e;
   NM_CHECK(out_host, "null output block");
+  NM_CHECK(0 <= row0 && row0 <= row1 && row1 <= H && W > 0, "bad row range");
   const long long R = (long long)(row1 - row0) * W;
   cudaStream_t st = h->own_stream;
   NmRenderOut dev{};
@@ -1459,7 +1461,7 @@ int nm_check_flags(NmHandle h, void* stream) {
   return check_kernel_flags(h);
 }
 
-int nm_ndc_rays(NmHandle h, int H, int W, float focal, float near, const float* origins_dev, int o_stride,
+int nm_ndc_rays(NmHandle h, int H, int W, double focal, double near, const float* origins_dev, int o_stride,
                 const float* dirs_dev, int64_t n, float* origins_out_dev, float* dirs_out_dev, void* stream) {
   if (int e = bind_device(h)) return e;
   NM_CHECK(origins_dev && dirs_dev && origins_out_dev && dirs_out_dev && n >= 0, "bad arguments");

@@ -134,16 +134,18 @@ int launch_mlp_tc_bwd(const NetDev& net, long long M, const float* dz_in, int dz
 int launch_mlp_simt(const NetDev& net, bool sigma_only, const MlpInput& in, float* out, cudaStream_t st,
                     int64_t* launches);
 
+// focal and near stay double: ndc_rays forms its scalars from the caller's python floats, so they are rounded to fp32 only
+// after that arithmetic (launch_raygen / launch_ndc); the pixel division uses (float)focal, as torch's tensor / scalar does.
 struct RayGenArgs {
   float pose[12];
   int H, W;
-  float focal;
+  double focal;
   int ndc;
-  float ndc_near;
+  double ndc_near;
   int row0, row1;
 };
 int launch_raygen(const RayGenArgs& a, float* origins_or_null, float* dirs, cudaStream_t st, int64_t* launches);
-int launch_ndc(int H, int W, float focal, float near, const float* origins, int o_stride, const float* dirs, long long n,
+int launch_ndc(int H, int W, double focal, double near, const float* origins, int o_stride, const float* dirs, long long n,
                float* out_o, float* out_d, cudaStream_t st, int64_t* launches);
 int launch_stratified(const float* s_table, int Nc, long long R, const float* near_far2, const float* near_dev,
                       const float* far_dev, int lindisp, int perturb, uint64_t seed, float* t_out, cudaStream_t st,

@@ -13,35 +13,47 @@ namespace {
 
 // ------------------------------------------------------------------------------------------------ a1 / a2
 // get_ray_bundle (src/nerf/nerf_helpers.py:226-277) and ndc_rays (:280-307).
+// The fp32 scalars of ndc_rays: its python-double arithmetic on the caller's unrounded focal and near, each result rounded
+// once to fp32, as torch rounds a python-scalar operand of an fp32 tensor op.
+struct NdcScalars {
+  float near, sx, sy, two_near, neg_two_near;
+};
+NdcScalars ndc_scalars(int H, int W, double focal, double near) {
+  return NdcScalars{(float)near, (float)(-1.0 / ((double)W / (2.0 * focal))), (float)(-1.0 / ((double)H / (2.0 * focal))),
+                    (float)(2.0 * near), (float)(-2.0 * near)};
+}
 struct RayGenDev {
   float pose[12];
   int H, W;
   float focal, half_w, half_h;
   int ndc;
-  float ndc_near, sx, sy, two_near;
+  NdcScalars ndc_s;
   int row0;
   long long n;
 };
-// ndc_rays body (src/nerf/nerf_helpers.py:283-305), op for op: shift the origin to the near plane, then project.
-__device__ __forceinline__ void ndc_warp(float near, float sx, float sy, float two_near, float o[3], float d[3]) {
-  const float t = -(near + o[2]) / d[2];
+// ndc_rays body (src/nerf/nerf_helpers.py:283-305), op for op: shift the origin to the near plane, then project.  The two
+// `2.0 * near / rays_o[..., 2]` terms divide a python scalar by a tensor, which torch evaluates as reciprocal(t) * scalar
+// (Tensor.__rtruediv__); every other division is tensor / tensor, a true division.
+__device__ __forceinline__ void ndc_warp(const NdcScalars& s, float o[3], float d[3]) {
+  const float t = -(s.near + o[2]) / d[2];
   o[0] = o[0] + t * d[0]; o[1] = o[1] + t * d[1]; o[2] = o[2] + t * d[2];
-  const float o0 = sx * o[0] / o[2], o1 = sy * o[1] / o[2], o2 = 1.0f + two_near / o[2];
-  const float d0 = sx * (d[0] / d[2] - o[0] / o[2]);
-  const float d1 = sy * (d[1] / d[2] - o[1] / o[2]);
-  const float d2 = -two_near / o[2];
+  const float rz = 1.0f / o[2];
+  const float o0 = s.sx * o[0] / o[2], o1 = s.sy * o[1] / o[2], o2 = 1.0f + rz * s.two_near;
+  const float d0 = s.sx * (d[0] / d[2] - o[0] / o[2]);
+  const float d1 = s.sy * (d[1] / d[2] - o[1] / o[2]);
+  const float d2 = rz * s.neg_two_near;
   o[0] = o0; o[1] = o1; o[2] = o2;
   d[0] = d0; d[1] = d1; d[2] = d2;
 }
 // ndc_rays on caller-supplied rays (the positional call of DataBundle.ndc, src/data/data_helpers.py:164-167).
-__global__ void ndc_kernel(float near, float sx, float sy, float two_near, const float* __restrict__ origins, int o_stride,
-                           const float* __restrict__ dirs, long long n, float* __restrict__ out_o, float* __restrict__ out_d) {
+__global__ void ndc_kernel(const NdcScalars s, const float* __restrict__ origins, int o_stride, const float* __restrict__ dirs,
+                           long long n, float* __restrict__ out_o, float* __restrict__ out_d) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   float o[3], d[3];
 #pragma unroll
   for (int j = 0; j < 3; ++j) { o[j] = origins[(long long)o_stride * i + j]; d[j] = dirs[3 * i + j]; }
-  ndc_warp(near, sx, sy, two_near, o, d);
+  ndc_warp(s, o, d);
 #pragma unroll
   for (int j = 0; j < 3; ++j) { out_o[3 * i + j] = o[j]; out_d[3 * i + j] = d[j]; }
 }
@@ -60,7 +72,7 @@ __global__ void raygen_kernel(const __grid_constant__ RayGenDev a, float* __rest
     d[j] = (x * a.pose[4 * j + 0] + y * a.pose[4 * j + 1]) + z * a.pose[4 * j + 2];
     o[j] = a.pose[4 * j + 3];
   }
-  if (a.ndc) ndc_warp(a.ndc_near, a.sx, a.sy, a.two_near, o, d);
+  if (a.ndc) ndc_warp(a.ndc_s, o, d);
   dirs[3 * i + 0] = d[0]; dirs[3 * i + 1] = d[1]; dirs[3 * i + 2] = d[2];
   if (origins) { origins[3 * i + 0] = o[0]; origins[3 * i + 1] = o[1]; origins[3 * i + 2] = o[2]; }
 }
@@ -476,13 +488,11 @@ __global__ void stats_pass2(const float* __restrict__ v, long long n, double mea
 int launch_raygen(const RayGenArgs& a, float* origins, float* dirs, cudaStream_t st, int64_t* launches) {
   RayGenDev d{};
   for (int i = 0; i < 12; ++i) d.pose[i] = a.pose[i];
-  d.H = a.H; d.W = a.W; d.focal = a.focal;
+  d.H = a.H; d.W = a.W;
+  d.focal = (float)a.focal;                          // (cols - W * 0.5) / focal: torch divides by the scalar rounded to fp32
   d.half_w = (float)(a.W * 0.5); d.half_h = (float)(a.H * 0.5);
-  d.ndc = a.ndc; d.ndc_near = a.ndc_near;
-  // python-double scalars of ndc_rays, rounded once to fp32 like torch does for tensor (op) python-scalar
-  d.sx = (float)(-1.0 / ((double)a.W / (2.0 * (double)a.focal)));
-  d.sy = (float)(-1.0 / ((double)a.H / (2.0 * (double)a.focal)));
-  d.two_near = (float)(2.0 * (double)a.ndc_near);
+  d.ndc = a.ndc;
+  d.ndc_s = ndc_scalars(a.H, a.W, a.focal, a.ndc_near);
   d.row0 = a.row0;
   d.n = (long long)(a.row1 - a.row0) * a.W;
   if (d.n <= 0) return 0;
@@ -492,13 +502,11 @@ int launch_raygen(const RayGenArgs& a, float* origins, float* dirs, cudaStream_t
   return 0;
 }
 
-int launch_ndc(int H, int W, float focal, float near, const float* origins, int o_stride, const float* dirs, long long n,
+int launch_ndc(int H, int W, double focal, double near, const float* origins, int o_stride, const float* dirs, long long n,
                float* out_o, float* out_d, cudaStream_t st, int64_t* launches) {
   if (n <= 0) return 0;
-  const float sx = (float)(-1.0 / ((double)W / (2.0 * (double)focal)));
-  const float sy = (float)(-1.0 / ((double)H / (2.0 * (double)focal)));
-  ndc_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(near, sx, sy, (float)(2.0 * (double)near), origins, o_stride, dirs, n,
-                                                          out_o, out_d);
+  ndc_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ndc_scalars(H, W, focal, near), origins, o_stride, dirs, n, out_o,
+                                                          out_d);
   NM_CUDA(cudaGetLastError());
   if (launches) ++*launches;
   return 0;
@@ -551,8 +559,8 @@ int launch_aabb(const float* voxels, int V, const float* origins, int o_stride, 
 
 int launch_tree_integrate(const int* idx, const float* w, const float* mw, long long n, float* memm, int V, int counter,
                           float* scratch2v, cudaStream_t st, int64_t* launches) {
-  if (n <= 0 || V <= 0) return 0;
   NM_CHECK(counter >= 1, "counter must be >= 1");
+  if (n <= 0 || V <= 0) return 0;
   NM_CUDA(cudaMemsetAsync(scratch2v, 0, sizeof(float) * 2 * (size_t)V, st));
   const int use_smem = V <= 6144;
   long long blocks = (n + 256 * 16 - 1) / (256 * 16);
@@ -602,7 +610,7 @@ int launch_volume_stats_pass(const float* vol, long long n, int pass, const doub
     stats_pass2<<<1184, 256, 0, st>>>(vol, n, 0.0, mean_dev, out_dev);
   }
   NM_CUDA(cudaGetLastError());
-  if (launches) *launches += 1;
+  if (launches) *launches += pass == 1 ? 2 : 1;
   return 0;
 }
 

@@ -121,7 +121,7 @@ int surface_points(const SurfaceView& v, float* pts, float* nrm, float* col, int
   carve(ws, n, &w);
   RayGenArgs g{};
   for (int k = 0; k < 12; ++k) g.pose[k] = v.pose[k];
-  g.H = v.H; g.W = v.W; g.focal = v.focal; g.ndc = 0; g.ndc_near = 1.0f; g.row0 = 0; g.row1 = v.H;
+  g.H = v.H; g.W = v.W; g.focal = v.focal; g.ndc = 0; g.ndc_near = 1.0; g.row0 = 0; g.row1 = v.H;
   if (int e = launch_raygen(g, nullptr, w.dirs, st, launches)) return e;
   SfArgs a{};
   a.depth_raw = v.depth_raw; a.acc = v.acc; a.rgb = v.rgb; a.dirs = w.dirs;

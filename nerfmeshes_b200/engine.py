@@ -389,6 +389,8 @@ class Engine:
         idx = idx.to(torch.int32).contiguous()
         w, mw = _f32c(weights, idx.device), _f32c(mask_weights, idx.device)
         assert memm.is_cuda and memm.dtype == torch.float32 and memm.is_contiguous() and w.numel() == idx.numel() == mw.numel()
+        if idx.numel() == 0:                # an empty batch (no storage to point at) changes nothing
+            return
         L.check(self.lib.nm_tree_integrate(self._h, _ptr(idx), _ptr(w), _ptr(mw), idx.numel(), _ptr(memm), memm.numel(),
                                            int(counter), self._stream()))
 
