@@ -17,9 +17,14 @@
 //                   walks the layer program: encodings -> for each layer, m64nWk16 wgmmas at W = min(n_out, 128) columns
 //                   into the register accumulator (128 fp32 registers per thread) -> epilogue straight from the
 //                   accumulator fragments back into the activation buffer.
-//   warps 8-11      producer: warp 8 issues cp.async.bulk weight stages (16 KB, hi|lo) into the ring.  Both
-//                   warpgroups consume every stage in schedule order; a stage is free once both have released it
-//                   (empty barrier count 2), so one L2 read of the weights feeds 128 points.
+//   warps 8-11      producer: warp 8 issues cp.async.bulk weight stages (16 KB, hi|lo) into the ring.  The two
+//                   warpgroups take turns on it (ping-pong): per round the producer streams layer 0's stages for
+//                   warpgroup 0, the same stages again for warpgroup 1, then layer 1 for warpgroup 0, and so on.  Each
+//                   fill has one owner, which waits on its own full barrier and alone releases the stage (empty barrier
+//                   count 1).  Warpgroup 1's stages of a layer land only as warpgroup 0 releases its own, and warpgroup
+//                   0's next layer only after all of them, so one warpgroup's epilogue runs under the other's MMAs.
+//                   A warpgroup without a tile in a round gets no stages at all; that is only ever warpgroup 1, after
+//                   its own last tile (with tile groups of G tiles, for up to G final rounds).
 // The view-direction encoding reuses the encoding buffer: every layer that reads the xyz encoding precedes the one that
 // reads the directions (checked at launch).
 //
@@ -63,7 +68,6 @@ struct TcParams {
   int n_passes;
   float act_scale, act_inv_scale;
   int num_stages;
-  int n_stages;     // stages of the wide weight stream streamed per round at this precision (nm_program.h wide_stages)
   long long n_tiles;
   int* err;
   uint32_t off_wg, off_bias, off_head, off_bars, off_comp;
@@ -98,9 +102,9 @@ static_assert(sizeof(TcParams) <= 4096, "TcParams must fit the 4 KB kernel-param
 #define NM_ST(...)
 #endif
 
-// barrier slots (8 B each) relative to off_bars (+ the NM_MLP_STALLS counters, 8 per warpgroup: wait, mma, start, encoding,
-// epilogue, compositor)
-constexpr uint32_t kBarWFull = 0, kBarWEmpty = 64, kBarStalls = 128, kBarBytes = 128 + (NM_MLP_STALLS ? 128 : 0);
+// barrier slots (8 B each) relative to off_bars: full[wg][s] at kBarWFull + 64 wg + 8 s, empty[s] (+ the NM_MLP_STALLS
+// counters, 8 per warpgroup: wait, mma, start, encoding, epilogue, compositor)
+constexpr uint32_t kBarWFull = 0, kBarWEmpty = 128, kBarStalls = 192, kBarBytes = 192 + (NM_MLP_STALLS ? 128 : 0);
 
 enum : int { ERR_ALIGN = 1, ERR_W_EMPTY = 2, ERR_W_FULL = 3 };
 
@@ -156,12 +160,16 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
   const int NS = P.num_stages;
   float* s_bias = reinterpret_cast<float*>(smem + P.off_bias);
   float* s_head = reinterpret_cast<float*>(smem + P.off_head);
-  const int n_layers = P.net.n_layers, n_stages = P.n_stages;
+  const int n_layers = P.net.n_layers;
 
   // ---------------------------------------------------------------- one-time setup
   if (threadIdx.x == 0) {
     if (sbase & 1023u) { atomicExch(P.err, ERR_ALIGN); __trap(); }
-    for (int i = 0; i < kMaxStages; ++i) { ptx::mbar_init(bars + kBarWFull + 8 * i, 1); ptx::mbar_init(bars + kBarWEmpty + 8 * i, 2); }
+    for (int i = 0; i < kMaxStages; ++i) {
+      ptx::mbar_init(bars + kBarWFull + 8 * i, 1);
+      ptx::mbar_init(bars + kBarWFull + 64 + 8 * i, 1);
+      ptx::mbar_init(bars + kBarWEmpty + 8 * i, 1);
+    }
     ptx::fence_mbar_init();
   }
   for (int i = threadIdx.x; i < P.net.n_bias; i += kThreads) s_bias[i] = (MODE == 2) ? 0.f : P.bias[i];
@@ -169,9 +177,9 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
   __syncthreads();
 
   // i-th tile of worker v (two workers per CTA, one per consumer warpgroup): groups of `tile_group` consecutive tiles are
-  // dealt round-robin to the workers.  Returns -1 past the end.  Both warpgroups walk the weight ring the same number of
-  // times: iteration i exists when worker 2 * blockIdx.x (the lower one) has a tile; warpgroup 1 runs a "ghost" iteration
-  // (ring traffic only) when its own tile of that round does not exist — which can only be its last one.
+  // dealt round-robin to the workers.  Returns -1 past the end.  Round i exists when worker 2 * blockIdx.x (the lower one)
+  // has a tile; for a given i the higher worker's tile is the lower one's + Gt, so it lacks one only after its own last
+  // tile (for up to Gt rounds), and both sides evaluate per round whether its stages are in the stream.
   const uint32_t Gt = (uint32_t)P.tile_group, V = 2u * gridDim.x, v0 = 2u * blockIdx.x;
   auto tile_of = [&](uint32_t v, uint32_t i) -> long long {
     const long long g = (long long)v + (long long)(i / Gt) * (long long)V;
@@ -188,18 +196,24 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
       uint32_t ph = 0;
       const bool exact = P.n_passes == 3;
       for (uint32_t i = 0; tile_of(v0, i) >= 0; ++i) {
-        int b = 0;                       // image stage
+        const int n_wg = tile_of(v0 + 1, i) >= 0 ? 2 : 1;
+        int b0 = 0;                      // image stage of the layer's first stage
         for (int li = 0; li < n_layers; ++li) {
           const LayerProg& L = P.net.layers[li];
           const bool wide = wide_width(L) == 128;
           // exact: every stage in full; fast: the hi stages of a 128-wide layer, the hi half of a 64-wide layer's blocks
           const uint32_t bytes = (exact || wide) ? (uint32_t)kStageBytes : (uint32_t)kHalfStage;
-          for (int e = b + wide_stages(L); b < e; b += (wide && !exact) ? 2 : 1) {
-            ptx::mbar_wait(bars + kBarWEmpty + 8 * slot, ph ^ 1, P.err, ERR_W_EMPTY);
-            ptx::mbar_expect_tx(bars + kBarWFull + 8 * slot, bytes);
-            ptx::bulk_g2s(sbase + (uint32_t)slot * kStageBytes, P.wpack + (size_t)b * kStageBytes, bytes, bars + kBarWFull + 8 * slot);
-            if (++slot == NS) { slot = 0; ph ^= 1; }
+          const int b1 = b0 + wide_stages(L);
+          for (int w = 0; w < n_wg; ++w) {
+            const uint32_t full = bars + kBarWFull + 64u * (uint32_t)w;
+            for (int b = b0; b < b1; b += (wide && !exact) ? 2 : 1) {
+              ptx::mbar_wait(bars + kBarWEmpty + 8 * slot, ph ^ 1, P.err, ERR_W_EMPTY);
+              ptx::mbar_expect_tx(full + 8 * slot, bytes);
+              ptx::bulk_g2s(sbase + (uint32_t)slot * kStageBytes, P.wpack + (size_t)b * kStageBytes, bytes, full + 8 * slot);
+              if (++slot == NS) { slot = 0; ph ^= 1; }
+            }
           }
+          b0 = b1;
         }
       }
     }
@@ -219,8 +233,11 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
   const float so = P.act_scale, si = P.act_inv_scale;
   const int n_passes = P.n_passes;
   const int Lx = P.net.L_xyz, Ld = P.net.L_dir, ix = P.net.inc_xyz, idr = P.net.inc_dir;
+  // The ring position walks every fill, the other warpgroup's included; parities are per slot and count own fills only, so
+  // a wait on full[wg][s] is never more than one phase from the barrier's.
+  const uint32_t full_w = bars + kBarWFull + 64u * (uint32_t)wg;
   int slot = 0;
-  uint32_t ph = 0;
+  uint32_t ph = 0;                 // bit s: parity of this warpgroup's next fill of slot s
   float acc[128];
   NM_ST(volatile long long* const st = reinterpret_cast<volatile long long*>(smem + P.off_bars + kBarStalls) + 8 * wg;
         if (t == 0) { st[0] = 0; st[1] = 0; st[2] = clock64(); st[3] = 0; st[4] = 0; st[5] = 0; })
@@ -363,28 +380,19 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
   };
 
   float sigma_val[2] = {0.f, 0.f};
-  for (uint32_t it = 0; tile_of(v0, it) >= 0; ++it) {
+  const int stream = n_passes == 3 ? 1 : 2;
+  for (uint32_t it = 0; tile_of(v, it) >= 0; ++it) {
     const long long tile = tile_of(v, it);
-    if (tile < 0) {
-      // ghost iteration: no tile of our own, but the other warpgroup consumes this round's stages — wait for each stage and
-      // hand it straight back
-      for (int b = 0; b < n_stages; ++b) {
-        if (t == 0) {
-          NM_ST(const long long c0 = clock64();)
-          ptx::mbar_wait(bars + kBarWFull + 8 * slot, ph, P.err, ERR_W_FULL);
-          NM_ST(st[0] += clock64() - c0;)
-          ptx::mbar_arrive(bars + kBarWEmpty + 8 * slot);
-        }
-        if (++slot == NS) { slot = 0; ph ^= 1; }
-      }
-      continue;
-    }
+    const bool peer = wg == 1 || tile_of(v0 + 1, it) >= 0;     // the other warpgroup's stages are in this round's stream
     if (MODE != 2) encode(tile, false);
     const long long m0 = tile * kTileM + r0, m1 = m0 + 8;
     const bool val0 = m0 < P.in.M, val1 = m1 < P.in.M;
     for (int li = 0; li < n_layers; ++li) {
       const LayerProg& L = P.net.layers[li];
       if (MODE != 2 && L.pe_src == SRC_PE_DIR) encode(tile, true);
+      // this layer's stages of the other warpgroup: warpgroup 0's precede ours, warpgroup 1's follow them
+      const int skip = peer ? wide_stages(L, stream) : 0;
+      if (wg == 1) slot = (slot + skip) % NS;
       // ------------------------------------------------------------ main loop: this layer's stages of the wide stream
       // (per K-block — the encoding source's first, then the activation K-blocks in ascending order — and column half: the
       // hi stage's a_hi*b_hi, a_lo*b_hi group, then the lo stage's a_hi*b_lo group; a 64-wide layer has both in one stage).
@@ -398,7 +406,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
         // one stage: wait for it, issue its group, release the previous stage once that group's MMAs are complete
         auto stage = [&](auto issue) {
           NM_ST(const long long c0 = clock64();)
-          ptx::mbar_wait_warp(bars + kBarWFull + 8 * slot, ph, P.err, ERR_W_FULL);
+          ptx::mbar_wait_warp(full_w + 8 * slot, (ph >> slot) & 1u, P.err, ERR_W_FULL);
           NM_ST(if (t == 0) st[0] += clock64() - c0;)
           ptx::wgmma_fence();                        // (what ptxas would otherwise inject before the group, C7519)
           issue(sbase + (uint32_t)slot * kStageBytes);
@@ -406,7 +414,8 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
           ptx::wgmma_wait<1>();
           if (prev >= 0 && t == 0) ptx::mbar_arrive(bars + kBarWEmpty + 8 * prev);
           prev = slot;
-          if (++slot == NS) { slot = 0; ph ^= 1; }
+          ph ^= 1u << slot;
+          if (++slot == NS) slot = 0;
         };
         const int n_kb = wide_kblocks(L), has_pe = L.pe_src ? 1 : 0;
         for (int kbi = 0; kbi < n_kb; ++kbi) {
@@ -446,6 +455,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
           if (n_passes == 3) main_loop(IntC<64>{}, IntC<1>{}); else main_loop(IntC<64>{}, IntC<0>{});
         }
       }
+      if (wg == 0) slot = (slot + skip) % NS;
       // ------------------------------------------------------------ epilogue, straight from the accumulator fragments
       NM_ST(const long long ce = clock64();)
       const int NC = L.n_out >> 6;
@@ -665,8 +675,6 @@ static int launch_prepared(TcParams& P, int num_sms, cudaStream_t st, int64_t* l
   for (int i = 0; i < hp.n_layers; ++i)
     NM_CHECK(hp.layers[i].kind == KIND_LOAD || hp.layers[i].n_out == 64 || hp.layers[i].n_out == 128 || hp.layers[i].n_out == 256,
              "layer %d: output width %d not 64, 128 or 256", i, hp.layers[i].n_out);
-  P.n_stages = 0;
-  for (int i = 0; i < hp.n_layers; ++i) P.n_stages += wide_stages(hp.layers[i], P.n_passes == 3 ? 1 : 2);
   uint32_t off = (uint32_t)ns * kStageBytes;
   P.off_wg = off; off += 2 * kWgBytes;
   P.off_bias = off; off += align_up(hp.n_bias * 4, 16);

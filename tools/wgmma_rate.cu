@@ -4,7 +4,9 @@
 //   variant 0: 4 x m64n64k16 per pass from 64x64 SW128 K-major blocks (a commit group per 64-column block, 12 wgmmas)
 //   variant 1: 2 x m64n128k16 per pass from 128x64 SW128 K-major blocks (a commit group per block, 12 wgmmas)
 //   variant 2: 1 x m64n256k16 per pass from 256x16 SW32 K-major steps (a commit group per K step, 3 wgmmas)
-// with commit -> wait_group 1 between groups, as the MLP kernel's stage loop does.
+// with commit -> wait_group 1 between groups, as the MLP kernel's stage loop does.  Variant 3 is variant 1 issued by ONE
+// warpgroup per SM (128 threads): whether a single warpgroup keeps the SM's four tensor cores as busy as two do, which a
+// ping-pong of the two consumer warpgroups (one issuing MMAs while the other runs its epilogue) relies on.
 //
 //     wgmma_rate <iterations>     prints "variant ms" lines for one launch of each variant
 #include <cstdio>
@@ -50,7 +52,7 @@ __global__ void __launch_bounds__(256, 1) rate_kernel(long long iters, float* si
         ptx::wgmma_commit();
         ptx::wgmma_wait<1>();
       }
-    } else if (V == 1) {
+    } else if (V == 1 || V == 3) {
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const uint64_t b_hi = ptx::make_kmajor_sw128_desc(s0 + h * 32768u), b_lo = ptx::make_kmajor_sw128_desc(s0 + h * 32768u + 16384u);
@@ -91,15 +93,15 @@ __global__ void __launch_bounds__(256, 1) rate_kernel(long long iters, float* si
 
 template <int V>
 static int run(int sms, long long iters, float* sink) {
-  const int smem = (int)(kB + 2 * kA);
+  const int smem = (int)(kB + 2 * kA), threads = V == 3 ? 128 : 256;
   CK(cudaFuncSetAttribute(rate_kernel<V>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  rate_kernel<V><<<sms, 256, smem>>>(iters / 16 + 1, sink);      // warm-up
+  rate_kernel<V><<<sms, threads, smem>>>(iters / 16 + 1, sink);      // warm-up
   CK(cudaGetLastError());
   cudaEvent_t e0, e1;
   CK(cudaEventCreate(&e0));
   CK(cudaEventCreate(&e1));
   CK(cudaEventRecord(e0));
-  rate_kernel<V><<<sms, 256, smem>>>(iters, sink);
+  rate_kernel<V><<<sms, threads, smem>>>(iters, sink);
   CK(cudaEventRecord(e1));
   CK(cudaEventSynchronize(e1));
   float ms = 0.f;
@@ -117,7 +119,7 @@ int main(int argc, char** argv) {
   printf("sms %d\nname %s\n", prop.multiProcessorCount, prop.name);
   for (int rep = 0; rep < 2; ++rep)
     if (run<0>(prop.multiProcessorCount, iters, sink) || run<1>(prop.multiProcessorCount, iters, sink) ||
-        run<2>(prop.multiProcessorCount, iters, sink))
+        run<2>(prop.multiProcessorCount, iters, sink) || run<3>(prop.multiProcessorCount, iters, sink))
       return 1;
   CK(cudaFree(sink));
   return 0;
