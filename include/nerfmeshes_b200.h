@@ -90,8 +90,11 @@ enum {
   NM_FLAG_TEACHER_T = 4,   /* t_vals is an INPUT: skip sampling, run net `which`=fine-if-present on it */
   NM_FLAG_RANDOM_VOXELS = 8, /* with NM_FLAG_BUFF: cfg.tree.use_random_sampling — multinomial voxel draws + uniform depth inside
                                the voxel (src/nerf/tree.py:280-297) instead of the deterministic placement; uses `seed` */
-  NM_FLAG_SKIP_EMPTY = 16   /* empty-space skipping (nm_build_occupancy): only the samples the pass's occupancy grid marks go
+  NM_FLAG_SKIP_EMPTY = 16,  /* empty-space skipping (nm_build_occupancy): only the samples the pass's occupancy grid marks go
                                through the network; inference only (rejected with NM_FLAG_TRAINING / NM_FLAG_TEACHER_T) */
+  NM_FLAG_SKIP_EMPTY_TRAIN = 32 /* empty-space skipping in training (see the occupancy section): only with NM_FLAG_TRAINING, by
+                               nm_render_rays, nm_backward_rays and nm_loss_backward; rejected with NM_FLAG_TEACHER_T and
+                               NM_FLAG_SKIP_EMPTY; takes a stale grid */
 };
 
 /* ---- lifecycle -------------------------------------------------------------------------------------- */
@@ -387,7 +390,20 @@ int nm_export_ply(const char* path, const float* points_host, const float* color
  * depth_raw, acc, disp, weights, mask_weights, t_vals, coarse_*) is bit-identical to the render without the flag when every
  * sample the grid skipped on that ray has a dense noisy pre-activation (raw sigma + the pass's noise) <= 0 or NaN.  A skipping render reads each pass's sample count back to the host (one
  * small copy and one stream synchronisation per pass per NM_CHUNK_RAYS chunk), so it cannot be captured in a CUDA graph; the
- * network runs on at most NM_SKIP_CHUNK_POINTS points per launch (default 4 Mi).  Loading a network's weights drops its grid.
+ * network runs on at most NM_SKIP_CHUNK_POINTS points per launch (default 4 Mi).
+ *
+ * Grid lifetime: loading a network's weights marks its grid STALE.  NM_FLAG_SKIP_EMPTY renders and nm_occupancy_query refuse
+ * a stale grid; NM_FLAG_SKIP_EMPTY_TRAIN takes it (keeping it fresh enough is the caller's schedule: BaseModel.
+ * enable_training_skip rebuilds every few optimiser steps).  nm_build_occupancy / nm_set_occupancy make a grid fresh.
+ *
+ * Training (NM_FLAG_SKIP_EMPTY_TRAIN with NM_FLAG_TRAINING): each pass compacts and stages its evaluated samples as above,
+ * keeps them until its backward, runs the network over them only (emitting the backward's operands when they fit
+ * NM_TRAIN_DIRECT_GB for that pass's evaluated count) and composites the expanded (R,S,4) buffer; the compositor adjoint
+ * hands the evaluated rows, compacted, to the network backward.  On every ray whose skipped samples all have a dense
+ * noisy pre-activation (raw sigma + the training noise) <= 0 or NaN, rgb / coarse_rgb and the loss terms are bit-identical
+ * to the dense training call and so are the evaluated samples' adjoints (a skipped sample's dense adjoint row is zero);
+ * the weight gradients differ from the dense ones by the order of fp32 atomic sums only.  A pass with no evaluated sample
+ * launches no network work.  nm_skip_stats counts these passes too.
  *
  * nm_build_occupancy: the grid of network `which` from its own density.  Lattice: torch.linspace(lo_a, hi_a, G+1) per axis,
  *   sigma from nm_grid_sigma's sigma-only sweep of that network (directions = positions); a cell is raw-occupied when the max
@@ -395,9 +411,10 @@ int nm_export_ply(const char* path, const float* points_host, const float* color
  *   Chebyshev distance (clamped at the box faces).  1 <= G <= 1024, 0 <= dilate <= G, threshold not NaN.  bits_out_dev (the
  *   ceil(G^3/32) words) or NULL.  Synchronises `stream` once.
  * nm_set_occupancy: installs caller bits (same layout) for network `which`; bits_dev NULL removes the grid.
- * nm_occupancy_query: evaluated_out_dev[m] = 1 if point m (pts_dev (M,3)) is evaluated under network `which`'s grid, else 0.
+ * nm_occupancy_query: evaluated_out_dev[m] = 1 if point m (pts_dev (M,3)) is evaluated under network `which`'s fresh grid,
+ *   else 0.
  * nm_skip_stats: out_host = {samples seen, samples evaluated} of the coarse (or only) pass, then of the fine pass, summed
- *   over skipping renders since the last call; resets them.  Synchronises the device. */
+ *   over skipping renders and skipping training passes since the last call; resets them.  Synchronises the device. */
 int nm_build_occupancy(NmHandle h, int which, const float* box_host, int G, float threshold, int dilate,
                        uint32_t* bits_out_dev_or_null, void* stream);
 int nm_set_occupancy(NmHandle h, int which, const float* box_host, int G, const uint32_t* bits_dev_or_null);

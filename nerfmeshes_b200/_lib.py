@@ -31,7 +31,7 @@ class NmRenderOut(C.Structure):
 
 
 PREC_EXACT, PREC_FAST, PREC_FP32 = 0, 1, 2
-FLAG_TRAINING, FLAG_BUFF, FLAG_TEACHER_T, FLAG_RANDOM_VOXELS, FLAG_SKIP_EMPTY = 1, 2, 4, 8, 16
+FLAG_TRAINING, FLAG_BUFF, FLAG_TEACHER_T, FLAG_RANDOM_VOXELS, FLAG_SKIP_EMPTY, FLAG_SKIP_EMPTY_TRAIN = 1, 2, 4, 8, 16, 32
 NET_COARSE, NET_FINE = 0, 1
 
 _P, _I, _L, _F, _D = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_double

@@ -81,8 +81,9 @@ struct NmHandle_t {
   Buf sp_ws;                       // sparse sweep (nm_sparse_sweep.cu): block flags, two bit-volumes, scans, one chunk of points
   int sp_grid[4] = {0, 0, 0, 0};   // {n0, n1, n2, block} of the last nm_sparse_sweep_lattice, and the volume it wrote:
   const float* sp_vol = nullptr;   // what nm_sparse_sweep_run must be called with
-  struct OccGrid {                 // empty-space skipping (nm_occupancy.cu, DESIGN §4.15): one grid per network slot, dropped
-    bool valid = false;            // by a weight load of that slot
+  struct OccGrid {                 // empty-space skipping (nm_occupancy.cu, DESIGN §4.15): one grid per network slot
+    bool valid = false;            // installed (nm_build_occupancy / nm_set_occupancy)
+    bool stale = false;            // the slot's weights were loaded after it: inference refuses it, training skipping takes it
     float lo[3], hi[3], inv[3];
     int G = 0;
     Buf bits;
@@ -90,6 +91,10 @@ struct NmHandle_t {
   Buf oc_ws;                       // grid build: one plane chunk of the sigma lattice, two G^3 byte volumes
   Buf sk_ws;                       // skipping render: marks, scan, index list (12 B per sample of a chunk pass) + one network
                                    // launch's points, directions and outputs (40 B per point, 160 MB at the default 4 Mi)
+  Buf ts_ws[2], ts_pts[2];         // skipping training step, per pass (0: coarse or only, 1: fine), held until the backward:
+                                   // marks, scan, index list (12 B per sample); staged points, directions (24 B per evaluated
+                                   // sample) and one network launch's outputs
+  Buf train_ws_c;                  // skipping training step: the coarse pass's emitted operands (the fine pass's are in train_ws)
   int64_t skip_counts[4] = {0, 0, 0, 0};   // samples seen / evaluated, coarse (or only) pass, fine pass (nm_skip_stats)
   Buf sg_ws;                       // density gradient (nm_sigma_grad): one chunk's forward / chain / tail workspace; grow-only,
                                    // held until nm_destroy (~22 KB per chunk point for the 8x256 network, ~5.8 GB at the default)
@@ -250,12 +255,44 @@ struct RayBatch {
 
 float* off(float* p, long long n) { return p ? p + n : nullptr; }
 
+// NM_FLAG_SKIP_EMPTY_TRAIN (DESIGN §4.15): what one pass of a skipping training forward leaves for its backward
+struct TrainSkip {
+  // in
+  bool emit = false;            // the pass carries a gradient and may leave the backward's operands (tensor cores, scale 0)
+  double budget = 0;            // bytes the emitted operands of both passes may take (NM_TRAIN_DIRECT_GB)
+  double* committed = nullptr;  // bytes already taken by the other pass's
+  // out
+  long long M = 0;              // evaluated samples
+  const int* pos = nullptr;     // exclusive scan of the marks (R*s + 1): sample m's compact slot
+  const float* pts = nullptr;   // (M,3) staged points
+  const float* dirs = nullptr;  // (M,3) their directions
+  float* ws = nullptr;          // the emitted operands (train_emit_setup carving for M points), or NULL: walk with recompute
+};
+
+// the flag rules of NM_FLAG_SKIP_EMPTY_TRAIN, checked before anything is launched
+int check_train_skip(NmHandle h, int flags) {
+  if (!(flags & NM_FLAG_SKIP_EMPTY_TRAIN)) return 0;
+  NM_CHECK(flags & NM_FLAG_TRAINING, "NM_FLAG_SKIP_EMPTY_TRAIN is a training path: it needs NM_FLAG_TRAINING "
+           "(inference renders skip with NM_FLAG_SKIP_EMPTY)");
+  NM_CHECK(!(flags & NM_FLAG_TEACHER_T), "NM_FLAG_SKIP_EMPTY_TRAIN does not take NM_FLAG_TEACHER_T");
+  NM_CHECK(!(flags & NM_FLAG_SKIP_EMPTY), "NM_FLAG_SKIP_EMPTY_TRAIN and NM_FLAG_SKIP_EMPTY exclude each other "
+           "(training and inference skipping)");
+  const int nets = (h->has_fine && !(flags & NM_FLAG_BUFF) && h->cfg.num_fine > 0) ? 2 : 1;
+  for (int k = 0; k < nets; ++k)
+    NM_CHECK(h->occ[k].valid, "NM_FLAG_SKIP_EMPTY_TRAIN: no occupancy grid for network %d (build one with nm_build_occupancy; "
+             "a weight load keeps it, stale, for training)", k);
+  return 0;
+}
+
 // NeRFModel.forward / BuFFModel.forward for one chunk of rays; `o` already offset to the chunk.
 // emit_c / emit_f: training only — the coarse (or only) / fine network's forward also leaves the backward's operands (MlpEmit)
 // need_raw: the caller reads h->raw_c / h->raw_f afterwards (the training backward) — otherwise the compositor runs inside the
 // MLP kernel and the per-sample network outputs never reach HBM (NM_FUSED_COMPOSITE=0 keeps the two-kernel path for A/B tests).
+// tsk: NM_FLAG_SKIP_EMPTY_TRAIN — per pass (0: coarse or only, 1: fine) what the backward needs (TrainSkip); with it the
+// passes size their emitted operands themselves and emit_c / emit_f are NULL.
 int render_chunk(NmHandle h, const RayBatch& rb, int flags, uint64_t seed, const NmRenderOut& o, cudaStream_t st,
-                 const MlpEmit* emit_c = nullptr, const MlpEmit* emit_f = nullptr, bool need_raw = false) {
+                 const MlpEmit* emit_c = nullptr, const MlpEmit* emit_f = nullptr, bool need_raw = false,
+                 TrainSkip* tsk = nullptr) {
   const NmRenderCfg& c = h->cfg;
   const long long R = rb.R;
   const int Nc = c.num_coarse;
@@ -278,24 +315,28 @@ int render_chunk(NmHandle h, const RayBatch& rb, int flags, uint64_t seed, const
     NM_CHECK(!training && !teacher && !need_raw && !emit_c && !emit_f,
              "NM_FLAG_SKIP_EMPTY is an inference path: it takes neither NM_FLAG_TRAINING nor NM_FLAG_TEACHER_T");
     for (int k = 0; k < ((Nf > 0) ? 2 : 1); ++k)
-      NM_CHECK(h->occ[k].valid, "NM_FLAG_SKIP_EMPTY: no occupancy grid for network %d (nm_build_occupancy / nm_set_occupancy; "
+      NM_CHECK(h->occ[k].valid && !h->occ[k].stale, "NM_FLAG_SKIP_EMPTY: no occupancy grid for network %d (nm_build_occupancy / nm_set_occupancy; "
                "loading that network's weights drops its grid)", k);
   }
   // empty-space skipping (DESIGN §4.15): only the samples network `which`'s grid marks go through it, as explicit points in
   // launches of at most skip_chunk_points(); every other sample enters the compositor as raw (0,0,0,-inf), which the pass's
-  // sigma noise cannot lift above 0
-  auto skip_raw = [&](int which, Buf& raw_buf, const float* t, int s) -> int {
+  // sigma noise cannot lift above 0.  Training (ts != NULL): the index data and ALL staged points stay in the pass's own
+  // buffers for the backward, and when the backward's operands for the M evaluated points fit the budget the network runs
+  // in one emitting launch over them.
+  auto skip_raw = [&](int which, Buf& raw_buf, const float* t, int s, TrainSkip* ts) -> int {
     NmHandle_t::OccGrid& g = h->occ[which];
     const long long n = R * s;
-    NM_CHECK(n + 1 < (1ll << 31), "NM_FLAG_SKIP_EMPTY: %lld samples in one chunk exceed the int32 index list (lower NM_CHUNK_RAYS)", n);
-    const long long P = skip_chunk_points();
+    NM_CHECK(n + 1 < (1ll << 31), "%s: %lld samples in one chunk exceed the int32 index list (lower NM_CHUNK_RAYS)",
+             ts ? "NM_FLAG_SKIP_EMPTY_TRAIN" : "NM_FLAG_SKIP_EMPTY", n);
+    long long P = skip_chunk_points();
     const size_t nb = (size_t)(n + 1) * 4, nblk = (size_t)((n + 1 + kScanBlockEntries - 1) / kScanBlockEntries) * 4;
     const long long cap = P < n ? P : (n > 0 ? n : 1);
     const size_t o_pos = (nb + 255) & ~(size_t)255, o_blk = 2 * o_pos, o_idx = o_blk + ((nblk + 255) & ~(size_t)255);
     const size_t o_pts = o_idx + o_pos, o_dir = o_pts + (((size_t)cap * 12 + 255) & ~(size_t)255);
     const size_t o_out = o_dir + (((size_t)cap * 12 + 255) & ~(size_t)255), bytes = o_out + (size_t)cap * 16;
-    if (int e = h->sk_ws.ensure(bytes)) return e;
-    uint8_t* ws = h->sk_ws.as<uint8_t>();
+    Buf& ws_buf = ts ? h->ts_ws[which] : h->sk_ws;
+    if (int e = ws_buf.ensure(ts ? o_pts : bytes)) return e;
+    uint8_t* ws = ws_buf.as<uint8_t>();
     int* idx = reinterpret_cast<int*>(ws + o_idx);
     long long M = 0;
     if (int e = raw_buf.ensure((size_t)n * 16)) return e;
@@ -306,12 +347,37 @@ int render_chunk(NmHandle h, const RayBatch& rb, int flags, uint64_t seed, const
     float* pts = reinterpret_cast<float*>(ws + o_pts);
     float* dirs = reinterpret_cast<float*>(ws + o_dir);
     float* out = reinterpret_cast<float*>(ws + o_out);
+    MlpEmit em{};
+    if (ts) {
+      *ts = TrainSkip{ts->emit, ts->budget, ts->committed};
+      ts->M = M;
+      ts->pos = reinterpret_cast<const int*>(ws + o_pos);
+      if (M == 0) return 0;                       // no network work; the pass's gradients stay untouched
+      const NetProgram& G = h->nets[which].full;
+      const size_t wsb = ts->emit ? train_ws_bytes(G, M, true) + 1024 : 0;
+      if (wsb && *ts->committed + (double)wsb <= ts->budget) {
+        Buf& wb = (which == NM_NET_COARSE && Nf > 0) ? h->train_ws_c : h->train_ws;
+        if (int e = wb.ensure(wsb + 1024)) return e;
+        ts->ws = reinterpret_cast<float*>(((uintptr_t)wb.p + 1023) & ~(uintptr_t)1023);
+        train_emit_setup(G, M, ts->ws, &em);
+        *ts->committed += (double)wsb;
+        P = M;                                    // the emitting launch covers every evaluated point
+      }
+      const long long lc = P < M ? P : M;
+      const size_t q_dir = (((size_t)M * 12 + 255) & ~(size_t)255), q_out = 2 * q_dir;
+      if (int e = h->ts_pts[which].ensure(q_out + (size_t)lc * 16)) return e;
+      uint8_t* tp = h->ts_pts[which].as<uint8_t>();
+      pts = reinterpret_cast<float*>(tp); dirs = reinterpret_cast<float*>(tp + q_dir); out = reinterpret_cast<float*>(tp + q_out);
+      if (int e = launch_occ_stage(idx, M, s, rb.origins, rb.o_stride, rb.dirs, t, pts, dirs, st, &h->launches)) return e;
+      ts->pts = pts; ts->dirs = dirs;
+    }
     for (long long j0 = 0; j0 < M; j0 += P) {
       const long long m = (M - j0 < P) ? M - j0 : P;
-      if (int e = launch_occ_stage(idx + j0, m, s, rb.origins, rb.o_stride, rb.dirs, t, pts, dirs, st, &h->launches)) return e;
+      if (!ts)
+        if (int e = launch_occ_stage(idx + j0, m, s, rb.origins, rb.o_stride, rb.dirs, t, pts, dirs, st, &h->launches)) return e;
       MlpInput in{};
-      in.mode = IN_POINTS; in.pts = pts; in.dirs = dirs; in.M = m;
-      if (int e = run_mlp(h, which, false, in, out, st)) return e;
+      in.mode = IN_POINTS; in.pts = ts ? pts + 3 * j0 : pts; in.dirs = ts ? dirs + 3 * j0 : dirs; in.M = m;
+      if (int e = run_mlp(h, which, false, in, out, st, (ts && ts->ws) ? &em : nullptr)) return e;
       if (int e = launch_occ_expand(out, idx + j0, m, raw_buf.as<float>(), st, &h->launches)) return e;
     }
     return 0;
@@ -323,8 +389,8 @@ int render_chunk(NmHandle h, const RayBatch& rb, int flags, uint64_t seed, const
     a.t = t; a.dirs = rb.dirs; a.R = R; a.S = s; a.noise_std = c.noise_std; a.seed = seed ^ salt;
     a.white_bg = c.white_background; a.training = training ? 1 : 0; a.thr = c.attenuation_threshold;
     a.rgb = rgb; a.depth = depth; a.depth_raw = depth_raw; a.acc = acc; a.disp = disp; a.weights = w; a.mask_weights = mw;
-    if (skip) {
-      if (int e = skip_raw(which, raw_buf, t, s)) return e;
+    if (skip || tsk) {
+      if (int e = skip_raw(which, raw_buf, t, s, tsk ? &tsk[which] : nullptr)) return e;
       a.raw = raw_buf.as<float>();
       return launch_composite(a, st, &h->launches);
     }
@@ -395,15 +461,21 @@ int render_rays_impl(NmHandle h, const float* origins, int o_stride, const float
   NM_CHECK((near_dev == nullptr) == (far_dev == nullptr), "near_dev / far_dev must be given together");
   NM_CHECK(near_dev || nf_host, "no near/far bounds given");
   NM_CHECK(h->s_table.p != nullptr, "sampler tables missing");
+  if (int e = check_train_skip(h, flags)) return e;
   const int S = out_samples(h, flags);
   const long long kChunk = chunk_rays();
+  double committed = 0;
+  TrainSkip ts[2];                   // a forward-only training render: nothing is kept for a backward
+  ts[0].committed = ts[1].committed = &committed;
+  TrainSkip* tsk = (flags & NM_FLAG_SKIP_EMPTY_TRAIN) ? ts : nullptr;
   for (long long r0 = 0; r0 < R; r0 += kChunk) {
     RayBatch rb{};
     rb.R = (R - r0 < kChunk) ? R - r0 : kChunk;
     rb.origins = origins + (long long)o_stride * r0; rb.o_stride = o_stride; rb.dirs = dirs + 3 * r0;
     if (nf_host) { rb.nf[0] = nf_host[0]; rb.nf[1] = nf_host[1]; }
     rb.near_dev = near_dev ? near_dev + r0 : nullptr; rb.far_dev = far_dev ? far_dev + r0 : nullptr;
-    if (int e = render_chunk(h, rb, flags, seed + (uint64_t)r0, offset_out(out, r0, S, h->cfg.num_coarse), st)) return e;
+    if (int e = render_chunk(h, rb, flags, seed + (uint64_t)r0, offset_out(out, r0, S, h->cfg.num_coarse), st, nullptr, nullptr,
+                             false, tsk)) return e;
   }
   return 0;
 }
@@ -447,6 +519,46 @@ int ensure_grads(NmHandle h, cudaStream_t st, bool zero) {
   return 0;
 }
 
+// sub-chunks of the network backward's walk: `waves` full waves of 128-point row blocks (one per SM) bound the activation
+// workspace (~20 KB per point)
+long long train_walk_points(NmHandle h) {
+  static const int waves = [] { const char* e = getenv("NM_TRAIN_WAVES"); int v = e ? atoi(e) : 0; return v > 0 ? v : 16; }();
+  return (long long)h->num_sms * 128 * waves;
+}
+
+// The backward of one skipping training pass (NM_FLAG_SKIP_EMPTY_TRAIN, DESIGN §4.15): the compositor adjoint over the
+// whole (R,s) buffer stores the rows of the evaluated samples only, compacted in index-list order, and the network
+// backward runs over the staged points and directions — on the operands the forward emitted, or in ranges of the staged
+// list with a recompute each.  A pass with no evaluated sample launches nothing: every skipped row is zero (alpha = 0
+// and a closed relu gate), so it adds nothing to any gradient.
+int train_skip_backward(NmHandle h, const RayBatch& rb, const float* raw, const float* t, int s, const float* d_rgb, uint64_t seed,
+                        int which, const TrainSkip& T, cudaStream_t st) {
+  const NmRenderCfg& c = h->cfg;
+  if (T.M == 0) return 0;
+  const bool use_tc = c.precision != NM_PREC_FP32;
+  if (int e = h->dout.ensure((size_t)T.M * 16)) return e;
+  if (int e = h->trans.ensure((size_t)rb.R * s * 4)) return e;
+  if (int e = launch_composite_backward(raw, t, rb.dirs, d_rgb, rb.R, s, c.noise_std, seed, c.white_background,
+                                        h->trans.as<float>(), h->dout.as<float>(), st, &h->launches, T.pos)) return e;
+  NetGrads g{h->g_wt[which].as<float>(), h->g_bias[which].as<float>(), h->g_head[which].as<float>()};
+  TrainMode md{use_tc ? 1 : 0, c.precision == NM_PREC_FAST ? 1 : 3, h->d_err};
+  MlpInput in{};
+  in.mode = IN_POINTS;
+  if (T.ws) {
+    in.pts = T.pts; in.dirs = T.dirs; in.M = T.M;
+    return mlp_backward(h->nets[which], in, h->dout.as<float>(), T.ws, &g, h->num_sms, md, st, &h->launches, 1);
+  }
+  long long sub = train_walk_points(h);
+  if (sub > T.M) sub = T.M;
+  if (int e = h->train_ws.ensure(train_ws_bytes(h->nets[which].full, sub, use_tc) + 1024)) return e;
+  float* ws = reinterpret_cast<float*>(((uintptr_t)h->train_ws.p + 1023) & ~(uintptr_t)1023);
+  for (long long j0 = 0; j0 < T.M; j0 += sub) {
+    in.pts = T.pts + 3 * j0; in.dirs = T.dirs + 3 * j0; in.M = (T.M - j0 < sub) ? T.M - j0 : sub;
+    if (int e = mlp_backward(h->nets[which], in, h->dout.as<float>() + 4 * j0, ws, &g, h->num_sms, md, st, &h->launches)) return e;
+  }
+  return 0;
+}
+
 // One chunk of rays: forward (fills the per-sample workspaces), then for each bundle that carries a gradient the
 // compositor adjoint and the network backward over sub-chunks of points.
 int train_chunk(NmHandle h, const RayBatch& rb, int flags, uint64_t seed, const float* d_rgb, const float* d_rgb_coarse,
@@ -468,10 +580,24 @@ int train_chunk(NmHandle h, const RayBatch& rb, int flags, uint64_t seed, const 
   const double direct_gb = dg_env ? atof(dg_env) : 48.0;
   const size_t ws_main = use_tc && c.act_scale_log2 == 0 ? train_ws_bytes(h->nets[two ? NM_NET_FINE : NM_NET_COARSE].full, R * S, true) + 1024 : 0;
   const size_t ws_coarse = (ws_main && two) ? train_ws_bytes(h->nets[NM_NET_COARSE].full, R * Nc, true) + 1024 : 0;
-  const bool direct = ws_main > 0 && (double)(ws_main + ws_coarse) <= direct_gb * 1e9 && (d_rgb || target) && (!two || d_rgb_coarse || target);
+  // Skipping (NM_FLAG_SKIP_EMPTY_TRAIN): each pass decides from its evaluated count M, known only after its compaction,
+  // whether its operands are emitted (inside render_chunk, against the same budget); the dense sizing below is not used.
+  const bool tskip = flags & NM_FLAG_SKIP_EMPTY_TRAIN;
+  const bool direct = !tskip && ws_main > 0 && (double)(ws_main + ws_coarse) <= direct_gb * 1e9 && (d_rgb || target) &&
+                      (!two || d_rgb_coarse || target);
   float *ws_m = nullptr, *ws_c = nullptr;
   MlpEmit em_main{}, em_coarse{};
-  if (direct) {
+  double committed = 0;
+  TrainSkip ts[2];                 // [0] coarse (or only) pass, [1] fine pass
+  for (int k = 0; k < 2; ++k) {
+    const bool grad = target || ((two && k == 0) ? d_rgb_coarse : d_rgb);
+    ts[k].emit = use_tc && c.act_scale_log2 == 0 && grad;
+    ts[k].budget = direct_gb * 1e9;
+    ts[k].committed = &committed;
+  }
+  if (tskip) {
+    if (int e = render_chunk(h, rb, flags, seed, o, st, nullptr, nullptr, true, ts)) return e;
+  } else if (direct) {
     if (int e = h->train_ws.ensure(ws_main + ws_coarse + 2048)) return e;
     ws_m = reinterpret_cast<float*>(((uintptr_t)h->train_ws.p + 1023) & ~(uintptr_t)1023);
     train_emit_setup(h->nets[two ? NM_NET_FINE : NM_NET_COARSE].full, R * S, ws_m, &em_main);
@@ -505,6 +631,10 @@ int train_chunk(NmHandle h, const RayBatch& rb, int flags, uint64_t seed, const 
   for (int pi = 0; pi < np; ++pi) {
     const Pass& P = passes[pi];
     NetDev& net = h->nets[P.which];
+    if (tskip) {
+      if (int e = train_skip_backward(h, rb, P.raw, P.t, P.s, P.g, seed ^ P.salt, P.which, ts[P.which], st)) return e;
+      continue;
+    }
     if (int e = h->dout.ensure((size_t)R * P.s * 16)) return e;
     if (int e = h->trans.ensure((size_t)R * P.s * 4)) return e;
     if (int e = launch_composite_backward(P.raw, P.t, rb.dirs, P.g, R, P.s, c.noise_std, seed ^ P.salt,
@@ -518,9 +648,7 @@ int train_chunk(NmHandle h, const RayBatch& rb, int flags, uint64_t seed, const 
       if (int e = mlp_backward(h->nets[P.which], in, h->dout.as<float>(), wsp, &gd, h->num_sms, md, st, &h->launches, 1)) return e;
       continue;
     }
-    // sub-chunks of `waves` full waves of 128-point row blocks (one per SM): bounds the activation workspace (~20 KB per point)
-    static const int waves = [] { const char* e = getenv("NM_TRAIN_WAVES"); int v = e ? atoi(e) : 0; return v > 0 ? v : 16; }();
-    long long rays_sub = ((long long)h->num_sms * 128 * waves) / P.s;
+    long long rays_sub = train_walk_points(h) / P.s;
     if (rays_sub < 1) rays_sub = 1;
     if (rays_sub > R) rays_sub = R;
     if (int e = h->train_ws.ensure(train_ws_bytes(net.full, rays_sub * P.s, use_tc) + 1024)) return e;
@@ -545,6 +673,7 @@ int train_impl(NmHandle h, const float* origins, int o_stride, const float* dirs
   NM_CHECK(dirs && origins, "null ray pointers");
   NM_CHECK((near_dev == nullptr) == (far_dev == nullptr), "near_dev / far_dev must be given together");
   NM_CHECK(near_dev || nf_host, "no near/far bounds given");
+  if (int e = check_train_skip(h, flags)) return e;
   NM_CHECK(!(flags & NM_FLAG_TEACHER_T), "NM_FLAG_TEACHER_T is not supported by the backward pass");
   NM_CHECK(target || d_rgb || d_rgb_coarse, "no gradient source (target or d_rgb)");
   NM_CHECK(h->s_table.p != nullptr, "sampler tables missing");
@@ -624,6 +753,8 @@ int nm_destroy(NmHandle h) {
   h->train_ws.release(); h->dout.release(); h->trans.release();
   h->ss_tab.release(); h->ss_ws.release(); h->ms_ws.release(); h->nn_ws.release(); h->sg_ws.release();
   h->cc_ws.release(); h->dc_ws.release(); h->sp_ws.release(); h->tx_ws.release(); h->rs_ws.release(); h->sf_ws.release(); h->oc_ws.release(); h->sk_ws.release();
+  for (int i = 0; i < 2; ++i) { h->ts_ws[i].release(); h->ts_pts[i].release(); }
+  h->train_ws_c.release();
   h->occ[0].bits.release(); h->occ[1].bits.release(); h->mc_ws.release(); h->mc_ws2.release();
   if (h->h_err) cudaFreeHost(h->h_err);
   cudaFree(h->d_stats);
@@ -651,7 +782,7 @@ int nm_load_weights(NmHandle h, int which, int n_tensors, const char* const* nam
   NM_CHECK(which == NM_NET_COARSE || (which == NM_NET_FINE && h->has_fine), "network slot %d not present", which);
   WeightSource src;
   src.n = n_tensors; src.names = names; src.ptrs = tensors_host; src.numel = numel;
-  h->occ[which].valid = false;     // a grid describes the weights it was built from
+  h->occ[which].stale = true;      // a grid describes the weights it was built from: inference refuses it from now on
   return pack_network(h->desc[which], src, &h->nets[which]);
 }
 
@@ -661,7 +792,7 @@ int nm_load_weights_dev(NmHandle h, int which, int n_tensors, const char* const*
   NM_CHECK(which == NM_NET_COARSE || (which == NM_NET_FINE && h->has_fine), "network slot %d not present", which);
   WeightSource src;
   src.n = n_tensors; src.names = names; src.ptrs = tensors_dev; src.numel = numel;
-  h->occ[which].valid = false;     // a grid describes the weights it was built from
+  h->occ[which].stale = true;      // a grid describes the weights it was built from: inference refuses it from now on
   return load_network_dev(h->desc[which], src, &h->nets[which], (cudaStream_t)stream, &h->launches);
 }
 
@@ -721,6 +852,7 @@ int nm_render_image(NmHandle h, const float* pose_host, int H, int W, double foc
   if (int e = bind_checked(h)) return e;
   NM_CHECK(out_dev && pose_host && near_far_host, "null argument");
   NM_CHECK(0 <= row0 && row0 <= row1 && row1 <= H && W > 0, "bad row range");
+  NM_CHECK(!(flags & NM_FLAG_SKIP_EMPTY_TRAIN), "NM_FLAG_SKIP_EMPTY_TRAIN is taken by nm_render_rays, nm_backward_rays and nm_loss_backward");
   const long long R = (long long)(row1 - row0) * W;
   cudaStream_t st = (cudaStream_t)stream;
   if (int e = h->dirs.ensure((size_t)R * 12)) return e;
@@ -1383,6 +1515,7 @@ int nm_query_host(NmHandle h, const float* origins_host, int o_stride, const flo
   if (int e = bind_device(h)) return e;
   NM_CHECK(origins_host && dirs_host && near_far_host && out_host && R > 0, "bad arguments");
   NM_CHECK(!(flags & NM_FLAG_TEACHER_T), "NM_FLAG_TEACHER_T is a device-pointer feature");
+  NM_CHECK(!(flags & NM_FLAG_SKIP_EMPTY_TRAIN), "NM_FLAG_SKIP_EMPTY_TRAIN is taken by nm_render_rays, nm_backward_rays and nm_loss_backward");
   cudaStream_t st = h->own_stream;
   const size_t ob = o_stride ? (size_t)R * 12 : 12;
   if (int e = h->stage_in[0].ensure(ob)) return e;
@@ -1589,6 +1722,7 @@ int nm_build_occupancy(NmHandle h, int which, const float* box_host, int G, floa
   memcpy(g.lo, p.lo, sizeof(p.lo)); memcpy(g.hi, p.hi, sizeof(p.hi)); memcpy(g.inv, p.inv, sizeof(p.inv));
   g.G = G;
   g.valid = true;
+  g.stale = false;
   return 0;
 }
 
@@ -1605,13 +1739,14 @@ int nm_set_occupancy(NmHandle h, int which, const float* box_host, int G, const 
   memcpy(g.lo, p.lo, sizeof(p.lo)); memcpy(g.hi, p.hi, sizeof(p.hi)); memcpy(g.inv, p.inv, sizeof(p.inv));
   g.G = G;
   g.valid = true;
+  g.stale = false;
   return 0;
 }
 
 int nm_occupancy_query(NmHandle h, int which, const float* pts_dev, int64_t M, uint8_t* evaluated_out_dev, void* stream) {
   if (int e = bind_checked(h)) return e;
   NM_CHECK(which == NM_NET_COARSE || (which == NM_NET_FINE && h->has_fine), "network slot %d not present", which);
-  NM_CHECK(h->occ[which].valid, "no occupancy grid for network %d", which);
+  NM_CHECK(h->occ[which].valid && !h->occ[which].stale, "no occupancy grid for network %d", which);
   NM_CHECK(M >= 0 && (M == 0 || (pts_dev && evaluated_out_dev)), "bad arguments");
   return launch_occ_query(occ_lookup(h->occ[which]), pts_dev, M, evaluated_out_dev, (cudaStream_t)stream, &h->launches);
 }

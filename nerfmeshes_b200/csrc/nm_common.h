@@ -181,9 +181,11 @@ struct TrainMode { int use_tc; int n_passes; int* d_err; };
 int mlp_backward(NetDev& net, const MlpInput& in, const float* dout, float* ws, NetGrads* g, int num_sms,
                  const TrainMode& mode, cudaStream_t st, int64_t* launches, int have_acts = 0);
 void train_emit_setup(const NetProgram& full, long long points, float* ws, MlpEmit* emit);
+// pos: NULL, dout (R,S,4); or the exclusive scan of a skipping pass's marks (R*S + 1 entries, nm_occupancy.cu), and dout
+// holds only the evaluated samples' rows, sample m's at pos[m] (empty-space skipping in training, DESIGN §4.15)
 int launch_composite_backward(const float* raw, const float* t, const float* dirs, const float* d_rgb, long long R, int S,
                               float noise_std, uint64_t seed, int white_bg, float* scratch, float* dout,
-                              cudaStream_t st, int64_t* launches);
+                              cudaStream_t st, int64_t* launches, const int* pos = nullptr);
 int launch_mse_grad(const float* rgb, const float* target, long long n, long long count, float* d_rgb, float* loss,
                     cudaStream_t st, int64_t* launches);
 // density gradient g = d raw sigma / d p (nm_sigma_grad.cu, orchestrated by sigma_grad in nm_train.cu; DESIGN 4.8)

@@ -465,14 +465,19 @@ struct CompositeBwdArgs {
   uint64_t seed;
   int white_bg;
   float* scratch;     // (R,S) transmittance
-  float* dout;        // (R,S,4)
+  float* dout;        // (R,S,4), or (M,4) with pos
+  const int* pos;     // compact variant: exclusive scan of the evaluated marks (R*S + 1); sample m is evaluated iff
+                      // pos[m+1] > pos[m], and its row goes to dout[pos[m]] (a skipped sample's is dropped: it is zero)
 };
 
 // One WARP per ray (a training chunk has a few thousand rays: a thread per ray leaves the GPU idle behind a serial
 // 2 x S-step dependency chain).  Lane l owns the contiguous samples [l*seg, (l+1)*seg): transmittance = exclusive product
 // scan of the segment products across lanes times the running product inside the segment; the suffix sum the same way
 // from the other end.  Association differs from the forward kernel's serial product by rounding only.
+// kCompact: the training pass of empty-space skipping — the same arithmetic, only the rows of evaluated samples are
+// stored, in index-list order, for the network backward over the staged points.
 constexpr int kCbSeg = 16;                  // samples per lane held in registers: S <= 512
+template <bool kCompact>
 __global__ void __launch_bounds__(128) composite_backward_kernel(const __grid_constant__ CompositeBwdArgs a) {
   const long long ray = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (ray >= a.R) return;
@@ -551,7 +556,12 @@ __global__ void __launch_bounds__(128) composite_backward_kernel(const __grid_co
       o.z = gb * w * q[u].z * (1.0f - q[u].z);
       o.w = (pre[u] > 0.f) ? dalpha * dist[u] * e : 0.f;                     // relu, alpha = 1 - exp(-sigma dist)
       if (!isfinite(o.w)) o.w = 0.f;                                         // dist = 1e10 on the last sample: 1e10 * 0
-      dout[i] = o;
+      if (kCompact) {
+        const int p = a.pos[ray * S + i];
+        if (a.pos[ray * S + i + 1] != p) reinterpret_cast<float4*>(a.dout)[p] = o;
+      } else {
+        dout[i] = o;
+      }
     }
   }
 }
@@ -656,11 +666,12 @@ void train_emit_setup(const NetProgram& G, long long P, float* ws_base, MlpEmit*
 
 int launch_composite_backward(const float* raw, const float* t, const float* dirs, const float* d_rgb, long long R, int S,
                               float noise_std, uint64_t seed, int white_bg, float* scratch, float* dout,
-                              cudaStream_t st, int64_t* launches) {
+                              cudaStream_t st, int64_t* launches, const int* pos) {
   if (R <= 0) return 0;
   NM_CHECK(S <= 32 * kCbSeg, "sample count %d exceeds the compositor adjoint's limit (%d)", S, 32 * kCbSeg);
-  CompositeBwdArgs a{raw, t, dirs, d_rgb, R, S, noise_std, seed, white_bg, scratch, dout};
-  composite_backward_kernel<<<(unsigned)((R + 3) / 4), 128, 0, st>>>(a);
+  CompositeBwdArgs a{raw, t, dirs, d_rgb, R, S, noise_std, seed, white_bg, scratch, dout, pos};
+  if (pos) composite_backward_kernel<true><<<(unsigned)((R + 3) / 4), 128, 0, st>>>(a);
+  else composite_backward_kernel<false><<<(unsigned)((R + 3) / 4), 128, 0, st>>>(a);
   NM_CUDA(cudaGetLastError());
   if (launches) ++*launches;
   return 0;

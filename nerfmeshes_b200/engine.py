@@ -83,7 +83,8 @@ class Engine:
         dc = net_desc(**coarse)
         df = net_desc(**fine) if fine is not None else None
         cfg = settings.to_c()
-        self._occupancy = set()         # network slots with a grid built from their current weights (a weight load drops it)
+        self._occupancy = set()         # network slots with a grid built from their current weights
+        self._occupancy_stale = set()   # network slots whose grid predates their weights (a weight load): training skipping only
         L.check(self.lib.nm_create(device, C.byref(dc), C.byref(df) if df is not None else None, C.byref(cfg),
                                    C.byref(self._h)))
 
@@ -125,7 +126,9 @@ class Engine:
             keep.append(a)
             names.append(k.encode())
         n = len(names)
-        self._occupancy.discard(which)
+        if which in self._occupancy:
+            self._occupancy.discard(which)
+            self._occupancy_stale.add(which)
         args = (self._h, which, n, (C.c_char_p * n)(*names), (C.c_void_p * n)(*ptrs), (C.c_int64 * n)(*numel))
         if on_dev:
             L.check(self.lib.nm_load_weights_dev(*args, self._stream()))
@@ -207,11 +210,12 @@ class Engine:
     DEFAULT_OUT = ("rgb", "depth", "depth_raw", "acc", "disp", "weights", "mask_weights")
 
     def render_rays(self, origins, dirs, near, far, *, training=False, buff=False, seed=0, want=None,
-                    teacher_t: Optional[torch.Tensor] = None, out=None, skip_empty=None) -> Dict[str, torch.Tensor]:
+                    teacher_t: Optional[torch.Tensor] = None, out=None, skip_empty=None,
+                    train_skip=False) -> Dict[str, torch.Tensor]:
         """NeRFModel.forward / BuFFModel.forward on a ray batch.  origins (3,), (1,3) or (R,3); dirs (R,3);
         near/far python floats / 0-dim tensors, or (R,) tensors (CUDA path only).  skip_empty: send only the samples the
         occupancy grids mark through the networks (NM_FLAG_SKIP_EMPTY, DESIGN 4.15); None = `self.skip_empty` outside
-        training."""
+        training.  train_skip: the same in a training render (NM_FLAG_SKIP_EMPTY_TRAIN), on grids that may be stale."""
         want = tuple(want or self.DEFAULT_OUT)
         dirs_t = torch.as_tensor(dirs)
         host = not dirs_t.is_cuda
@@ -225,7 +229,7 @@ class Engine:
         else:
             assert o.shape == (R, 3), "origins must be (3,), (1,3) or (R,3)"
             o_stride = 3
-        flags = self._flags(training, buff, skip_empty)
+        flags = self._flags(training, buff, skip_empty, train_skip)
         S = self.num_samples(buff)
         per_ray = isinstance(near, torch.Tensor) and near.dim() > 0 and near.shape[0] == R and near.numel() == R and R > 1
         nf = (C.c_float * 2)(0.0, 0.0)
@@ -273,26 +277,29 @@ class Engine:
     def zero_grad(self):
         L.check(self.lib.nm_zero_grad(self._h, self._stream()))
 
-    def backward_rays(self, origins, dirs, near, far, d_rgb, d_coarse_rgb=None, *, training=True, buff=False, seed=0):
+    def backward_rays(self, origins, dirs, near, far, d_rgb, d_coarse_rgb=None, *, training=True, buff=False, seed=0,
+                      train_skip=False):
         """Accumulate dL/dtheta given dL/d rgb_map of the main (and optionally the coarse) bundle; the forward is
-        re-run inside with the same flags and seed (same samples, same noise)."""
+        re-run inside with the same flags and seed (same samples, same noise).  train_skip: empty-space skipping on the
+        current grids (NM_FLAG_SKIP_EMPTY_TRAIN); the forward being differentiated must have used the same grids."""
         o, o_stride, d, R, nf, near_d, far_d = self._ray_args(origins, dirs, near, far)
         g = None if d_rgb is None else _f32c(d_rgb, d.device)
         gc = None if d_coarse_rgb is None else _f32c(d_coarse_rgb, d.device)
         assert (g is None or g.shape == (R, 3)) and (gc is None or gc.shape == (R, 3))
-        flags = self._flags(training, buff)
+        flags = self._flags(training, buff, None, train_skip)
         if R:
             L.check(self.lib.nm_backward_rays(self._h, _ptr(o), o_stride, _ptr(d), R, nf, _ptr(near_d), _ptr(far_d), flags,
                                               seed, _ptr(g), _ptr(gc), self._stream()))
 
-    def loss_backward(self, origins, dirs, near, far, target_rgb, *, training=True, buff=False, seed=0):
+    def loss_backward(self, origins, dirs, near, far, target_rgb, *, training=True, buff=False, seed=0, train_skip=False):
         """The reference's training loss and its backward in one call: returns a (2,) device tensor
-        [mse(coarse-or-only rgb_map, target), mse(fine rgb_map, target)] (src/models/model_nerf.py:118-126)."""
+        [mse(coarse-or-only rgb_map, target), mse(fine rgb_map, target)] (src/models/model_nerf.py:118-126).
+        train_skip: empty-space skipping on the current grids (NM_FLAG_SKIP_EMPTY_TRAIN, DESIGN 4.15)."""
         o, o_stride, d, R, nf, near_d, far_d = self._ray_args(origins, dirs, near, far)
         tgt = _f32c(target_rgb, d.device)
         assert tgt.shape == (R, 3)
         loss = torch.zeros(2, dtype=torch.float32, device=d.device)
-        flags = self._flags(training, buff)
+        flags = self._flags(training, buff, None, train_skip)
         if R:
             L.check(self.lib.nm_loss_backward(self._h, _ptr(o), o_stride, _ptr(d), R, nf, _ptr(near_d), _ptr(far_d), flags,
                                               seed, _ptr(tgt), _ptr(loss), self._stream()))
@@ -304,20 +311,27 @@ class Engine:
         return out
 
     # ------------------------------------------------------------------ BuFF tree maintenance (SURVEY §8f-4)
-    def _flags(self, training, buff, skip_empty=None):
+    def _flags(self, training, buff, skip_empty=None, train_skip=False):
         """render-call flags; `voxel_random` mirrors cfg.tree.use_random_sampling (src/nerf/tree.py:280).  skip_empty None
         follows `self.skip_empty` outside training; an explicit True is passed on as asked (the library rejects it in
+        training).  train_skip: NM_FLAG_SKIP_EMPTY_TRAIN, on fresh or stale grids (the library rejects it outside
         training)."""
         skip = (self.skip_empty and not training) if skip_empty is None else bool(skip_empty)
+        nets = (L.NET_COARSE,) if buff or not self.has_fine else (L.NET_COARSE, L.NET_FINE)
         if skip:
-            for which in ((L.NET_COARSE,) if buff or not self.has_fine else (L.NET_COARSE, L.NET_FINE)):
+            for which in nets:
                 if which not in self._occupancy:
                     raise L.NmError(f"empty-space skipping: network {which} has no occupancy grid for its current weights "
                                     "(the weights changed after build_occupancy_grid, or none was built); call "
                                     "build_occupancy_grid again")
+        if train_skip:
+            for which in nets:
+                if which not in self._occupancy and which not in self._occupancy_stale:
+                    raise L.NmError(f"training-time empty-space skipping: network {which} has no occupancy grid; call "
+                                    "enable_training_skip (or build_occupancy_grid) first")
         return ((L.FLAG_TRAINING if training else 0) | (L.FLAG_BUFF if buff else 0) |
                 (L.FLAG_RANDOM_VOXELS if buff and getattr(self, "voxel_random", False) else 0) |
-                (L.FLAG_SKIP_EMPTY if skip else 0))
+                (L.FLAG_SKIP_EMPTY if skip else 0) | (L.FLAG_SKIP_EMPTY_TRAIN if train_skip else 0))
 
     # ------------------------------------------------------------------ empty-space skipping (DESIGN 4.15)
     @staticmethod
@@ -338,6 +352,7 @@ class Engine:
         b = self._box(box)
         bits = torch.empty(self.occupancy_words(res), dtype=torch.int32, device=self.device)
         self._occupancy.discard(which)
+        self._occupancy_stale.discard(which)
         L.check(self.lib.nm_build_occupancy(self._h, which, b.ctypes.data, int(res), float(threshold), int(dilate), _ptr(bits),
                                             self._stream()))
         self._occupancy.add(which)
@@ -346,6 +361,7 @@ class Engine:
     def set_occupancy(self, which: int, box, res: int, bits: Optional[torch.Tensor]):
         """Install caller bits (layout of build_occupancy) as network `which`'s grid; None removes it."""
         self._occupancy.discard(which)
+        self._occupancy_stale.discard(which)
         if bits is None:
             L.check(self.lib.nm_set_occupancy(self._h, which, None, 0, None))
             return
@@ -365,7 +381,8 @@ class Engine:
         return out.bool().reshape(lead)
 
     def skip_stats(self) -> Dict[str, int]:
-        """Samples seen / evaluated per pass by skipping renders since the last call (nm_skip_stats); resets them."""
+        """Samples seen / evaluated per pass by skipping renders and skipping training passes since the last call
+        (nm_skip_stats); resets them."""
         out = (C.c_int64 * 4)()
         L.check(self.lib.nm_skip_stats(self._h, out))
         return dict(coarse_seen=out[0], coarse_evaluated=out[1], fine_seen=out[2], fine_evaluated=out[3])

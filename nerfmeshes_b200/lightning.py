@@ -114,6 +114,11 @@ class LightningHooks:
 
     # ------------------------------------------------------------------ model_nerf.py:88-151 / model_buff.py:75-117
     def training_step(self, ray_batch, batch_idx):
+        # nerf.train.occupancy_every (optional; absent or 0 = off): empty-space skipping in training, grids rebuilt every
+        # that many steps (BaseModel.enable_training_skip, DESIGN 4.15)
+        every = int(self.cfg.nerf.train.get("occupancy_every", 0) or 0)
+        if every and (self._train_skip is None or self._train_skip["every"] != every):
+            self.enable_training_skip(every=every)
         b = _ray_batch(ray_batch)
         dev = self.device
         o, d, tgt = b["ray_origins"].to(dev), b["ray_directions"].to(dev), b["ray_targets"].to(dev)

@@ -115,8 +115,9 @@ class _RenderGrad(torch.autograd.Function):
     autograd one gradient per parameter — what loss.backward() yields in the reference (model_nerf.py:88-151)."""
 
     @staticmethod
-    def forward(ctx, model, rays, seed, buff, training, rgb, coarse_rgb, *params):
+    def forward(ctx, model, rays, seed, buff, training, train_skip, rgb, coarse_rgb, *params):
         ctx.model, ctx.rays, ctx.seed, ctx.buff, ctx.training = model, rays, seed, buff, training
+        ctx.train_skip = train_skip        # the grids the forward skipped on are still installed: they change only at a step
         ctx.has_coarse = coarse_rgb is not None
         if coarse_rgb is None:
             return rgb.clone()
@@ -129,9 +130,9 @@ class _RenderGrad(torch.autograd.Function):
         o, d, near, far = ctx.rays
         eng.zero_grad()
         eng.backward_rays(o, d, near, far, g_rgb, g_coarse if ctx.has_coarse else None, training=ctx.training,
-                          buff=ctx.buff, seed=ctx.seed)
+                          buff=ctx.buff, seed=ctx.seed, train_skip=ctx.train_skip)
         grads = [eng.get_grad(which, name, p) for which, name, p in model._named_net_params()]
-        return (None,) * 7 + tuple(grads)
+        return (None,) * 8 + tuple(grads)
 
 
 class BaseModel(torch.nn.Module):
@@ -155,6 +156,7 @@ class BaseModel(torch.nn.Module):
         self._eng: Optional[Engine] = None
         self._synced = {}
         self._cuda_index = None
+        self._train_skip = None          # enable_training_skip's settings and schedule state, or None (off)
 
     # ------------------------------------------------------------------ engine plumbing
     def _nets(self):
@@ -212,6 +214,21 @@ class BaseModel(torch.nn.Module):
         self._eng.skip_empty = bool(self.skip_empty) and not self.training     # training renders stay dense
         return self._eng
 
+    def _occupancy_box(self, box, what):
+        """The grid box: the caller's, else [near - mean, far - mean]^3 with mean = (near + far) / 2; NDC needs one."""
+        if box is not None:
+            return box
+        if _cfg_get(self.cfg, "dataset.use_ndc", False):
+            raise L.NmError(f"{what}: an NDC model needs an explicit box (NDC coordinates)")
+        near, far = float(self.cfg.dataset.near), float(self.cfg.dataset.far)
+        mean = (near + far) / 2
+        return [near - mean] * 3 + [far - mean] * 3
+
+    def _build_grids(self, res, box, threshold, dilate):
+        eng = self._engine()
+        return {which: eng.build_occupancy(which, box, res, threshold, dilate)
+                for which, net in enumerate(self._nets()) if net is not None}
+
     def build_occupancy_grid(self, res: int = 128, box=None, threshold: float = -10.0, dilate: int = 2):
         """Occupancy grids of every network from its own density (Engine.build_occupancy, DESIGN 4.15), then skip_empty:
         eval-mode renders (forward, query, eval_poses, render_image_sharded, surface_points, compare_with_nerf) send only
@@ -221,20 +238,47 @@ class BaseModel(torch.nn.Module):
         hi_z) in network-input coordinates; default [near - mean, far - mean]^3 with mean = (near + far) / 2 (the BuFF
         tree's root box); an NDC model needs an explicit box.  Changing the weights afterwards makes the next skipping
         render raise until the grids are built again.  Returns {slot: bits}."""
-        if box is None:
-            if _cfg_get(self.cfg, "dataset.use_ndc", False):
-                raise L.NmError("build_occupancy_grid: an NDC model needs an explicit box (NDC coordinates)")
-            near, far = float(self.cfg.dataset.near), float(self.cfg.dataset.far)
-            mean = (near + far) / 2
-            box = [near - mean] * 3 + [far - mean] * 3
-        eng = self._engine()
-        out = {}
-        for which, net in enumerate(self._nets()):
-            if net is not None:
-                out[which] = eng.build_occupancy(which, box, res, threshold, dilate)
+        out = self._build_grids(res, self._occupancy_box(box, "build_occupancy_grid"), threshold, dilate)
         self.skip_empty = True
         self._engine()
         return out
+
+    def enable_training_skip(self, every: int = 16, res: int = 128, box=None, threshold: float = -10.0, dilate: int = 2):
+        """Empty-space skipping in training (NM_FLAG_SKIP_EMPTY_TRAIN, DESIGN 4.15): every training-mode render (forward
+        in train mode and its backward, train.training_step) sends only the samples its network's occupancy grid marks
+        through the network.  The grids (parameters and default box as build_occupancy_grid) are rebuilt from the current
+        weights before the first training render and then whenever the step has advanced by `every` since the last
+        rebuild; the step is `global_step` when training_step is given one, else the count of training_step calls (of
+        training-mode forward calls outside training_step).  A ray whose skipped samples all have a noisy pre-activation
+        <= 0 trains exactly as the dense step.  Eval-mode skipping stays `skip_empty`'s (build_occupancy_grid).  Grids are
+        not stored in checkpoints: a resumed run rebuilds at its first step.  Under torchrun every rank rebuilds from the
+        same weights with the same deterministic build, so the ranks' grids agree.  every = 0 switches it off."""
+        every = int(every)
+        if every < 0:
+            raise ValueError("enable_training_skip: every must be >= 0")
+        if every == 0:
+            self._train_skip = None
+            return
+        self._train_skip = dict(every=every, res=int(res), box=self._occupancy_box(box, "enable_training_skip"),
+                                threshold=float(threshold), dilate=int(dilate), built=None, calls=0, in_step=False,
+                                rebuilds=[])
+
+    def _train_skip_tick(self, step=None):
+        """Start of a training step: rebuild the grids when the schedule says so.  Returns whether the step skips.  Inside
+        training_step (`in_step`) a forward does not tick again, so no rebuild falls between a forward and its backward."""
+        ts = self._train_skip
+        if ts is None or not self.training:
+            return False
+        if ts["in_step"] and step is None:
+            return True
+        if step is None:
+            step = ts["calls"]
+            ts["calls"] += 1
+        if ts["built"] is None or step < ts["built"] or step - ts["built"] >= ts["every"]:
+            self._build_grids(ts["res"], ts["box"], ts["threshold"], ts["dilate"])
+            ts["built"] = step
+            ts["rebuilds"].append(step)
+        return True
 
     def _after_engine_created(self):
         pass
@@ -257,7 +301,7 @@ class BaseModel(torch.nn.Module):
         self._seed_counter = getattr(self, "_seed_counter", 0) + 1
         return (torch.initial_seed() * 1000003 + self._seed_counter) & 0x7FFFFFFFFFFFFFFF
 
-    def _attach_grad(self, rays, seed, buff, rgb, coarse_rgb=None):
+    def _attach_grad(self, rays, seed, buff, rgb, coarse_rgb=None, train_skip=False):
         """Make rgb maps differentiable w.r.t. the network parameters when autograd is recording."""
         named = self._named_net_params()
         # training mode only: evaluation scripts call query() outside torch.no_grad() and expect plain tensors
@@ -265,7 +309,7 @@ class BaseModel(torch.nn.Module):
             return rgb, coarse_rgb
         if not rgb.is_cuda:
             raise L.NmError("training needs CUDA ray tensors (the backward pass has no host-buffer variant)")
-        res = _RenderGrad.apply(self, rays, seed, buff, self.training, rgb, coarse_rgb, *[p for _, _, p in named])
+        res = _RenderGrad.apply(self, rays, seed, buff, self.training, train_skip, rgb, coarse_rgb, *[p for _, _, p in named])
         return (res, None) if coarse_rgb is None else res
 
     def _mode_cfg(self):
@@ -403,13 +447,16 @@ class NeRFModel(BaseModel):
 
     def forward(self, x, seed=None):
         ray_origins, ray_directions, near, far = self._unpack(x)
+        tskip = self._train_skip_tick()
         eng = self._engine()
         seed = self._pick_seed(seed)
         want = ["rgb", "depth", "depth_raw", "acc", "disp", "weights", "mask_weights"]
         if self.model_fine is not None:
             want += ["coarse_rgb", "coarse_acc", "coarse_disp", "coarse_weights"]
-        o = eng.render_rays(ray_origins, ray_directions, near, far, training=self.training, seed=seed, want=want)
-        o["rgb"], crgb = self._attach_grad((ray_origins, ray_directions, near, far), seed, False, o["rgb"], o.get("coarse_rgb"))
+        o = eng.render_rays(ray_origins, ray_directions, near, far, training=self.training, seed=seed, want=want,
+                            train_skip=tskip)
+        o["rgb"], crgb = self._attach_grad((ray_origins, ray_directions, near, far), seed, False, o["rgb"], o.get("coarse_rgb"),
+                                           tskip)
         if crgb is not None:
             o["coarse_rgb"] = crgb
         main = OutputBundle(o["rgb"], o["depth"], o["weights"], o["mask_weights"], o["acc"], o["disp"], o["depth_raw"])
@@ -467,11 +514,13 @@ class BuFFModel(BaseModel):
         seed = self._pick_seed(seed)
         if torch.as_tensor(ray_origins).dim() < 2:
             raise IndexError("BuFFModel needs ray origins of shape (1,3) or (R,3) (src/nerf/tree.py:231)")
+        tskip = self._train_skip_tick()
         eng = self._engine()
         self._sync_tree(eng)
         eng.voxel_random = bool(_cfg_get(self.cfg, "tree.use_random_sampling", False))      # src/nerf/tree.py:280
         o = eng.render_rays(ray_origins, ray_directions, near, far, training=self.training, buff=True, seed=seed,
-                            want=["rgb", "depth", "depth_raw", "acc", "disp", "weights", "mask_weights", "t_vals"])
+                            want=["rgb", "depth", "depth_raw", "acc", "disp", "weights", "mask_weights", "t_vals"],
+                            train_skip=tskip)
         if self.training and o["rgb"].is_cuda:
             # accumulate the (detached) sample weights into the voxels (model_buff.py:65-66; tree.py:177-206)
             step_gate = int(_cfg_get(self.cfg, "tree.step_size_integration_offset", 0) or 0)
@@ -479,7 +528,7 @@ class BuFFModel(BaseModel):
                 idx = eng.ray_voxel_indices(ray_origins, ray_directions, near, far, seed=seed)
                 eng.check_flags()      # a truncated hit list (> 512 voxels on a ray) must not reach the tree statistics
                 self.tree.ray_batch_integration(self.global_step, idx, o["weights"], o["mask_weights"])
-        o["rgb"], _ = self._attach_grad((ray_origins, ray_directions, near, far), seed, True, o["rgb"])
+        o["rgb"], _ = self._attach_grad((ray_origins, ray_directions, near, far), seed, True, o["rgb"], None, tskip)
         b = OutputBundle(o["rgb"], o["depth"], o["weights"], o["mask_weights"], o["acc"], o["disp"], o["depth_raw"])
         b.t_vals = o["t_vals"]
         return b

@@ -30,6 +30,19 @@ def training_step(model, ray_batch, ray_targets, *, chunksize: Optional[int] = N
         raise RuntimeError("training_step needs model.train()")
     if global_step is not None:
         model.global_step = int(global_step)
+    # empty-space skipping (BaseModel.enable_training_skip): the schedule ticks once per step, here, before any render
+    ts = model._train_skip
+    tskip = model._train_skip_tick(None if global_step is None else int(global_step))
+    if ts is not None:
+        ts["in_step"] = True
+    try:
+        return _step(model, ray_batch, ray_targets, chunksize, seed, group, allreduce, tskip)
+    finally:
+        if ts is not None:
+            ts["in_step"] = False
+
+
+def _step(model, ray_batch, ray_targets, chunksize, seed, group, allreduce, tskip):
     named = model._named_net_params()
     if type(model).__name__ == "BuFFModel":
         # through forward(): it owns the tree-integration hook (model_buff.py:65-66); gradients via the autograd bridge
@@ -56,7 +69,8 @@ def training_step(model, ray_batch, ray_targets, *, chunksize: Optional[int] = N
     for i in range(0, R, chunk):
         sl = slice(i, i + chunk)
         o = ray_origins[sl] if per_ray_o else ray_origins
-        loss += eng.loss_backward(o, ray_directions[sl], near, far, ray_targets[sl], training=True, seed=base_seed + i)
+        loss += eng.loss_backward(o, ray_directions[sl], near, far, ray_targets[sl], training=True, seed=base_seed + i,
+                                  train_skip=tskip)
     for which, name, p in named:
         g = eng.get_grad(which, name, p)
         p.grad = g.div_(n_chunks) if p.grad is None else p.grad.add_(g.div_(n_chunks))
