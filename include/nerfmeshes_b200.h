@@ -529,6 +529,13 @@ int nm_debug_pack_wide(const NmNetDesc* desc, int n_tensors, const char* const* 
  * `samples_per_ray` samples (nm_mlp_tc.cu).  Returns the group size g = lcm(S,64)/64 (0: the fused compositor is not used
  * for this S); if tiles_out != NULL it receives the tile indices worker `cta` of `grid` workers processes, in order, for a launch of n_tiles tiles (at most cap entries; *n_out = count). */
 int nm_debug_tile_schedule(int samples_per_ray, int64_t n_tiles, int grid, int cta, int64_t* tiles_out, int64_t cap, int64_t* n_out);
+/* Host-only: the fused MLP kernel's shared-memory layout for a layer program (the NetProgram nm_debug_pack returns), a
+ * dynamic shared-memory limit of max_smem bytes, the fused compositor on (comp_on != 0) or off, inference (training == 0)
+ * or the training modes (which keep the bias and head vectors in shared memory) and a ring-slot cap (slot_cap <= 0: none;
+ * NM_MLP_RING_SLOTS sets it for launches).  out5 = {ring slots, activation buffers' offset, barriers' offset, compositor
+ * carry offset, total bytes}.  Fails (<0) when the network leaves room for fewer than two slots. */
+int nm_debug_mlp_layout(const void* program, size_t program_size, int max_smem, int comp_on, int training, int slot_cap,
+                        int64_t* out5);
 
 /* Device-side error flags, readable even after a kernel trapped: out2[0] = tensor-core pipeline watchdog code (0 = ok),
  * out2[1] = AABB hit-list overflow (a ray through more than 512 voxels; cleared once nm_check_flags or an entry point has
@@ -543,6 +550,10 @@ int nm_check_flags(NmHandle h, void* stream);
 /* ---- introspection ---------------------------------------------------------------------------------- */
 /* number of kernels launched through this handle since creation (bench.py's gpu_launches). */
 int64_t nm_launch_count(NmHandle h);
+/* number of points this handle has sent through a network's sigma-only program since creation: sigma-only point queries,
+ * the density sweeps, and the coarse pass of a two-network inference render that asks for no coarse colour (when the
+ * network has a separate sigma head, i.e. view directions). */
+int64_t nm_sigma_only_points(NmHandle h);
 /* duration in ms of the last fused-MLP launch sequence, measured with CUDA events on the call's stream when
  * timing is enabled (bench.py's roofline); <0 if disabled. */
 int nm_set_timing(NmHandle h, int enable);

@@ -104,7 +104,9 @@ _SIGNATURES = {
     "nm_check_flags": (C.c_int, [_P, _P]),
     "nm_ndc_rays": (C.c_int, [_P, _I, _I, _D, _D, _P, _I, _P, _L, _P, _P, _P]),
     "nm_launch_count": (C.c_int64, [_P]),
+    "nm_sigma_only_points": (C.c_int64, [_P]),
     "nm_debug_tile_schedule": (C.c_int, [_I, _L, _I, _I, _P, _L, _P]),
+    "nm_debug_mlp_layout": (C.c_int, [_P, C.c_size_t, _I, _I, _I, _I, _P]),
     "nm_set_timing": (C.c_int, [_P, _I]),
     "nm_mlp_time_ms": (C.c_double, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
 }

@@ -65,6 +65,7 @@ struct NmHandle_t {
   std::vector<cudaEvent_t> ev;
   size_t ev_used = 0;
   int64_t mlp_points = 0, mlp_launches = 0;
+  int64_t sigma_points = 0;        // points sent through a network's sigma-only program since creation
   Buf mc_ws, mc_ws2;               // marching cubes: the count step's bit masks and scans, read by the emit step; the emit
                                    // step's vertex / triangle records
   int64_t mc_counts[2] = {0, 0};   // {vertices, triangles} of the last count step: sizes of the emit step
@@ -235,6 +236,7 @@ int run_mlp(NmHandle h, int which, bool sigma_only, const MlpInput& in, float* o
   else rc = launch_mlp_tc(net, sigma_only, h->cfg.precision == NM_PREC_FAST ? 1 : 3, h->cfg.act_scale_log2, in, out,
                           h->num_sms, h->d_err, st, &h->launches, emit, comp);
   if (rc) return rc;
+  if (sigma_only) h->sigma_points += in.M;
   if (h->timing) {
     NM_CUDA(cudaEventRecord(e1, st));
     h->mlp_points += in.M;
@@ -395,7 +397,14 @@ int render_chunk(NmHandle h, const RayBatch& rb, int flags, uint64_t seed, const
       return launch_composite(a, st, &h->launches);
     }
     const bool fuse = fused_env && !need_raw && !emit && c.precision != NM_PREC_FP32 && mlp_tc_composite_group(s) > 0;
-    if (fuse) return run_mlp(h, which, false, rays_input(t, s), nullptr, st, nullptr, &a);
+    // The coarse pass of a two-network inference render whose caller reads no coarse colour: its weights (and so the fine
+    // samples), acc and disp depend on sigma alone, so the sigma-only program runs (bit-identical sigma, without the
+    // feature, direction and rgb layers).  A network without view directions has one output layer for rgb and sigma; its
+    // sigma-only program is the full one, so it keeps the full path.
+    const NetProgram& sp = h->nets[which].sigma;
+    const bool sigma_only = fuse && which == NM_NET_COARSE && Nf > 0 && !training && rgb == nullptr &&
+                            sp.layers[sp.n_layers - 1].kind == KIND_SIGMA;
+    if (fuse) return run_mlp(h, which, sigma_only, rays_input(t, s), nullptr, st, nullptr, &a);
     if (int e = raw_buf.ensure((size_t)R * s * 16)) return e;
     if (int e = run_mlp(h, which, false, rays_input(t, s), raw_buf.as<float>(), st, emit)) return e;
     a.raw = raw_buf.as<float>();
@@ -1612,6 +1621,8 @@ int nm_kernel_flags(NmHandle h, int32_t* out2) {
 
 int64_t nm_launch_count(NmHandle h) { return h ? h->launches : -1; }
 
+int64_t nm_sigma_only_points(NmHandle h) { return h ? h->sigma_points : -1; }
+
 int nm_debug_tile_schedule(int samples_per_ray, int64_t n_tiles, int grid, int cta, int64_t* tiles_out, int64_t cap, int64_t* n_out) {
   const int g = mlp_tc_composite_group(samples_per_ray);
   if (tiles_out && n_out) {
@@ -1626,6 +1637,17 @@ int nm_debug_tile_schedule(int samples_per_ray, int64_t n_tiles, int grid, int c
     *n_out = n;
   }
   return g;
+}
+
+int nm_debug_mlp_layout(const void* program, size_t program_size, int max_smem, int comp_on, int training, int slot_cap,
+                        int64_t* out5) {
+  NM_CHECK(program && out5, "null argument");
+  NM_CHECK(program_size >= sizeof(NetProgram), "program buffer too small (%zu needed)", sizeof(NetProgram));
+  MlpTcLayout l;
+  if (int e = mlp_tc_layout(*reinterpret_cast<const NetProgram*>(program), max_smem, comp_on != 0, training != 0, slot_cap, &l)) return e;
+  const int64_t v[5] = {l.num_stages, l.off_wg, l.off_bars, l.off_carry, l.bytes};
+  for (int i = 0; i < 5; ++i) out5[i] = v[i];
+  return 0;
 }
 
 int nm_set_timing(NmHandle h, int enable) {

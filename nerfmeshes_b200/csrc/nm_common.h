@@ -125,7 +125,15 @@ int debug_pack(const NmNetDesc& d, const WeightSource& src, bool sigma_only, boo
 struct CompositeArgs;
 // comp != nullptr (inference on ray inputs): the compositor runs inside the kernel on the staged outputs of every tile and
 // writes the per-ray maps (and weights, if asked); `out` is not written.  mlp_tc_composite_group(S) == 0: not eligible.
+// With sigma_only, comp is accepted too: the program's sigma enters the compositor with rgb (0, 0, 0), for a pass whose
+// caller reads no colour map (the weights, acc and disp depend on sigma alone).
 int mlp_tc_composite_group(int samples_per_ray);
+// shared-memory layout of the fused MLP kernel (byte offsets into its dynamic shared memory; the ring is at 0)
+struct MlpTcLayout {
+  int num_stages;                       // 16 KB weight-ring slots
+  uint32_t off_wg, off_bias, off_head, off_bars, off_carry, bytes;
+};
+int mlp_tc_layout(const NetProgram& prog, int max_smem, bool comp_on, bool training, int slot_cap, MlpTcLayout* out);
 int launch_mlp_tc(const NetDev& net, bool sigma_only, int n_passes, int act_scale_log2, const MlpInput& in, float* out,
                   int num_sms, int* d_err, cudaStream_t st, int64_t* launches, const MlpEmit* emit = nullptr,
                   const CompositeArgs* comp = nullptr);

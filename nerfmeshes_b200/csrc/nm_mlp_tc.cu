@@ -26,7 +26,9 @@
 //                   A warpgroup without a tile in a round gets no stages at all; that is only ever warpgroup 1, after
 //                   its own last tile (with tile groups of G tiles, for up to G final rounds).
 // The view-direction encoding reuses the encoding buffer: every layer that reads the xyz encoding precedes the one that
-// reads the directions (checked at launch).
+// reads the directions (checked at launch).  So does the fused compositor's staging, from the final layer's epilogue to the
+// next tile's encoding.  Inference reads the bias and head vectors through the read-only data cache, which leaves shared
+// memory to the weight ring (4 slots on an H100).
 //
 // Three template modes — 0 inference; 1 training forward, whose epilogue also emits the backward's operands (relu bit
 // masks, head activations, point-major bf16 hi/lo packs); 2 the whole data-gradient chain of the backward on a backward
@@ -55,7 +57,7 @@ constexpr uint32_t kKBlock = 2 * 8192;             // one K-block of a 64-point 
 constexpr uint32_t kActBytes = 4 * kKBlock;        // activation buffer of one warpgroup (K up to 256)
 constexpr uint32_t kWgBytes = kActBytes + kKBlock; // + its encoding buffer
 constexpr int kMaxStages = 8;
-constexpr uint32_t kCompBytes = 64 * 16 + 64 * 4 + 64 * 4 + 64;   // per warpgroup: staged q / products, keep / T, weights, carry slots
+constexpr uint32_t kCarryBytes = 64;             // per warpgroup: the compositor's two carry slots (its staging lives in the encoding buffer)
 
 struct TcParams {
   NetProgram net;   // by value: lives in the constant bank
@@ -70,7 +72,7 @@ struct TcParams {
   int num_stages;
   long long n_tiles;
   int* err;
-  uint32_t off_wg, off_bias, off_head, off_bars, off_comp;
+  uint32_t off_wg, off_bias, off_head, off_bars, off_carry;   // off_bias / off_head: modes 1 and 2 only
   int has_emit;     // training: the epilogue also writes the backward pass's operands (MlpEmit)
   MlpEmit emit;
   // mode 2: the data-gradient chain of the training backward (a KIND_LOAD / KIND_BWD program, W^T stages in bf16 hi/lo):
@@ -158,9 +160,14 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   const uint32_t bars = sbase + P.off_bars;
   const int NS = P.num_stages;
+  const int n_layers = P.net.n_layers;
+  // Bias and head vectors: inference reads them through the read-only data cache, which leaves its shared memory to the
+  // weight ring; the training modes, whose epilogues stream their emitted operands through L1, keep copies in shared memory.
   float* s_bias = reinterpret_cast<float*>(smem + P.off_bias);
   float* s_head = reinterpret_cast<float*>(smem + P.off_head);
-  const int n_layers = P.net.n_layers;
+  const float* vbias = MODE == 0 ? P.bias : s_bias;
+  const float* vhead = MODE == 0 ? P.head : s_head;
+  auto ldv = [](const float* p) -> float { if constexpr (MODE == 0) return __ldg(p); else return *p; };
 
   // ---------------------------------------------------------------- one-time setup
   if (threadIdx.x == 0) {
@@ -172,8 +179,10 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
     }
     ptx::fence_mbar_init();
   }
-  for (int i = threadIdx.x; i < P.net.n_bias; i += kThreads) s_bias[i] = (MODE == 2) ? 0.f : P.bias[i];
-  for (int i = threadIdx.x; i < P.net.n_head; i += kThreads) s_head[i] = P.head[i];
+  if (MODE != 0) {
+    for (int i = threadIdx.x; i < P.net.n_bias; i += kThreads) s_bias[i] = (MODE == 2) ? 0.f : P.bias[i];
+    for (int i = threadIdx.x; i < P.net.n_head; i += kThreads) s_head[i] = P.head[i];
+  }
   __syncthreads();
 
   // i-th tile of worker v (two workers per CTA, one per consumer warpgroup): groups of `tile_group` consecutive tiles are
@@ -278,15 +287,17 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
   // weight, mask, the four products;  D  one lane per (segment, accumulator) runs the five ordered sums.  The ray cut by
   // the tile's upper edge leaves T and its partial sums in a carry slot for the next tile (tiles of a group are
   // consecutive for this warpgroup and groups start on ray boundaries).
-  uint8_t* comp_s = smem + P.off_comp + (uint32_t)wg * kCompBytes;
+  // The staging arrays live in the encoding buffer, dead from the final layer's MMAs to the next tile's encoding; the carry
+  // slots, which outlive the tile, have their own.
+  float* carry = reinterpret_cast<float*>(smem + P.off_carry + (uint32_t)wg * kCarryBytes);
   auto composite_tile = [&](uint32_t itp, long long tp) {
     const CompositeArgs& A = P.comp;
     const int r = t;
-    float4* stage = reinterpret_cast<float4*>(comp_s);                      // q per sample, later (w r, w g, w b, w t)
-    float* keepT = reinterpret_cast<float*>(comp_s + 64 * 16);              // keep per sample, later T
+    float4* stage = reinterpret_cast<float4*>(pe);                          // q per sample, later (w r, w g, w b, w t)
+    float* keepT = reinterpret_cast<float*>(pe + 64 * 16);                  // keep per sample, later T
     float* wv = keepT + 64;                                                 // weight per sample
-    const float* carry_in = wv + 64 + ((itp & 1) ^ 1) * 8;                  // written by the previous tile
-    float* carry_out = wv + 64 + (itp & 1) * 8;
+    const float* carry_in = carry + ((itp & 1) ^ 1) * 8;                    // written by the previous tile
+    float* carry_out = carry + (itp & 1) * 8;
     const long long p0 = tp * kTileM, p1 = min(p0 + (long long)kTileM, P.in.M);
     const int S = A.S;
     const long long ray_first = p0 / S;
@@ -495,6 +506,10 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
 #pragma unroll
           for (int j8 = 0; j8 < 8; ++j8) {
             const int col = nc * 64 + j8 * 8 + cq;
+            // bias_off is a multiple of 64 (layer widths are): an aligned pair
+            float2 bias2 = make_float2(0.f, 0.f);
+            if constexpr (MODE == 0) bias2 = __ldg(reinterpret_cast<const float2*>(vbias + L.bias_off + col));
+            else if constexpr (MODE == 1) bias2 = *reinterpret_cast<const float2*>(vbias + L.bias_off + col);
             float x[2][2];
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
@@ -510,14 +525,14 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
 #pragma unroll
                 for (int u = 0; u < 2; ++u) {
                   float y = acc[nc * 32 + j8 * 4 + 2 * e + u] * so;
-                  if (L.aux2) y = fmaf(dsg[e], s_head[L.head_off + col + u], y);
+                  if (L.aux2) y = fmaf(dsg[e], ldv(vhead + L.head_off + col + u), y);
                   const uint32_t w = valid ? mk_in[e][j8 >> 2] : 0u;
                   x[e][u] = ((w >> ((col + u) & 31)) & 1u) ? y : 0.f;
                 }
               } else {
 #pragma unroll
                 for (int u = 0; u < 2; ++u) {
-                  float y = fmaf(acc[nc * 32 + j8 * 4 + 2 * e + u], so, s_bias[L.bias_off + col + u]);
+                  float y = fmaf(acc[nc * 32 + j8 * 4 + 2 * e + u], so, u ? bias2.y : bias2.x);
                   if (L.relu) y = fmaxf(y, 0.f);
                   x[e][u] = y;
                 }
@@ -526,11 +541,12 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
 #pragma unroll
             for (int hh = 0; hh < 4; ++hh) {
               if (hh >= heads_c) break;
-              const float* w = s_head + L.head_off + hh * L.n_out + col;
+              const float* w = vhead + L.head_off + hh * L.n_out + col;
+              const float w0 = ldv(w), w1 = ldv(w + 1);
 #pragma unroll
               for (int e = 0; e < 2; ++e) {
-                part[e][hh] = fmaf(w[0], x[e][0], part[e][hh]);
-                part[e][hh] = fmaf(w[1], x[e][1], part[e][hh]);
+                part[e][hh] = fmaf(w0, x[e][0], part[e][hh]);
+                part[e][hh] = fmaf(w1, x[e][1], part[e][hh]);
               }
             }
 #pragma unroll
@@ -610,18 +626,23 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
             part[e][hh] += __shfl_xor_sync(0xffffffffu, part[e][hh], 1);
             part[e][hh] += __shfl_xor_sync(0xffffffffu, part[e][hh], 2);
           }
-        const float* hb = s_head + L.head_off + heads * L.n_out;
+        const float* hb = vhead + L.head_off + heads * L.n_out;
+        // the compositor stages the final layer's outputs in the encoding buffer: every warp's wgmmas are done reading it
+        if (MODE == 0 && P.comp_on && L.is_final) ptx::named_bar_sync(bar_id, 128);
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const long long m = e ? m1 : m0;
           const bool valid = e ? val1 : val0;
           if (L.kind == KIND_SIGMA) {
-            sigma_val[e] = part[e][0] + hb[0];
-            if (L.is_final && (lane & 3) == 0 && valid && P.out) P.out[m] = sigma_val[e];   // sigma-only program
+            sigma_val[e] = part[e][0] + ldv(hb);
+            if (L.is_final && (lane & 3) == 0) {      // sigma-only program
+              if (MODE == 0 && P.comp_on) reinterpret_cast<float4*>(pe)[r0 + 8 * e] = make_float4(0.f, 0.f, 0.f, sigma_val[e]);
+              else if (valid && P.out) P.out[m] = sigma_val[e];
+            }
           } else if ((lane & 3) == 0 && (P.comp_on || (valid && P.out))) {
             float o[4];
 #pragma unroll
-            for (int hh = 0; hh < 4; ++hh) o[hh] = (hh < heads) ? part[e][hh] + hb[hh] : 0.f;
+            for (int hh = 0; hh < 4; ++hh) o[hh] = (hh < heads) ? part[e][hh] + ldv(hb + hh) : 0.f;
             const float sg = (L.kind == KIND_RGB) ? sigma_val[e] : o[3];
             if (P.out_sigma_only) {
               P.out[m] = sg;
@@ -631,7 +652,7 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
               res.y = 1.f / (1.f + expf(-o[1]));
               res.z = 1.f / (1.f + expf(-o[2]));
               res.w = sg;
-              if (MODE == 0 && P.comp_on) reinterpret_cast<float4*>(comp_s)[r0 + 8 * e] = res;
+              if (MODE == 0 && P.comp_on) reinterpret_cast<float4*>(pe)[r0 + 8 * e] = res;
               else reinterpret_cast<float4*>(P.out)[m] = res;
             }
           }
@@ -652,6 +673,43 @@ __global__ void __launch_bounds__(kThreads, 1) mlp_tc_kernel(const __grid_consta
 
 }  // namespace
 
+// The kernel's shared-memory layout for program `hp`, a dynamic shared-memory limit of `max_smem` bytes, the fused
+// compositor on or off and the mode (training: 1 and 2, which keep the bias and head vectors in shared memory): as many
+// 16 KB ring slots as fit after the two warpgroups' activation and encoding buffers, the vectors, the barriers and the
+// compositor's carry slots, at most kMaxStages and at most `slot_cap` (<= 0: no cap).  Pure host logic, so that the CPU
+// tests check the layout the kernel launches with.
+int mlp_tc_layout(const NetProgram& hp, int max_smem, bool comp_on, bool training, int slot_cap, MlpTcLayout* out) {
+  auto align_up = [](uint32_t x, uint32_t a) { return (x + a - 1) / a * a; };
+  const uint32_t vb = training ? align_up(hp.n_bias * 4, 16) : 0u, vh = training ? align_up((hp.n_head > 0 ? hp.n_head : 4) * 4, 16) : 0u;
+  const uint32_t fixed = 2 * kWgBytes + vb + vh + kBarBytes + (comp_on ? 2 * kCarryBytes : 0u);
+  int ns = ((int)max_smem - (int)fixed) / (int)kStageBytes;
+  NM_CHECK(ns >= 2, "network too large for the shared-memory budget (%u B fixed, %d B available)", fixed, max_smem);
+  if (ns > kMaxStages) ns = kMaxStages;
+  if (slot_cap > 0 && ns > slot_cap) ns = slot_cap < 2 ? 2 : slot_cap;
+  for (int i = 0; i < hp.n_layers; ++i)
+    NM_CHECK(hp.layers[i].kind == KIND_LOAD || hp.layers[i].n_out == 64 || hp.layers[i].n_out == 128 || hp.layers[i].n_out == 256,
+             "layer %d: output width %d not 64, 128 or 256", i, hp.layers[i].n_out);
+  MlpTcLayout l{};
+  l.num_stages = ns;
+  uint32_t off = (uint32_t)ns * kStageBytes;
+  l.off_wg = off; off += 2 * kWgBytes;
+  l.off_bias = off; off += vb;
+  l.off_head = off; off += vh;
+  l.off_bars = off; off += kBarBytes;
+  l.off_carry = off; off += comp_on ? 2 * kCarryBytes : 0u;
+  l.bytes = off;
+  NM_CHECK((int)off <= max_smem, "shared-memory layout overflow");
+  *out = l;
+  return 0;
+}
+
+// NM_MLP_RING_SLOTS=n (A/B and tests): at most n ring slots (n >= 2; it can only lower the depth the layout allows).  Read
+// per launch, so a test can flip it between calls.
+static int ring_slot_cap() {
+  const char* e = getenv("NM_MLP_RING_SLOTS");
+  return e ? atoi(e) : 0;
+}
+
 // shared-memory layout + launch of a prepared parameter block
 static int launch_prepared(TcParams& P, int num_sms, cudaStream_t st, int64_t* launches) {
   const NetProgram& hp = P.net;
@@ -662,29 +720,17 @@ static int launch_prepared(TcParams& P, int num_sms, cudaStream_t st, int64_t* l
       if (hp.layers[i].pe_src == SRC_PE_DIR) dir_seen = true;
     }
   }
-  auto align_up = [](uint32_t x, uint32_t a) { return (x + a - 1) / a * a; };
   int dev = 0, max_smem = 0;
   NM_CUDA(cudaGetDevice(&dev));
   NM_CUDA(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-  const uint32_t fixed = 2 * kWgBytes + align_up(hp.n_bias * 4, 16) + align_up((hp.n_head > 0 ? hp.n_head : 4) * 4, 16) +
-                         kBarBytes + (P.comp_on ? 2 * kCompBytes : 0u);
-  int ns = ((int)max_smem - (int)fixed) / kStageBytes;
-  if (ns > kMaxStages) ns = kMaxStages;
-  NM_CHECK(ns >= 2, "network too large for the shared-memory budget (%u B fixed, %d B available)", fixed, max_smem);
-  P.num_stages = ns;
-  for (int i = 0; i < hp.n_layers; ++i)
-    NM_CHECK(hp.layers[i].kind == KIND_LOAD || hp.layers[i].n_out == 64 || hp.layers[i].n_out == 128 || hp.layers[i].n_out == 256,
-             "layer %d: output width %d not 64, 128 or 256", i, hp.layers[i].n_out);
-  uint32_t off = (uint32_t)ns * kStageBytes;
-  P.off_wg = off; off += 2 * kWgBytes;
-  P.off_bias = off; off += align_up(hp.n_bias * 4, 16);
-  P.off_head = off; off += align_up((hp.n_head > 0 ? hp.n_head : 4) * 4, 16);
-  P.off_bars = off; off += kBarBytes;
-  P.off_comp = off; off += P.comp_on ? 2 * kCompBytes : 0u;
-  if (P.tile_group < 1) P.tile_group = 1;
-  NM_CHECK((int)off <= max_smem, "shared-memory layout overflow");
-
   const int mode = P.mode == 2 ? 2 : (P.has_emit ? 1 : 0);
+  MlpTcLayout lay;
+  if (int e = mlp_tc_layout(hp, max_smem, P.comp_on != 0, mode != 0, ring_slot_cap(), &lay)) return e;
+  P.num_stages = lay.num_stages;
+  P.off_wg = lay.off_wg; P.off_bias = lay.off_bias; P.off_head = lay.off_head; P.off_bars = lay.off_bars; P.off_carry = lay.off_carry;
+  const uint32_t off = lay.bytes;
+  if (P.tile_group < 1) P.tile_group = 1;
+
   auto kern = mode == 2 ? mlp_tc_kernel<2> : (mode == 1 ? mlp_tc_kernel<1> : mlp_tc_kernel<0>);
   static thread_local unsigned configured_devs[3] = {0, 0, 0};   // per-device opt-in to the large dynamic shared memory window
   if (!(configured_devs[mode] & (1u << (dev & 31)))) {
@@ -733,10 +779,12 @@ int launch_mlp_tc(const NetDev& net, bool sigma_only, int n_passes, int act_scal
   }
   P.tile_group = 1;
   if (comp) {
-    NM_CHECK(!emit && !sigma_only && in.mode == IN_RAYS && comp->S == in.S && comp->R * (long long)comp->S == in.M && comp->t == in.t,
+    NM_CHECK(!emit && in.mode == IN_RAYS && comp->S == in.S && comp->R * (long long)comp->S == in.M && comp->t == in.t,
              "fused compositor: needs the ray front end on the compositor's own samples");
     P.tile_group = mlp_tc_composite_group(comp->S);
     NM_CHECK(P.tile_group > 0, "fused compositor: %d samples per ray not supported", comp->S);
+    NM_CHECK(!sigma_only || (!comp->rgb && hp.layers[hp.n_layers - 1].kind == KIND_SIGMA),
+             "fused compositor: the sigma-only program must end in a sigma layer and write no colour map");
     P.comp_on = 1; P.comp = *comp; P.out = nullptr;
   }
   return launch_prepared(P, num_sms, st, launches);

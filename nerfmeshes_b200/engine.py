@@ -876,6 +876,10 @@ class Engine:
     def launch_count(self) -> int:
         return int(self.lib.nm_launch_count(self._h))
 
+    def sigma_only_points(self) -> int:
+        """Points sent through a network's sigma-only program since the handle was made."""
+        return int(self.lib.nm_sigma_only_points(self._h))
+
     def set_timing(self, on: bool):
         L.check(self.lib.nm_set_timing(self._h, int(on)))
 
